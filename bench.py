@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- RenderNet forward rendering throughput on B200 (contract in the task statement).
+"""bench.py -- RenderNet forward rendering throughput on H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--config 2|4|5] [--precision exact|fast] [--gather nccl|peer|none]
+                  [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W
   python bench.py --impl reference ...      # CPU restatement of the reference's TF-1 graph, host cores
@@ -17,9 +18,11 @@ all-gathered on a side stream (north_star: "NCCL all-gather only for the output 
 parity bar on ANY weights (tests/test_gpu_exact.py::test_full_size_stress_weights_...); "fast" = fp16 operands, 1 product:
 meets the bar for the reference's initialisers (the weights this bench uses) but not for high-gain weights.  The other
 mode is timed too and reported under "other_precision".  Prints ONE JSON line (rank 0).
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what its last timed step computed (the images a caller of the engine
+receives) as DIR/<name>.npy in float32; inputs and weights are seeded, so two builds can be compared output for output.
 """
 import argparse
-import hashlib
 import json
 import os
 import subprocess
@@ -67,7 +70,8 @@ def measured_peaks():
             d = json.load(f)
         return dict(hbm=d["hbm_gbs"], burst=d["bf16_tflops"], sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured")
-    return dict(hbm=6650.0, burst=1590.0, sustained=1400.0, source="fallback")  # B200_PROFILING.md fallback
+    # H100 SXM data sheet (dense BF16, HBM3) -- not measured; a power-limited card reaches less
+    return dict(hbm=3350.0, burst=989.0, sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -185,11 +189,6 @@ def run_reference(args, rank, world):
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
-def _file_sha(path):
-    with open(path, "rb") as f:
-        return hashlib.sha256(f.read()).hexdigest()[:16]
-
-
 def kernel_roofline(torch, ops, dev, B, cin, cout, k, precision, peaks, label):
     """Times the dominant kernel alone (CUDA events on its launch stream, 20 back-to-back launches, >= 100 MB of inputs so
     nothing survives in L2 between launches) and relates the ALGORITHMIC FLOPs of one launch to the measured burst peak."""
@@ -219,6 +218,22 @@ def kernel_roofline(torch, ops, dev, B, cin, cout, k, precision, peaks, label):
             "note": ("exact mode issues 3 fp16 tensor-core products per algorithmic MAC (x_hi.w_hi + x_lo.w_hi + x_hi.w_lo): "
                      "`frac` relates ALGORITHMIC flops to the bf16 peak, `tensor_issue_frac` the issued ones"
                      if precision == "exact" else "one fp16 tensor-core product per algorithmic MAC")}
+
+
+DUMP_BUDGET = 64 * 10**6   # bytes of .npy files --dump-outputs may write (64 MB)
+
+
+def dump_outputs(dirname, arrays):
+    """arrays: name -> device tensor.  Each becomes DIR/<name>.npy (float32).  When the arrays together exceed DUMP_BUDGET, each
+    is represented by a fixed seeded sample of its leading-axis entries (same indices on every run, kept in order)."""
+    os.makedirs(dirname, exist_ok=True)
+    per = (DUMP_BUDGET - 4096 * len(arrays)) // len(arrays)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        n = min(len(a), max(1, per // a[0].nbytes))
+        if n < len(a):
+            a = a[np.sort(np.random.default_rng(0).choice(len(a), n, replace=False))]
+        np.save(os.path.join(dirname, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def run_ours(args, rank, world, local_rank):
@@ -281,8 +296,8 @@ def run_ours(args, rank, world, local_rank):
         tex = synthetic_texture(B, rank) if cfg == 4 else None
         units_per_step_global = world * B
 
-    def measure(precision, with_e2e, gather_kind):
-        """-> dict(ms_step, per_rank, value, e2e..., launches) for one precision."""
+    def measure(precision, with_e2e, gather_kind, keep_outputs=False):
+        """-> dict(ms_step, per_rank, value, e2e..., launches[, outputs]) for one precision."""
         eng = build(precision, B)
         sh = ShardedRenderEngine(eng, gather_kind) if cfg != 5 else None
         if sh is not None and sh.peer is not None and not sh.verify_peer_against_nccl():
@@ -342,6 +357,13 @@ def run_ours(args, rank, world, local_rank):
                 eng.result(eng.submitted - 1)
         torch.cuda.synchronize()
         ms_total, per = timed(args.steps, False)
+        outputs = None
+        if keep_outputs:                              # what the last timed step computed, before anything else runs
+            if cfg == 5:
+                outputs = {"frames": out_frames.clone()}
+            else:
+                names = ["albedo", "normal"] if cfg == 4 else ["image", "image_u8"]
+                outputs = {n: t.clone() for n, t in zip(names, eng.outputs)}
         phases = None
         if args.phases and sh is not None:            # where does a step's time go: graph replay vs the gather on the compute stream
             sh.timing = []
@@ -360,7 +382,7 @@ def run_ours(args, rank, world, local_rank):
              "value": units_per_step_global * args.steps / (ms_total / 1e3),
              "launches": eng.launches_per_step * (nchunk if cfg == 5 else 1),
              "gather": sh.kind_note if sh is not None else ("NCCL all-gather of the frames" if world > 1 else "single GPU"),
-             "cuda_graph": eng.graph is not None}
+             "cuda_graph": eng.graph is not None, "outputs": outputs}
         if with_e2e:
             ms_e2e, per_e = timed(args.steps, True)
             r["e2e_value"] = units_per_step_global * args.steps / (ms_e2e / 1e3)
@@ -376,7 +398,9 @@ def run_ours(args, rank, world, local_rank):
         sampler.start()
     main_prec = args.precision
     other_prec = "fast" if main_prec == "exact" else "exact"
-    M = measure(main_prec, True, args.gather)
+    M = measure(main_prec, True, args.gather, keep_outputs=args.dump_outputs is not None and rank == 0)
+    if M["outputs"] is not None:
+        dump_outputs(args.dump_outputs, M.pop("outputs"))
     clocks = sampler.stop(set(range(world))) if rank == 0 else None
     O = None if args.no_other_precision else measure(other_prec, False, "none")
 
@@ -391,21 +415,9 @@ def run_ours(args, rank, world, local_rank):
         klabel = "igemm_kernel 3x3 conv 512->512 @64x64, B=24 (Texture net res2 trunk: 21 of its launches, 75 % of its MACs)"
     else:
         kshape = dict(cin=1024, cout=1024, k=3)
-        klabel = "igemm_kernel<256,cta_group::2> 3x3 conv 1024->1024 @64x64, B=24 (Shader res2 trunk: 21 of the 65 launches, 77 % of the MACs)"
+        klabel = "igemm_kernel<256> 3x3 conv 1024->1024 @64x64, B=24 (Shader res2 trunk: 21 of its launches, 77 % of the MACs)"
     roof = kernel_roofline(torch, ops, dev, 24, precision=main_prec, peaks=peaks, label=klabel + f" [{main_prec}]", **kshape)
     roof_other = kernel_roofline(torch, ops, dev, 24, precision=other_prec, peaks=peaks, label=klabel + f" [{other_prec}]", **kshape)
-    tfile = os.path.join(ROOT, "profiles", "top_kernel_traffic.json")
-    roof["traffic"] = None
-    if os.path.exists(tfile):
-        with open(tfile) as f:
-            tj = json.load(f)
-        entry = tj.get(main_prec, tj if main_prec == "fast" else {})
-        roof["traffic"] = entry.get("dram_bytes_per_launch")
-        roof["traffic_source"] = {"file": "profiles/top_kernel_traffic.json", "sha256_16": _file_sha(tfile),
-                                  "ncu_capture": entry.get("source"),
-                                  "note": "dram__bytes_read.sum + dram__bytes_write.sum of this kernel from an `ncu --set full` capture "
-                                          "(not measurable inside a timed run); algorithmic bytes per launch "
-                                          f"{entry.get('algorithmic_bytes_per_launch')}"}
     per_flop = FLOP_PER_RENDER[model]
     step_tflops = M["value"] * per_flop / 1e12 / world
     roof["whole_step_tflops"] = step_tflops
@@ -446,7 +458,7 @@ def run_ours(args, rank, world, local_rank):
                        "weights": "reference initialisers (xavier-uniform, seeded); random-init, no checkpoint exists offline",
                        "precision": main_prec, "precision_note": prec_note[main_prec],
                        "cuda_graph": M["cuda_graph"],
-                       "l2": "no explicit flush: every layer streams 200-1600 MB of activations (> 126 MB L2) per step"},
+                       "l2": "no explicit flush: every layer streams 200-1600 MB of activations (> 50 MB L2) per step"},
             "per_rank_ms": M["per_rank_ms"],
             "phases": M["phases"],
             "clocks": clocks,
@@ -491,6 +503,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-other-precision", action="store_true")
     ap.add_argument("--no-b8", action="store_true", help="reference arm: skip the extra B=8 CPU sample")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write the last timed step's output images as DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

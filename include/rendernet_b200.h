@@ -1,4 +1,4 @@
-/* rendernet_b200.h -- C ABI of librendernet_b200.so: the B200 (sm_100a) kernels behind RenderNet's
+/* rendernet_b200.h -- C ABI of librendernet_b200.so: the H100 (sm_90a) kernels behind RenderNet's
  * forward-rendering hot path.
  *
  * The reference (thunguyenphuoc/RenderNet) is pure Python over TensorFlow-1 and has NO FFI of its own;
@@ -77,7 +77,7 @@ int rn_cast_16_to_f32(const void* src, float* dst, long long n, int fmt, void* s
 int rn_bias_act_16(const void* x, const float* bias, const float* alpha, int act, const void* residual,
                    void* out16, float* out32, long long n, int C, int fmt, void* stream);
 
-/* ---- tensor-core implicit-GEMM convolution (tcgen05 + TMA) ----------------------------------------
+/* ---- tensor-core implicit-GEMM convolution (wgmma + TMA) ------------------------------------------
  * out[b,y,x,z,n] = act( bias[n] + sum_t sum_ci  x[b, y+dy_t, x+dx_t, z+dz_t, ci] * w_packed[t][n][ci] ) + residual
  * with zero outside the input (TF SAME padding is expressed through the tap offsets).
  * The output element offset is o_base + b*o_b + y*o_y + x*o_x + z*o_z + n, which lets one call write a
@@ -120,10 +120,10 @@ typedef struct rn_conv_desc {
   /* geometry of the depth-folded conv3d behind a banded filter (channels per depth of x / of the output, z stride; 0 = not
    * given): lets the launcher issue the edge K blocks of the band, which touch only half of the N tile's output depths,
    * as N = 64 MMAs instead of multiplying structural zeros.  w_packed must then come from rn_pack_conv3d_banded (K blocks in
-   * processing order, a "single-CTA" and a "CTA-pair" arrangement of the half tiles back to back). */
+   * processing order, the rows a half tile needs first). */
   int band_cin, band_cout, band_sz;
   int cluster;              /* thread-block-cluster size for the weight-tile TMA multicast: 0 auto, 1, 2 or 4 */
-  int cta_group;            /* 0 auto, 1 = single-CTA MMA, 2 = paired tcgen05.mma.cta_group::2 (M = 256) */
+  int cta_group;            /* 0 auto or 1 (single-CTA MMA); anything else is rejected: sm_90 has no paired MMA */
   /* y-halo sharing (2-D only): taps ordered tap = ky*nx + kx with dy(ky) = dy(0) + ky; the ny taps of a filter column
    * then share one activation load of BH+ny-1 image rows.  0/1 = off.  tile_w: M-tile width override (0 = 16).
    * msub: M sub-tiles per CTA tile -- 2 = two 128-row accumulators share every weight stage (Cout tile <= 128; halves
@@ -135,24 +135,24 @@ typedef struct rn_conv_desc {
   /* fmt == RN_FMT_F16X2: element offsets of the LO plane of x, of w_packed and of out16 / a 16-bit residual (multiples
    * of 8).  The reference-shaped wrappers below derive them from the tensor shapes ([2][numel] pairs). */
   long long x_plane, w_plane, o_plane;
-  /* per-call overrides of the launch heuristics, 0 = library default: epilogue warp groups (1 or 2); residual register
-   * prefetch / TMA-store epilogue (1 = on, -1 = off) */
+  /* accepted and ignored (kept so that the struct layout stays stable): the sm_90 kernel has a single epilogue form, two
+   * consumer warpgroups storing their own rows directly */
   int epi_groups, res_prefetch, tma_store;
   const rn_phong* phong;    /* NULL, or the fused Phong epilogue (act = RN_ACT_SIGMOID, N = F pixels x 3 channels <= 16) */
 } rn_conv_desc;
 int rn_conv_igemm(const rn_conv_desc* d, void* stream);
 /* Per-call overrides of the launch heuristics for the reference-shaped wrappers below (their last argument before
- * `stream`; NULL = library defaults).  0 = default for every field; cluster 1/2/4; cta_group 1/2; kps = k-groups per
- * pipeline stage; msub 1/2 M sub-tiles; epilogue_groups 1/2; res_prefetch / tma_store / yhalo: 1 = on, -1 = off.
+ * `stream`; NULL = library defaults).  0 = default for every field; cluster 1/2/4; cta_group 1; kps = k-groups per
+ * pipeline stage; msub 1/2 M sub-tiles; yhalo: 1 = on, -1 = off; epilogue_groups / res_prefetch / tma_store are ignored.
  * Every combination computes bit-identical results (tests/test_gpu_kernels.py::*_bit_identical). */
 typedef struct rn_tuning {
   int cluster, cta_group, kps, msub, epilogue_groups, res_prefetch, tma_store, yhalo;
 } rn_tuning;
 /* The launch plan rn_conv_igemm would use for `d`, without touching the device (works on a host without a GPU; the SM
- * count then defaults to 148).  Pointers in `d` are only tested for null / 16-byte alignment.  out[0..n_out) receives
+ * count then defaults to 132).  Pointers in `d` are only tested for null / 16-byte alignment.  out[0..n_out) receives
  * {N tile, cluster size, cta_group, M sub-tiles, epilogue warp groups, ny (halo sharing), tile W, tile H, tile D,
- *  k-groups per stage, stages, dynamic shared memory bytes, grid, tiles, epilogue mode (0 direct, 1 TMA store, 2 TMA
- *  scatter), swizzle row bytes}; n_out <= 16.  Same status codes as rn_conv_igemm. */
+ *  k-groups per stage, stages, dynamic shared memory bytes, grid, tiles, epilogue mode (always 0: direct stores),
+ *  swizzle row bytes}; n_out <= 16.  Same status codes as rn_conv_igemm. */
 int rn_conv_plan(const rn_conv_desc* d, int* out, int n_out);
 
 /* Reference-shaped wrappers over rn_conv_igemm (stride 1, TF SAME), 16-bit in/out:
@@ -168,7 +168,7 @@ int rn_conv3d_same(const void* x, const void* w_packed, const float* bias, const
  * depth-folded 2-D convolution: the D axis is part of the GEMM's N (128 = (128/Cout) output depths x Cout) and K
  * ((128/Cout + 2) input depths x Cin, padded to 64-element blocks), so TMA moves full 128-byte rows and each
  * activation byte is fetched from L2 9x instead of 27x.  w_banded from rn_pack_conv3d_banded
- * (2 arrangements x [9][kblocks][128][64] 16-bit -- one for single-CTA, one for CTA-pair launches --, bytes =
+ * ([9][kblocks][128][64] 16-bit, bytes =
  * rn_conv3d_banded_bytes per plane; RN_FMT_F16X2: twice that, LO plane after the HI plane); bias/alpha are per Cout (length Cout) and are
  * expanded over depth internally via bias_full/alpha_full scratch [D*Cout] fp32 supplied by the caller
  * (fill them with rn_expand_channels).  x: [B,H,W,D,Cin]; residual, out: [B,H,W,ceil(D/sz),Cout], 16-bit.
@@ -290,7 +290,7 @@ int rn_resample_backward_f32(const float* vox, const float* minv, const float* g
 /* ---- backward pass, stage 2: weight gradients (training step, RenderNet_Shader.py:159-167) -------------------------------
  * dW of a stride-1 SAME conv2d (slim.conv2d / layer_util.conv2d, tools/layer_util.py:147-184) on the tensor cores:
  *   dw[ky][kx][ci][co] = sum_{b,y,x} x[b, y+ky-pb, x+kx-pb, ci] * g[b, y, x, co]        (TF filter layout, fp32)
- * x 16-bit [B,H,W,Cin] (the layer's input), g 16-bit [B,H,W,Cout] (dL/d conv output); both are read as MN-major tcgen05
+ * x 16-bit [B,H,W,Cin] (the layer's input), g 16-bit [B,H,W,Cout] (dL/d conv output); both are read as MN-major wgmma
  * operands directly from their channel-last layout (K = pixels).  Cin % 128 == 0, Cout % 128 == 0, kh*kw <= 16,
  * fmt RN_FMT_F16 or RN_FMT_F16X2.  dw is overwritten. */
 int rn_conv2d_weight_grad(const void* x, const void* g, float* dw, int B, int H, int W, int Cin, int Cout, int kh, int kw,

@@ -10,12 +10,12 @@ extension.
 Pinning status: the reference ships no tests, no golden tensors and no weights, and
 TensorFlow-1 cannot be installed here, so this restatement is pinned against
 fixtures produced by executing the *reference's own Python source* (from
-/root/reference) over a NumPy shim of the TF-1 primitives it calls
+the reference source tree) over a NumPy shim of the TF-1 primitives it calls
 (``oracle/tf1_shim.py`` + ``tests/golden/make_golden.py`` -> ``tests/golden/*.npz``).
 TF's own C++ kernels remain unpinned ("parity pinned to reference Python over a TF
 shim; TF kernels unpinned").
 
-All file:line citations are into /root/reference.
+All file:line citations are into the reference source tree.
 """
 from __future__ import annotations
 

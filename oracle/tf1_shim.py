@@ -1,6 +1,6 @@
 """A tiny eager NumPy stand-in for the TensorFlow-1 primitives the reference's hot path
 calls.  TEST INFRASTRUCTURE ONLY (used by tests/golden/make_golden.py to execute the
-reference's *own* Python source from /root/reference and freeze its outputs).
+reference's *own* Python source from the reference source tree and freeze its outputs).
 
 TensorFlow 1.x cannot be installed in this environment (no network, Python 3.12).
 The reference's hot path is ordinary Python that composes ~50 TF primitives

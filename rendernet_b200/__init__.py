@@ -1,4 +1,4 @@
-"""rendernet_b200 -- B200-native (sm_100a) implementation of RenderNet's forward rendering hot path.
+"""rendernet_b200 -- H100-native (sm_90a) implementation of RenderNet's forward rendering hot path.
 
 Host side mirrors the reference's Python call surface (tools/layer_util.py, tools/resampling_voxel_grid.py,
 tools/model_util.py, tools/Phong_shading.py, tools/binvox_rw.py, RenderNet_Shader.py, RenderNet_demo.py);

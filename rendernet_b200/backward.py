@@ -10,7 +10,7 @@ realised layer appends (kind, input, filter, activation, residual, output).  `ba
 
   * activations: PReLU / sigmoid derivatives from the STORED post-activation tensors (rn_prelu_backward_16, rn_sigmoid_backward);
   * data gradient of a stride-1 SAME convolution = a stride-1 convolution of the output gradient with the spatially mirrored,
-    channel-transposed filter -> the SAME tcgen05 implicit-GEMM kernel as the forward pass (rn_conv_igemm) with a mirrored
+    channel-transposed filter -> the SAME wgmma implicit-GEMM kernel as the forward pass (rn_conv_igemm) with a mirrored
     tap list; 3^3 convs through the depth-folded (banded) form; the residual adds of the forward graph become the fused
     `residual` input of the gradient convolution (gradient accumulation at a fan-out costs no extra pass);
   * data gradient of a stride-1 transposed conv = a forward SAME conv with the very same filter array;
@@ -204,7 +204,7 @@ class ShaderInputGradients:
                  tensor_core_wgrad: bool = True):
         """dimg: dL/dimg [B,512,512,3|1] (NumPy or tensor).  Returns (dL/dvoxels [B,S,S,S,1] or None, dL/dview_params [B,3] or None).
         want_weight_grads: also fills `self.weight_grads` {variable name: fp32 device tensor in the variable's TF layout} for EVERY
-        variable the forward pass used -- filters (tcgen05 weight-gradient kernel for the wide stride-1 2-D layers and, depth-folded,
+        variable the forward pass used -- filters (wgmma weight-gradient kernel for the wide stride-1 2-D layers and, depth-folded,
         the 3^3 layers; the strided-correlation kernel rn_conv_weight_grad_direct for the thin / strided / transposed ones), biases
         and PReLU slopes (pre-activation recomputed: alpha starts at 0, tools/layer_util.py:38).  tensor_core_wgrad=False sends
         every filter through the direct kernel (cross-check)."""

@@ -45,7 +45,7 @@ __device__ __forceinline__ float ld16(const uint16_t* __restrict__ p, long long 
   }
   return v;
 }
-inline int grid_for(long long n, int block, int cap = 148 * 32) {
+inline int grid_for(long long n, int block, int cap = 132 * 32) {
   long long g = (n + block - 1) / block;
   return static_cast<int>(g < 1 ? 1 : (g > cap ? cap : g));
 }

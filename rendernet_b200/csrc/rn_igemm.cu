@@ -1,4 +1,4 @@
-// rn_igemm.cu -- implicit-GEMM convolution on 5th-gen tensor cores (tcgen05) for sm_100a.
+// rn_igemm.cu -- implicit-GEMM convolution on Hopper tensor cores (wgmma) for sm_90a.
 //
 // One kernel serves every dense contraction of the RenderNet forward path (reference call sites:
 // tools/layer_util.py:21 projection 1x1, :101-104 3x3 res blocks, :253 conv3d, :212 conv2d_transpose;
@@ -8,16 +8,15 @@
 //     128-row A tile is ONE tiled-TMA box {KB channels, BD, BW, BH} fetched at a shifted coordinate; TMA's
 //     out-of-bounds zero fill implements TF "SAME" padding (asymmetric pads are just different offsets).
 //   * B (weights) is pre-packed [tap][Cout][Cin] so a {KB, BN} box is a K-major operand tile.
-//   * Both land in shared memory in the 32/64/128-byte swizzled K-major layout that tcgen05.mma reads
-//     through shared-memory descriptors; accumulators live in TMEM (2 x BN fp32 columns, double-buffered
-//     so the epilogue of tile i overlaps the MMAs of tile i+1).
-//   * Warp roles: warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread MMA issuer,
-//     warps 2..5 = epilogue (tcgen05.ld -> bias/PReLU/residual/sigmoid -> 16B global stores).
+//   * Both land in shared memory in the 32/64/128-byte swizzled K-major layout that wgmma reads through
+//     shared-memory descriptors; fp32 accumulators live in the registers of two consumer warpgroups (64 rows each).
+//   * Warpgroup roles: warpgroup 0 = TMA producer, warpgroups 1-2 = wgmma issue + epilogue
+//     (bias/PReLU/residual/sigmoid -> 16B global stores).
 //   * Persistent: grid = #SMs, static round-robin tile schedule with N fastest so concurrently running
 //     CTAs share the same activation rows in L2.
 //
 // This file is the host side (argument validation, tile / pipeline sizing, TMA tensor maps); the kernel template lives
-// in rn_igemm_kernel.cuh and is instantiated in rn_igemm_inst_*.cu.
+// in rn_igemm_kernel.cuh and is instantiated in rn_igemm_inst.cu.
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
@@ -29,29 +28,25 @@
 
 namespace rn {
 
-// launch_ms<BN, CL, CG, MS, EG, SPLIT> is defined in rn_igemm_kernel.cuh and explicitly instantiated once per variant
+// launch_ms<BN, CL, MS, SPLIT, HALF> is defined in rn_igemm_kernel.cuh and explicitly instantiated once per variant
 // (rn_igemm_inst.cu x the Makefile's VARIANTS list); this table must list exactly those variants.
-template <int BN, int CL, int CG, int MS, int EG, bool SPLIT>
+template <int BN, int CL, int MS, bool SPLIT, bool HALF>
 cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t stream);
 
-static cudaError_t launch_variant(int BN, int CL, int CG, int MS, int EG, int SP, const IgemmParams& p, int grid, size_t smem,
+static cudaError_t launch_variant(int BN, int CL, int MS, int SP, int HF, const IgemmParams& p, int grid, size_t smem,
                                   cudaStream_t stream) {
-#define RN_V(bn, cl, cg, ms, eg, sp) \
-  if (BN == bn && CL == cl && CG == cg && MS == ms && EG == eg && SP == sp) return launch_ms<bn, cl, cg, ms, eg, (sp != 0)>(p, grid, smem, stream);
-  // one epilogue warp group
-  RN_V(256, 2, 2, 1, 1, 0) RN_V(256, 4, 1, 1, 1, 0) RN_V(256, 2, 1, 1, 1, 0) RN_V(256, 1, 1, 1, 1, 0)
-  RN_V(128, 2, 2, 1, 1, 0) RN_V(128, 4, 1, 1, 1, 0) RN_V(128, 2, 1, 1, 1, 0) RN_V(128, 1, 1, 1, 1, 0)
-  RN_V(128, 2, 2, 2, 1, 0) RN_V(128, 4, 1, 2, 1, 0) RN_V(128, 2, 1, 2, 1, 0) RN_V(128, 1, 1, 2, 1, 0)
-  RN_V(64, 1, 1, 1, 1, 0) RN_V(64, 1, 1, 2, 1, 0) RN_V(32, 1, 1, 1, 1, 0) RN_V(32, 1, 1, 2, 1, 0)
-  RN_V(16, 1, 1, 1, 1, 0) RN_V(16, 1, 1, 2, 1, 0)
-  // two epilogue warp groups
-  RN_V(256, 2, 2, 1, 2, 0) RN_V(128, 2, 2, 1, 2, 0) RN_V(128, 2, 2, 2, 2, 0) RN_V(128, 2, 1, 1, 2, 0) RN_V(128, 2, 1, 2, 2, 0)
-  RN_V(64, 1, 1, 2, 2, 0) RN_V(32, 1, 1, 2, 2, 0) RN_V(16, 1, 1, 2, 2, 0)
-  // operand-split "exact" mode (fmt 2): CTA pairs or single CTAs, always two epilogue groups
-  RN_V(256, 2, 2, 1, 2, 1) RN_V(256, 1, 1, 1, 2, 1)
-  RN_V(128, 2, 2, 1, 2, 1) RN_V(128, 2, 2, 2, 2, 1) RN_V(128, 1, 1, 1, 2, 1) RN_V(128, 1, 1, 2, 2, 1)
-  RN_V(64, 1, 1, 1, 2, 1) RN_V(64, 1, 1, 2, 2, 1) RN_V(32, 1, 1, 1, 2, 1) RN_V(32, 1, 1, 2, 2, 1)
-  RN_V(16, 1, 1, 1, 2, 1) RN_V(16, 1, 1, 2, 2, 1)
+#define RN_V(bn, cl, ms, sp, hf) \
+  if (BN == bn && CL == cl && MS == ms && SP == sp && HF == hf) \
+    return launch_ms<bn, cl, ms, (sp != 0), (hf != 0)>(p, grid, smem, stream);
+  RN_V(256, 1, 1, 0, 0) RN_V(256, 2, 1, 0, 0) RN_V(256, 4, 1, 0, 0)
+  RN_V(128, 1, 1, 0, 0) RN_V(128, 2, 1, 0, 0) RN_V(128, 4, 1, 0, 0) RN_V(128, 1, 2, 0, 0) RN_V(128, 2, 2, 0, 0) RN_V(128, 4, 2, 0, 0)
+  RN_V(64, 1, 1, 0, 0) RN_V(64, 1, 2, 0, 0) RN_V(32, 1, 1, 0, 0) RN_V(32, 1, 2, 0, 0) RN_V(16, 1, 1, 0, 0) RN_V(16, 1, 2, 0, 0)
+  // operand-split "exact" mode (fmt 2): single CTAs
+  RN_V(256, 1, 1, 1, 0) RN_V(128, 1, 1, 1, 0) RN_V(128, 1, 2, 1, 0) RN_V(64, 1, 1, 1, 0) RN_V(64, 1, 2, 1, 0)
+  RN_V(32, 1, 1, 1, 0) RN_V(32, 1, 2, 1, 0) RN_V(16, 1, 1, 1, 0) RN_V(16, 1, 2, 1, 0)
+  // banded filters (N tile 128) with half-tile K blocks
+  RN_V(128, 1, 1, 0, 1) RN_V(128, 2, 1, 0, 1) RN_V(128, 4, 1, 0, 1) RN_V(128, 1, 2, 0, 1) RN_V(128, 2, 2, 0, 1)
+  RN_V(128, 4, 2, 0, 1) RN_V(128, 1, 1, 1, 1) RN_V(128, 1, 2, 1, 1)
 #undef RN_V
   return cudaErrorInvalidDeviceFunction;   // plan_conv chose a variant that is not built
 }
@@ -77,7 +72,7 @@ static CUtensorMapSwizzle swizzle_of(int row_bytes) {
 std::atomic<long long> g_launch_count{0};   // kernels launched by this library (bench.py's gpu_launches)
 
 // Library defaults of the launch heuristics.  They can be overridden ONCE per process through the environment variable
-// RN_TUNE ("epi=1,msub=1,kps=4,cluster=4,cta_group=1,res_prefetch=0,tma_store=0,yhalo=0"; read at first use, immutable
+// RN_TUNE ("msub=1,kps=4,cluster=4,yhalo=0"; read at first use, immutable
 // afterwards -- a tuning / A-B aid, see scripts/ab_step.py) and per call through the 0-means-auto fields of rn_conv_desc.
 // There is no mutable global state.
 static Tuning parse_tuning() {
@@ -91,12 +86,8 @@ static Tuning parse_tuning() {
     if (v >= lo && v <= hi) *dst = v;
   };
   get("cluster", &t.cluster, 1, 4);
-  get("cta_group", &t.cta_group, 1, 2);
   get("kps", &t.kps, 0, 16);
   get("msub", &t.msub, 0, 2);
-  get("epi", &t.epi_groups, 1, 2);
-  get("res_prefetch", &t.res_prefetch, 0, 1);
-  get("tma_store", &t.tma_store, 0, 1);
   get("yhalo", &t.yhalo, 0, 1);
   get("tiled_tex_conv", &t.tiled_tex_conv, 0, 1);
   get("pdl", &t.pdl, 0, 1);
@@ -107,19 +98,20 @@ const Tuning& tuning() {
   return t;
 }
 
-// SM count of the CURRENT device (cached per device ordinal); 148 when no device is visible (rn_conv_plan on a CPU host)
+// SM count of the CURRENT device (cached per device ordinal); 132 (H100 SXM) when no device is visible (rn_conv_plan on a
+// CPU host)
 int num_sms() {
   static std::atomic<int> cache[64];
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
     cudaGetLastError();
-    return 148;
+    return 132;
   }
   int n = cache[dev].load(std::memory_order_relaxed);
   if (n == 0) {
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
       cudaGetLastError();
-      return 148;
+      return 132;
     }
     cache[dev].store(n, std::memory_order_relaxed);
   }
@@ -134,12 +126,12 @@ extern "C" long long rn_launch_count(void) { return rn::g_launch_count.load(std:
 
 namespace rn {
 struct ConvPlan {
-  int BN, CL, CG, EG, grid, sub, stg_bytes, PCh, KB, D;
+  int BN, CL, grid, sub, KB, D;
   size_t smem;
 };
 
-// Everything rn_conv_igemm decides before it touches the device: N tile, M tile box, halo sharing, M sub-tiles, cluster /
-// CTA-pair mode, epilogue groups, pipeline depth, shared-memory size, epilogue mode.  Pure host arithmetic on the
+// Everything rn_conv_igemm decides before it touches the device: N tile, M tile box, halo sharing, M sub-tiles, cluster
+// size, pipeline depth, shared-memory size.  Pure host arithmetic on the
 // descriptor (pointers are only tested for null / alignment), so rn_conv_plan can report it on a machine without a GPU.
 static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
   if (d == nullptr || d->x == nullptr || d->w_packed == nullptr || d->bias == nullptr) return -1;
@@ -151,6 +143,7 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
     return -18;   // fp16 hi/lo pairs: the LO plane of every 16-bit tensor must be given (16-byte aligned offsets)
   if (d->Cin % 16 != 0 || d->cout_pad % 16 != 0 || d->Cout > d->cout_pad || d->Cout < 1) return -4;
   if (d->act == ACT_PRELU && d->alpha == nullptr) return -5;
+  if (d->cta_group > 1) return -22;         // sm_90 has no paired (two-CTA) MMA
   if (d->out16 == nullptr && d->out32 == nullptr) return -6;
   const int D = d->ndim == 3 ? d->D : 1;
   if (d->B < 1 || d->H < 1 || d->W < 1 || D < 1) return -7;
@@ -189,34 +182,7 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
   // variant cannot keep >= 3 stages in flight (tiny images -> no CTA pairing -> 3 full-width B tiles per group),
   // fall back to one A load per tap.
   auto pow2_le = [](int v, int cap) { int r = 1; while (r * 2 <= cap && r < v) r *= 2; return r; };
-  if (!split) {
-    for (int t = 0; t < d->ntaps; ++t) {
-      p.tap[t][0] = d->taps[3 * t + 0];
-      p.tap[t][1] = d->taps[3 * t + 1];
-      p.tap[t][2] = d->taps[3 * t + 2];
-      p.tap[t][3] = 0;
-      p.tap_b[t] = static_cast<uint8_t>(t);
-    }
-  } else {
-    // Split ("exact") mode: tap t = ky*nx0 + kx0 becomes three pseudo-taps with the same input offset:
-    // (x_lo, w_hi), (x_hi, w_lo), (x_hi, w_hi).  Order along the k loop: ALL correction terms of the tile first, the hi.hi
-    // terms last.  The tensor core's fp32 accumulation truncates (round toward zero, one truncation per MMA step), so the
-    // error of a step scales with the magnitude the accumulator has at that moment: while only 2^-11-sized corrections
-    // have been summed it is negligible, and only the hi.hi third of the steps runs against the full-size accumulator
-    // (measured on the 3x3 1024->1024 trunk: profiles/r02_exact_accumulation_order.log).  Within each of the three
-    // passes the ky-major order that y-halo sharing needs is preserved: pseudo kx' = j*nx0 + kx0, tap = ky*(3*nx0) + kx'.
-    const int nx0 = d->ntaps / p.ny;
-    for (int t = 0; t < d->ntaps; ++t) {
-      const int ky = t / nx0, kx0 = t % nx0;
-      for (int j = 0; j < 3; ++j) {          // j = 0: x_lo.w_hi, 1: x_hi.w_lo, 2: x_hi.w_hi
-        const int q = ky * (3 * nx0) + j * nx0 + kx0;
-        p.tap[q][0] = d->taps[3 * t + 0];
-        p.tap[q][1] = d->taps[3 * t + 1];
-        p.tap[q][2] = d->taps[3 * t + 2];
-        p.tap[q][3] = static_cast<int8_t>(j == 0 ? 1 : (j == 1 ? 2 : 0));
-        p.tap_b[q] = static_cast<uint8_t>(t);
-      }
-    }
+  if (split) {
     p.ntaps = 3 * d->ntaps;
     p.split = 1;
   }
@@ -232,40 +198,13 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
   }
   p.rank = d->ndim == 3 ? 5 : 4;
   p.W = d->W; p.H = d->H; p.D = D; p.B = d->B;
-  // TMA-store epilogue: dense 16-bit NHWC output only (no fp32 copy, no ragged / split columns)
-  const int PCh = BN >= 64 ? 64 : BN;
-  const bool dense_out = d->ndim == 2 && d->o_nsplit == 0 && d->o_base == 0 && d->o_z == 0 && d->o_x == d->cout_pad &&
-                         d->o_y == static_cast<long long>(d->W) * d->o_x && d->o_b == static_cast<long long>(d->H) * d->o_y;
-  const bool use_tma_store = !split && (d->tma_store > 0 || (d->tma_store == 0 && tn.tma_store));
-  p.tma_store = (use_tma_store && d->out16 != nullptr && d->out32 == nullptr && d->Cout == d->cout_pad && dense_out &&
-                 (reinterpret_cast<uintptr_t>(d->out16) & 15) == 0) ? 1 : 0;
-  // merged stride-2 transposed conv (rn_conv2d_transpose_s2_merged): output [B, H, 2(ay), W, 2*Cout(ax,co)]
-  const bool scatter_out = d->ndim == 2 && d->o_nsplit > 0 && d->o_nsplit % PCh == 0 && d->o_base == 0 && d->o_z == 0 &&
-                           d->o_x == d->o_nsplit && d->o_nhi == static_cast<long long>(d->W) * d->o_x &&
-                           d->o_y == 2 * d->o_nhi && d->o_b == static_cast<long long>(d->H) * d->o_y &&
-                           d->cout_pad == 2 * d->o_nsplit;
-  if (use_tma_store && scatter_out && d->out16 != nullptr && d->out32 == nullptr && d->Cout == d->cout_pad &&
-      (reinterpret_cast<uintptr_t>(d->out16) & 15) == 0)
-    p.tma_store = 2;
-  int grid = 0, CL = 1, CG = 1, sub = 0, EG = 1, stg_bytes = 0;
-  // M sub-tiles: two 128-row accumulators per CTA share every weight stage (BN <= 128 so that 2 x 2 x BN TMEM columns
-  // fit).  Halves the weight bytes per MAC; measured on every BN <= 128 layer of the network (banded 3^3 convs
-  // 0.28 -> 0.22 ms, e_conv10 0.43 -> 0.26, e_conv7_1 0.25 -> 0.17: profiles/r01_probe_msub.log), never slower.
+  int grid = 0, CL = 1, sub = 0;
+  // M sub-tiles: two 128-row accumulators per CTA share every weight stage (BN <= 128, so that 2 x BN/2 accumulator
+  // registers per consumer thread fit).  Halves the weight bytes per MAC.
   int want_ms = d->msub > 0 ? d->msub : (tn.msub > 0 ? tn.msub : 2);
   if (want_ms > 2) return -16;
   if (BN > 128 || d->ndim != 2) want_ms = 1;
-  // Epilogue warp groups: a second group of four epilogue warps (own staging buffer) where the kernel variant exists and
-  // the extra 16 KB do not cost the pipeline its third stage, its halo sharing or its second accumulator.
-  const int ny_req = p.ny, ms_req = want_ms;
-  IgemmParams p_one;                         // sizing with one epilogue group (always valid), kept as the fall-back
-  int grid_one = 0, CL_one = 1, CG_one = 1, sub_one = 0, stg_one = 0;
-  const int epi_max = d->epi_groups > 0 ? d->epi_groups : tn.epi_groups;
-  for (int eg = split ? 2 : 1; eg <= ((epi_max == 2 || split) ? 2 : 1); ++eg) {   // split kernels exist with two groups only
-  EG = eg;
-  p.ny = ny_req;
-  want_ms = ms_req;
-  stg_bytes = p.tma_store ? (eg * kTileM * PCh * 2 + 1024) : 0;
-  const int budget = 232448 - 1024 - 256 - stg_bytes;
+  const int budget = kMaxSmem - 1024 - 256 - kStgBytes;
   for (int attempt = 0; attempt < 3; ++attempt) {
     p.ms = want_ms;
     int rem = kTileM;
@@ -285,26 +224,23 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
     p.tiles_y = (d->H + p.BH * p.ms - 1) / (p.BH * p.ms);
     p.tiles_z = (D + p.BD - 1) / p.BD;
     p.num_tiles = d->B * p.tiles_x * p.tiles_y * p.tiles_z * p.n_tiles;
-    // persistent grid, cluster size CL for the B multicast, CG = 2 for the paired (cta_group::2) MMA
+    // persistent grid, cluster size CL for the B multicast (split kernels run on single CTAs)
     grid = num_sms();
     if (d->max_ctas > 0 && d->max_ctas < grid) grid = d->max_ctas;
     if (grid > p.num_tiles) grid = p.num_tiles;
     const int m_tiles = p.num_tiles / p.n_tiles;
-    CL = 1; CG = 1;
-    if (BN >= 128) {
+    CL = 1;
+    if (BN >= 128 && !split) {
       const int want = d->cluster > 0 ? d->cluster : tn.cluster;
-      const int want_cg = d->cta_group > 0 ? d->cta_group : tn.cta_group;
-      if (want_cg == 2 && m_tiles % 2 == 0 && grid >= 2) { CL = 2; CG = 2; }
-      else if (split) CL = 1;                     // split variants: CTA pairs or single CTAs
-      else if (want >= 4 && m_tiles % 4 == 0 && grid >= 4) CL = 4;
+      if (want >= 4 && m_tiles % 4 == 0 && grid >= 4) CL = 4;
       else if (want >= 2 && m_tiles % 2 == 0 && grid >= 2) CL = 2;
     }
     grid -= grid % CL;
     p.a_sub_bytes = ((p.BD * p.BW * (p.BH * p.ms + p.ny - 1) * p.row_bytes + 1023) / 1024) * 1024;
-    p.b_sub_bytes = (((BN / CG) * p.row_bytes + 1023) / 1024) * 1024;
+    p.b_sub_bytes = ((BN * p.row_bytes + 1023) / 1024) * 1024;
     sub = p.a_sub_bytes + p.ny * p.b_sub_bytes;       // one group: A (halo) + ny weight tiles
     const int total_k = (p.ntaps / p.ny) * p.kblocks;
-    // groups per stage: ~64 KB stages amortise the per-stage barrier round trips (measured: tune3/tune4 logs)
+    // groups per stage: ~64 KB stages amortise the per-stage barrier round trips
     p.kps = (65536 + sub / 2) / sub;
     if (p.kps < 1) p.kps = 1;
     if (p.kps > 8) p.kps = 8;
@@ -321,21 +257,39 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
     if (want_ms > 1) want_ms = 1;           // retry with one accumulator per tile,
     else p.ny = 1;                          // then without halo sharing
   }
-  if (eg == 1) {
-    p_one = p; grid_one = grid; CL_one = CL; CG_one = CG; sub_one = sub; stg_one = stg_bytes;
-  } else if (!split) {
-    const bool have_variant = (BN == 256 && CG == 2) || (BN == 128 && (CG == 2 || (CG == 1 && CL == 2))) ||
-                              (BN < 128 && p.ms == 2);
-    const bool same_shape = p.ms == p_one.ms && p.ny == p_one.ny && CL == CL_one && CG == CG_one;
-    if (!(have_variant && same_shape && p.stages >= 3)) {    // keep the single-group sizing
-      p = p_one; grid = grid_one; CL = CL_one; CG = CG_one; sub = sub_one; stg_bytes = stg_one; EG = 1;
+  if (p.stages < 2) return -10;
+  if (!split) {
+    for (int t = 0; t < d->ntaps; ++t) {
+      p.tap[t][0] = d->taps[3 * t + 0];
+      p.tap[t][1] = d->taps[3 * t + 1];
+      p.tap[t][2] = d->taps[3 * t + 2];
+      p.tap[t][3] = 0;
+      p.tap_b[t] = static_cast<uint8_t>(t);
+    }
+  } else {
+    // Split ("exact") mode: tap t = ky*nx0 + kx0 becomes three pseudo-taps with the same input offset:
+    // (x_lo, w_hi), (x_hi, w_lo), (x_hi, w_hi).  Order along the k loop: ALL correction terms of the tile first, the hi.hi
+    // terms last.  The tensor core's fp32 accumulation truncates (round toward zero, one truncation per MMA step), so the
+    // error of a step scales with the magnitude the accumulator has at that moment: while only 2^-11-sized corrections
+    // have been summed it is negligible, and only the hi.hi third of the steps runs against the full-size accumulator
+    // (DESIGN.md §4).  Within each of the three
+    // passes the ky-major order that y-halo sharing needs is preserved: pseudo kx' = j*nx0 + kx0, tap = ky*(3*nx0) + kx'
+    // (built from the FINAL ny: without halo sharing nx0 = ntaps and the order is simply j-major).
+    const int nx0 = d->ntaps / p.ny;
+    for (int t = 0; t < d->ntaps; ++t) {
+      const int ky = t / nx0, kx0 = t % nx0;
+      for (int j = 0; j < 3; ++j) {          // j = 0: x_lo.w_hi, 1: x_hi.w_lo, 2: x_hi.w_hi
+        const int q = ky * (3 * nx0) + j * nx0 + kx0;
+        p.tap[q][0] = d->taps[3 * t + 0];
+        p.tap[q][1] = d->taps[3 * t + 1];
+        p.tap[q][2] = d->taps[3 * t + 2];
+        p.tap[q][3] = static_cast<int8_t>(j == 0 ? 1 : (j == 1 ? 2 : 0));
+        p.tap_b[q] = static_cast<uint8_t>(t);
+      }
     }
   }
-  }
-  if (p.stages < 2) return -10;
-  pl.BN = BN; pl.CL = CL; pl.CG = CG; pl.EG = EG; pl.grid = grid; pl.sub = sub; pl.stg_bytes = stg_bytes; pl.PCh = PCh;
-  pl.KB = KB; pl.D = D;
-  pl.smem = static_cast<size_t>(p.stages) * p.kps * sub + 1024 + 256 + stg_bytes;
+  pl.BN = BN; pl.CL = CL; pl.grid = grid; pl.sub = sub; pl.KB = KB; pl.D = D;
+  pl.smem = static_cast<size_t>(p.stages) * p.kps * sub + 1024 + 256 + kStgBytes;
   return 0;
 }
 }  // namespace rn
@@ -345,8 +299,9 @@ extern "C" int rn_conv_plan(const rn_conv_desc* d, int* out, int n_out) {
   rn::ConvPlan pl;
   const int rc = rn::plan_conv(d, p, pl);
   if (rc != 0) return rc;
-  const int v[16] = {pl.BN, pl.CL, pl.CG, p.ms, pl.EG, p.ny, p.BW, p.BH, p.BD, p.kps, p.stages, static_cast<int>(pl.smem),
-                     pl.grid, p.num_tiles, p.tma_store, p.row_bytes};
+  // cta_group is always 1 and the epilogue always the two consumer warpgroups' direct stores (mode 0)
+  const int v[16] = {pl.BN, pl.CL, 1, p.ms, 2, p.ny, p.BW, p.BH, p.BD, p.kps, p.stages, static_cast<int>(pl.smem),
+                     pl.grid, p.num_tiles, 0, p.row_bytes};
   for (int i = 0; i < n_out && i < 16; ++i) out[i] = v[i];
   return 0;
 }
@@ -360,9 +315,8 @@ extern "C" int rn_conv_igemm(const rn_conv_desc* d, void* stream_v) {
   if (prc != 0) return prc;
   PFN_encodeTiled enc = get_encode_fn();
   if (enc == nullptr) return -8;
-  const int BN = pl.BN, CL = pl.CL, CG = pl.CG, EG = pl.EG, grid = pl.grid, PCh = pl.PCh, KB = pl.KB, D = pl.D;
+  const int BN = pl.BN, CL = pl.CL, grid = pl.grid, KB = pl.KB, D = pl.D;
   const size_t smem = pl.smem;
-
 
   const CUtensorMapDataType dt = d->fmt == 1 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const bool split = d->fmt == 2;
@@ -395,15 +349,10 @@ extern "C" int rn_conv_igemm(const rn_conv_desc* d, void* stream_v) {
   }
   if (r != CUDA_SUCCESS) return 1000 + static_cast<int>(r);
   const uint16_t* w_hi = static_cast<const uint16_t*>(d->w_packed);
-  if (p.band_half && CG == 2) {   // CTA-pair arrangement of the half tiles follows the single-CTA one
-    const long long arr = 9LL * p.kblocks * 128 * 64;
-    w_hi += arr;
-    if (split) w_lo += arr;
-  }
   if (d->w_banded) {  // [ntaps*kblocks][BN][KB], identical for every N tile
     const cuuint64_t dims[3] = {(cuuint64_t)KB, (cuuint64_t)BN, (cuuint64_t)d->ntaps * p.kblocks};
     const cuuint64_t strides[2] = {(cuuint64_t)KB * 2, (cuuint64_t)KB * 2 * BN};
-    const cuuint32_t box[3] = {(cuuint32_t)KB, (cuuint32_t)(BN / CL), 1};  // CL == 2 also for the paired MMA
+    const cuuint32_t box[3] = {(cuuint32_t)KB, (cuuint32_t)(BN / CL), 1};  // each CTA of a cluster fetches 1/CL of B
     r = enc(&p.tmB, dt, 3, const_cast<uint16_t*>(w_hi), dims, strides, box, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
             swizzle_of(p.row_bytes), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r == CUDA_SUCCESS && split)
@@ -412,7 +361,7 @@ extern "C" int rn_conv_igemm(const rn_conv_desc* d, void* stream_v) {
   } else {
     const cuuint64_t dims[3] = {(cuuint64_t)d->Cin, (cuuint64_t)d->cout_pad, (cuuint64_t)d->ntaps};
     const cuuint64_t strides[2] = {(cuuint64_t)d->Cin * 2, (cuuint64_t)d->Cin * 2 * d->cout_pad};
-    const cuuint32_t box[3] = {(cuuint32_t)KB, (cuuint32_t)(BN / CL), 1};  // CL == 2 also for the paired MMA
+    const cuuint32_t box[3] = {(cuuint32_t)KB, (cuuint32_t)(BN / CL), 1};  // each CTA of a cluster fetches 1/CL of B
     r = enc(&p.tmB, dt, 3, const_cast<uint16_t*>(w_hi), dims, strides, box, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
             swizzle_of(p.row_bytes), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r == CUDA_SUCCESS && split)
@@ -421,42 +370,10 @@ extern "C" int rn_conv_igemm(const rn_conv_desc* d, void* stream_v) {
   }
   if (r != CUDA_SUCCESS) return 2000 + static_cast<int>(r);
 
-  if (p.tma_store == 2) {
-    const cuuint64_t C2 = static_cast<cuuint64_t>(d->o_nsplit);          // 2*Cout elements per (x, ay)
-    const cuuint64_t dims[5] = {C2, (cuuint64_t)d->W, 2, (cuuint64_t)d->H, (cuuint64_t)d->B};
-    const cuuint64_t strides[4] = {C2 * 2, (cuuint64_t)d->o_nhi * 2, (cuuint64_t)d->o_y * 2, (cuuint64_t)d->o_b * 2};
-    const cuuint32_t box[5] = {(cuuint32_t)PCh, (cuuint32_t)p.BW, 1, (cuuint32_t)p.BH, 1};
-    r = enc(&p.tmO, dt, 5, d->out16, dims, strides, box, ones, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_of(PCh * 2),
-            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return 3000 + static_cast<int>(r);
-  } else if (p.tma_store) {
-    const cuuint64_t Ct = static_cast<cuuint64_t>(d->cout_pad);
-    const cuuint64_t dims[4] = {Ct, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->B};
-    const cuuint64_t strides[3] = {Ct * 2, Ct * 2 * d->W, Ct * 2 * d->W * d->H};
-    const cuuint32_t box[4] = {(cuuint32_t)PCh, (cuuint32_t)p.BW, (cuuint32_t)p.BH, 1};
-    r = enc(&p.tmO, dt, 4, d->out16, dims, strides, box, ones, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_of(PCh * 2),
-            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return 3000 + static_cast<int>(r);
-  }
-  // residual L2 prefetch: 16-bit residual laid out exactly like the dense 16-bit output (same map, other base pointer)
-  p.res_l2_prefetch = 0;
-  const bool res_pre = d->res_prefetch > 0 || (d->res_prefetch == 0 && tuning().res_prefetch);
-  if (res_pre && p.tma_store == 1 && d->residual != nullptr && !d->residual_is_f32 &&
-      (reinterpret_cast<uintptr_t>(d->residual) & 15) == 0) {
-    const cuuint64_t Ct = static_cast<cuuint64_t>(d->cout_pad);
-    const cuuint64_t dims[4] = {Ct, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->B};
-    const cuuint64_t strides[3] = {Ct * 2, Ct * 2 * d->W, Ct * 2 * d->W * d->H};
-    const cuuint32_t box[4] = {(cuuint32_t)PCh, (cuuint32_t)p.BW, (cuuint32_t)p.BH, 1};
-    r = enc(&p.tmR, dt, 4, const_cast<void*>(d->residual), dims, strides, box, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            swizzle_of(PCh * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return 4000 + static_cast<int>(r);
-    p.res_l2_prefetch = 1;
-  }
   p.out16 = d->out16; p.out32 = d->out32; p.res = d->residual; p.res_is_f32 = d->residual_is_f32;
   p.bias = d->bias; p.alpha = d->alpha; p.act = d->act; p.n_valid = d->Cout;
   p.o_base = d->o_base; p.o_b = d->o_b; p.o_y = d->o_y; p.o_x = d->o_x; p.o_z = d->o_z;
   p.o_nsplit = d->o_nsplit; p.o_nhi = d->o_nhi;
-  p.res_prefetch = res_pre ? 1 : 0;
   p.o_plane = d->o_plane;
   if (d->phong != nullptr) {      // fused Phong composite (16-column kernels, sigmoid epilogue, direct fp32 / uint8 stores)
     if (BN != 16 || d->act != ACT_SIGMOID || d->Cout % 3 != 0 || d->Cout > 15 || d->o_nsplit != 0 || d->residual != nullptr ||
@@ -472,6 +389,6 @@ extern "C" int rn_conv_igemm(const rn_conv_desc* d, void* stream_v) {
   auto al16 = [](const void* q) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   p.vec_ok = strides8 && al16(d->out16) && al16(d->out32) && al16(d->residual) ? 1 : 0;
 
-  const cudaError_t e = launch_variant(BN, CL, CG, p.ms, EG, p.split, p, grid, smem, stream);
+  const cudaError_t e = launch_variant(BN, CL, p.ms, p.split, p.band_half, p, grid, smem, stream);
   return e == cudaSuccess ? 0 : static_cast<int>(e);
 }

@@ -1,4 +1,4 @@
-// rn_igemm.cuh -- parameter block shared by the host launcher and the tcgen05 implicit-GEMM kernel.
+// rn_igemm.cuh -- parameter block shared by the host launcher and the wgmma implicit-GEMM kernel.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -6,15 +6,15 @@
 namespace rn {
 
 constexpr int kMaxTaps = 48;   // 16 filter taps x 3 operand-split terms (fmt 2)
-constexpr int kTileM = 128;  // rows (pixels / voxels) per CTA tile == TMEM lanes
+constexpr int kMaxSmem = 232448;   // opt-in dynamic shared memory per block on sm_90 (227 KB)
+constexpr int kStgBytes = 2 * 64 * 36 * 4;   // epilogue staging: 64 rows x (32 + 4 padding) fp32 per consumer warpgroup
+constexpr int kTileM = 128;  // rows (pixels / voxels) per CTA (sub-)tile: 64 per consumer warpgroup
 
 enum Act : int { ACT_NONE = 0, ACT_PRELU = 1, ACT_SIGMOID = 2 };
 
 struct alignas(64) IgemmParams {
   CUtensorMap tmA;  // activations, channel-last: rank 4 {C,W,H,B} or rank 5 {C,D,W,H,B}; box {KB,[BD],BW,BH,1}
   CUtensorMap tmB;  // weights [tap][CoutPad][Cin]: rank 3 {Cin,CoutPad,taps}; box {KB,BN,1}
-  CUtensorMap tmR;  // 16-bit residual, same geometry and box as tmO (dense output): L2 prefetch of the next tile's rows
-  CUtensorMap tmO;  // 16-bit output {Cout,W,H,B}; box {panel cols (<=64), BW, BH, 1}: TMA-store epilogue (tma_store != 0)
   CUtensorMap tmA2; // split mode (fmt 2): the LO plane of the activations, same geometry as tmA
   CUtensorMap tmB2; // split mode: the LO plane of the packed weights, same geometry as tmB
   int rank;
@@ -24,7 +24,7 @@ struct alignas(64) IgemmParams {
   int n_tiles;                    // CoutPad / BN
   int num_tiles;                  // B*tiles_y*tiles_x*tiles_z*n_tiles
   int ntaps, kblocks;             // k-iterations = ntaps * kblocks, each KB = row_bytes/2 input channels
-  int row_bytes;                  // 32 / 64 / 128 (== TMA + UMMA swizzle span)
+  int row_bytes;                  // 32 / 64 / 128 (== TMA + wgmma swizzle span)
   int kps;                        // k-iterations per pipeline stage
   int stages;
   int a_sub_bytes, b_sub_bytes;   // smem bytes of one k-iteration's A / B sub-buffer (1024-multiples)
@@ -39,7 +39,7 @@ struct alignas(64) IgemmParams {
                                   // LO plane (tmA2), bit 1: B operand comes from the LO plane (tmB2) -- split mode only
   uint8_t tap_b[kMaxTaps];        // tap coordinate of pseudo-tap t in the packed filter (== t unless split)
   // Split mode (fmt 2, "exact"): every 16-bit tensor is a PAIR of fp16 planes, hi = fp16(v), lo = fp16(v - hi), ~22
-  // mantissa bits together.  Each filter tap becomes three pseudo-taps accumulated into the same TMEM tile:
+  // mantissa bits together.  Each filter tap becomes three pseudo-taps accumulated into the same accumulator tile:
   // x_hi.w_hi + x_lo.w_hi + x_hi.w_lo (the lo.lo term is below fp32 resolution); the epilogue reads a hi+lo residual and
   // writes hi and lo planes.  The reference computes these convolutions in fp32 (tools/layer_util.py:171,212,253).
   int split;
@@ -56,15 +56,12 @@ struct alignas(64) IgemmParams {
   float* out32;                   // fp32 output or nullptr
   const void* res;                // residual (same indexing as the output) or nullptr
   int res_is_f32;
-  int res_l2_prefetch;            // 1: tmR is valid; the epilogue prefetches the NEXT tile's residual boxes into L2
-  int res_prefetch;               // 1: 16-bit residual rows are fetched one panel ahead into registers
   const float* bias;              // [CoutPad]
   const float* alpha;             // [CoutPad] (PReLU) or nullptr
   int act;
   int n_valid;                    // real Cout (<= CoutPad); columns beyond are dropped
   int vec_ok;                     // output/residual rows are 16B aligned -> vector path
   long long o_base, o_b, o_y, o_x, o_z;  // output element offset = o_base + b*o_b + y*o_y + x*o_x + z*o_z + n
-  int tma_store;                  // 1: epilogue stages 64-column panels in swizzled smem and stores them with TMA
   // Phong composite + uint8 fused into the sigmoid epilogue of the x-folded last up-conv (SURVEY §8 f-2; 16-column kernels only):
   // a GEMM row holds the 3 channels of phong_F adjacent pixels; out32 then receives the SHADED colour and out_u8 its uint8 form.
   const float* phong_light_dir;   // [B,3] or nullptr (off)
@@ -113,13 +110,11 @@ inline BandLayout band_layout(int Cin, int Cout, int sz) {
 
 // launch-heuristic defaults (immutable after first use; RN_TUNE environment override -- rn_igemm.cu)
 struct Tuning {
-  int cluster = 2;        // B-multicast cluster size when the descriptor says 0
-  int cta_group = 2;      // 2: paired tcgen05.mma.cta_group::2 tiles where the shape allows
+  int cluster = 1;        // B-multicast cluster size when the descriptor says 0.  1: on the H100 the weight multicast of a
+                          // 2 / 4-CTA cluster made the 3x3 1024->1024 trunk conv 2.6x / 6.5x slower (2.60 vs 6.76 / 17.0
+                          // ms per B=24 launch, fp16), the stage releases couple every CTA of the cluster
   int kps = 0;            // k-groups per pipeline stage (0 = heuristic)
   int msub = 0;           // M sub-tiles per CTA tile (0 = heuristic)
-  int epi_groups = 2;     // epilogue warp groups where a two-group kernel variant exists
-  int res_prefetch = 1;   // fetch 16-bit residual rows one panel ahead in the epilogue
-  int tma_store = 1;      // TMA-store epilogue where the output is a dense 16-bit NHWC tensor
   int yhalo = 1;          // y-halo sharing of the activation operand (3x3, banded 3^3, merged / x-folded transposed)
   int tiled_tex_conv = 1; // shared-memory tiled kernel for the texture decoder's 4^3 8->4 conv (0: generic kernel; A/B, tests)
   int pdl = 0;            // programmatic dependent launch: igemm launches carry the programmatic-stream-serialization attribute,

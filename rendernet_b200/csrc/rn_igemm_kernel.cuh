@@ -1,4 +1,4 @@
-// rn_igemm_kernel.cuh -- implicit-GEMM convolution on 5th-gen tensor cores (tcgen05) for sm_100a.
+// rn_igemm_kernel.cuh -- implicit-GEMM convolution on Hopper tensor cores (wgmma) for sm_90a.
 //
 // One kernel serves every dense contraction of the RenderNet forward path (reference call sites:
 // tools/layer_util.py:21 projection 1x1, :101-104 3x3 res blocks, :253 conv3d, :212 conv2d_transpose;
@@ -8,21 +8,20 @@
 //     128-row A tile is ONE tiled-TMA box {KB channels, BD, BW, BH} fetched at a shifted coordinate; TMA's
 //     out-of-bounds zero fill implements TF "SAME" padding (asymmetric pads are just different offsets).
 //   * B (weights) is pre-packed [tap][Cout][Cin] so a {KB, BN} box is a K-major operand tile.
-//   * Both land in shared memory in the 32/64/128-byte swizzled K-major layout that tcgen05.mma reads
-//     through shared-memory descriptors; accumulators live in TMEM (2 x BN fp32 columns, double-buffered
-//     so the epilogue of tile i overlaps the MMAs of tile i+1).
-//   * Warp roles: warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread MMA issuer,
-//     warps 2..5 = epilogue (tcgen05.ld -> bias/PReLU/residual/sigmoid -> 16B global stores).
+//   * Both land in shared memory in the 32/64/128-byte swizzled K-major layout that wgmma reads through
+//     shared-memory descriptors.
+//   * Warpgroup roles: warpgroup 0 = TMA producer (one thread issues, the rest give their registers away through
+//     setmaxnreg), warpgroups 1 and 2 = consumers: each issues m64nBNk16 wgmmas for 64 of the tile's 128 rows into fp32
+//     register accumulators and then runs the epilogue of those rows (bias/PReLU/residual/sigmoid -> 16-byte stores).
 //   * Persistent: grid = #SMs, static round-robin tile schedule with N fastest so concurrently running
-//     CTAs share the same activation rows in L2.
+//     CTAs share the same activation rows in L2.  The producer runs ahead into the next tile while the consumers drain.
 //
 // This header holds the device code and the per-variant launcher template `launch_ms`.  It is included only by
-// rn_igemm_inst.cu, which the Makefile compiles once per <BN, CL, CG, MS, EG, SPLIT> variant (one object each, so that
+// rn_igemm_inst.cu, which the Makefile compiles once per <BN, CL, MS, SPLIT, HALF> variant (one object each, so that
 // `make -j` spreads them over the cores); rn_igemm.cu (host side: validation, tile/pipeline sizing, tensor maps) declares
 // the template and dispatches to the instantiated variants.
 #pragma once
 #include <atomic>
-#include <type_traits>
 #include <cstdio>
 #include <cstring>
 #include <cuda_bf16.h>
@@ -35,8 +34,11 @@ namespace rn {
 
 extern std::atomic<long long> g_launch_count;   // kernels launched by this library (bench.py's gpu_launches)
 
-constexpr int kNumThreads = 192;
-constexpr int kMaxDevices = 64;   // device ordinals with cached per-device state
+constexpr int kNumThreads = 384;                // producer warpgroup + two consumer warpgroups
+constexpr int kMaxDevices = 64;                 // device ordinals with cached per-device state
+constexpr int kStgCols = 32;                    // accumulator columns staged through shared memory per epilogue pass
+constexpr int kStgStride = kStgCols + 4;        // floats per staged row (padding spreads the rows over the banks)
+static_assert(kStgBytes == 2 * 64 * kStgStride * 4, "one 64-row staging panel per consumer warpgroup (rn_igemm.cuh)");
 
 struct TileCoord {
   int b, x0, y0, z0, n0;
@@ -60,21 +62,20 @@ __device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int tile,
   return t;
 }
 
-// stg != 0: the 16-bit result goes to the shared-memory staging panel (row `m`, 16-byte chunk index `chunk0`..) in the
-// TMA swizzle of a `prow`-byte row instead of to global memory (the residual is still read from global).
+// Epilogue of CW consecutive accumulator columns n0.. of one output row (element offset `off`): bias, activation, residual,
+// 16-bit and/or fp32 stores.
 template <int CW, bool SPLIT = false>
-__device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const uint32_t* __restrict__ r, int n0,
-                                               long long off, bool row_valid, uint32_t stg = 0, int m = 0,
-                                               int chunk0 = 0, int prow = 128, const uint4* rpre = nullptr, int bidx = 0) {
-  if (!row_valid && stg == 0) return;
+__device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const float* __restrict__ a, int n0, long long off,
+                                               bool row_valid, int bidx) {
+  if (!row_valid) return;
   float v[CW];
 #pragma unroll
   for (int i = 0; i < CW; i += 4) {
     const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + i));
-    v[i + 0] = __uint_as_float(r[i + 0]) + b4.x;
-    v[i + 1] = __uint_as_float(r[i + 1]) + b4.y;
-    v[i + 2] = __uint_as_float(r[i + 2]) + b4.z;
-    v[i + 3] = __uint_as_float(r[i + 3]) + b4.w;
+    v[i + 0] = a[i + 0] + b4.x;
+    v[i + 1] = a[i + 1] + b4.y;
+    v[i + 2] = a[i + 2] + b4.z;
+    v[i + 3] = a[i + 3] + b4.w;
   }
   if (p.act == ACT_PRELU) {
 #pragma unroll
@@ -93,21 +94,19 @@ __device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const uint3
     // Last up-conv of the Shader net (x-folded, N = F pixels x 3 channels <= 16): Phong composite + uint8 quantisation of the
     // sigmoid output while it is still in registers (tools/Phong_shading.py:202-228, RenderNet_demo.py:58).
     if (p.phong_light_dir != nullptr && p.act == ACT_SIGMOID && n0 == 0) {
-      if (row_valid) {
-        const float* ld = p.phong_light_dir + 3 * bidx;
-        const float lx = __ldg(ld), ly = __ldg(ld + 1), lz = __ldg(ld + 2);
-        float col[3] = {__ldg(p.phong_light_col + 3 * bidx), __ldg(p.phong_light_col + 3 * bidx + 1), __ldg(p.phong_light_col + 3 * bidx + 2)};
+      const float* ld = p.phong_light_dir + 3 * bidx;
+      const float lx = __ldg(ld), ly = __ldg(ld + 1), lz = __ldg(ld + 2);
+      float col[3] = {__ldg(p.phong_light_col + 3 * bidx), __ldg(p.phong_light_col + 3 * bidx + 1), __ldg(p.phong_light_col + 3 * bidx + 2)};
 #pragma unroll
-        for (int px = 0; px < 5; ++px) {
-          if (px < p.phong_F) {
-            float sh[3];
-            phong_pixel(v[3 * px], v[3 * px + 1], v[3 * px + 2], lx, ly, lz, col, p.phong_ambient, p.phong_kd, p.phong_white,
-                        p.phong_mask, sh);
+      for (int px = 0; px < 5; ++px) {
+        if (px < p.phong_F) {
+          float sh[3];
+          phong_pixel(v[3 * px], v[3 * px + 1], v[3 * px + 2], lx, ly, lz, col, p.phong_ambient, p.phong_kd, p.phong_white,
+                      p.phong_mask, sh);
 #pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              if (p.out32 != nullptr) p.out32[off + 3 * px + c] = sh[c];
-              if (p.out_u8 != nullptr) p.out_u8[off + 3 * px + c] = phong_u8(sh[c]);
-            }
+          for (int c = 0; c < 3; ++c) {
+            if (p.out32 != nullptr) p.out32[off + 3 * px + c] = sh[c];
+            if (p.out_u8 != nullptr) p.out_u8[off + 3 * px + c] = phong_u8(sh[c]);
           }
         }
       }
@@ -116,7 +115,7 @@ __device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const uint3
   }
   const bool full = p.vec_ok && (n0 + CW <= p.n_valid);
   if (full) {
-    if (p.res != nullptr && row_valid) {
+    if (p.res != nullptr) {
       if (p.res_is_f32) {
         const float4* rp = reinterpret_cast<const float4*>(static_cast<const float*>(p.res) + off + n0);
 #pragma unroll
@@ -128,7 +127,7 @@ __device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const uint3
         const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.res) + off + n0);
 #pragma unroll
         for (int i = 0; i < CW / 8; ++i) {
-          const uint4 q = rpre != nullptr ? rpre[i] : __ldg(rp + i);   // rpre: fetched a panel ahead by the caller
+          const uint4 q = __ldg(rp + i);
           const uint32_t w[4] = {q.x, q.y, q.z, q.w};
           if constexpr (SPLIT) {      // residual = hi + lo (exact in fp32: <= 22 significant bits)
             const uint4 ql = __ldg(rp + i + (p.o_plane >> 3));
@@ -155,11 +154,10 @@ __device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const uint3
     }
     if (p.out16 != nullptr) {
       uint4* op = reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.out16) + off + n0);
-      const int sw = prow == 128 ? (m & 7) : (prow == 64 ? ((m >> 1) & 3) : ((m >> 2) & 1));
 #pragma unroll
       for (int i = 0; i < CW / 8; ++i) {
         uint32_t w[4];
-        if constexpr (SPLIT) {        // hi = fp16(v), lo = fp16(v - hi): two planes, direct stores (tma_store is off in split mode)
+        if constexpr (SPLIT) {        // hi = fp16(v), lo = fp16(v - hi): two planes
           uint32_t wl[4];
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
@@ -182,8 +180,7 @@ __device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const uint3
               w[j] = *reinterpret_cast<uint32_t*>(&h);
             }
           }
-          if (stg != 0) st_shared_v4(stg + m * prow + (((chunk0 + i) ^ sw) << 4), w[0], w[1], w[2], w[3]);
-          else op[i] = make_uint4(w[0], w[1], w[2], w[3]);
+          op[i] = make_uint4(w[0], w[1], w[2], w[3]);
         }
       }
     }
@@ -223,29 +220,23 @@ __device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const uint3
 // CL = thread-block-cluster size (1, 2 or 4).  The CL CTAs of a cluster work on CL consecutive M tiles of the SAME
 // N tile; each loads 1/CL of every weight (B) tile and TMA-multicasts it to all of them, so B is fetched from L2
 // once per cluster instead of once per CTA.  A smem stage may only be refilled when every CTA of the cluster has
-// released it (empty barrier count = CL; each MMA warp commits to all CTAs' empty barriers).
+// released it: the empty barrier counts the 8 consumer warps of each of the CL CTAs, and every consumer warp arrives on
+// the barrier of every CTA of the cluster.
 //
-// CG = 2 (implies CL = 2): the pair issues ONE tcgen05.mma.cta_group::2 per k-step with M = 256: each CTA stages its
-// own 128 A rows and only HALF of the B tile (BN/2 rows); the tensor cores of both SMs read both halves.  Per SM
-// this cuts the operand bytes per MMA cycle from 48 KB to 32 KB per k-block (BN = 256), which matters because the
-// 1-CTA kernel is bound by the ~64 B/clk an SM can ingest from L2.  Only the leader CTA (rank 0) issues MMAs; its
-// full barrier collects the TMA bytes of both CTAs; commits are multicast to both CTAs' barriers; the peer's
-// epilogue warps release the accumulator on the leader's barrier with a remote arrive.
-//
-// EG = epilogue warp groups (1 or 2).  EG = 2 adds warps 6..9: both groups of four warps cover the four TMEM lane
-// quadrants, each drains half of the tile's panels (its own M sub-tile, or its own half of the columns) through its own
-// staging buffer and named barrier.  For the short-K tiles (1x1 projection unit, banded 3^3 convs, thin decoder layers)
-// the epilogue is latency-bound (tcgen05.ld behind queued MMAs, residual rows from L2) and was the critical path.
-// SPLIT = operand-split "exact" mode (fmt 2, see IgemmParams::split): compiled only for the two-epilogue-group variants.
-template <int BN, int CL, int CG, int MS, int EG, bool SPLIT>
-__global__ void __launch_bounds__(64 + 128 * EG, 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
-  static_assert(CG == 1 || (CG == 2 && CL == 2), "cta_group::2 runs on a 2-CTA cluster");
-  static_assert(EG == 1 || EG == 2, "one or two epilogue warp groups");
-  static_assert(!SPLIT || EG == 2, "split mode is instantiated for the two-group epilogue only");
-  static_assert(MS == 1 || (MS == 2 && BN <= 128), "two accumulators per tile need 4 x BN <= 512 TMEM columns");
-  constexpr int CW = (BN >= 32) ? 32 : 16;                     // epilogue column chunk
-  constexpr int ms = MS;                                       // M sub-tiles (accumulators) per tile (== p.ms)
-  constexpr uint32_t kTmemCols = (2 * MS * BN < 32) ? 32u : static_cast<uint32_t>(2 * MS * BN);  // double-buffered accumulators
+// MS = M sub-tiles (accumulators) per CTA tile: with MS = 2 every weight stage feeds two 128-row accumulators, halving the
+// weight traffic per MAC (BN <= 128: 2 x BN/2 fp32 registers per consumer thread).
+// SPLIT = operand-split "exact" mode (fmt 2, see IgemmParams::split).
+// HALF = banded filter with half-tile K blocks (IgemmParams::band_half): the accumulator is kept as two N = BN/2 halves in
+// separate register arrays, and an edge K block issues only the MMAs of the half it feeds.  (Selecting the MMA width at run
+// time on one array makes ptxas serialise every wgmma of the kernel, so the other kernels do not carry this path.)
+template <int BN, int CL, int MS, bool SPLIT, bool HALF>
+__global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
+  static_assert(MS == 1 || (MS == 2 && BN <= 128), "two accumulators per tile need 2 x BN/2 <= 128 registers per thread");
+  constexpr int NP = HALF ? 2 : 1;                             // accumulator parts per M sub-tile
+  constexpr int NACC = BN / 2 / NP;                            // accumulator registers per thread, M sub-tile and part
+  constexpr int JP = BN / 8 / NP;                              // 8-column blocks per part
+  constexpr int SC = BN < kStgCols ? BN : kStgCols;            // columns per epilogue pass
+  constexpr int TPR = SC / 16;                                 // epilogue threads per row (16 columns each)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
@@ -256,38 +247,24 @@ __global__ void __launch_bounds__(64 + 128 * EG, 1) igemm_kernel(const __grid_co
   const int stage_bytes = p.kps * sub_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + static_cast<size_t>(p.stages) * stage_bytes);
   uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* tfull_bar = empty_bar + p.stages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  // TMA-store staging panel (128 rows x <=128 B, swizzled), 1024-aligned, after the barrier block
-  const uint32_t stg_base = (smem_u32(smem) + static_cast<uint32_t>(p.stages) * stage_bytes + 256u + 1023u) & ~1023u;
+  float* stg_all = reinterpret_cast<float*>(smem + static_cast<size_t>(p.stages) * stage_bytes + 256);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
-    if (p.tma_store) tma_prefetch_desc(&p.tmO);
-    if (p.res_l2_prefetch) tma_prefetch_desc(&p.tmR);
     if constexpr (SPLIT) { tma_prefetch_desc(&p.tmA2); tma_prefetch_desc(&p.tmB2); }
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], CG == 2 ? 1 : CL);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], (CG == 2 ? 8 : 4) * EG);   // 4 epilogue warps per group (x2 CTAs feeding the leader's barrier)
+      mbar_init(&empty_bar[s], 8 * CL);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<CG>(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CL > 1) cluster_sync();   // peers' barriers are initialised before any multicast / remote commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch (no-ops for a normally launched grid): everything above — barrier init, TMEM allocation,
-  // descriptor prefetch, the cluster handshake — touched only kernel parameters and this CTA's own resources, so it may run
-  // while the previous kernel of the stream drains.  Let OUR dependents be scheduled as our CTAs retire, then wait for the
-  // previous grid to complete (and its writes to be visible) before any thread reads or writes global memory.
+  if constexpr (CL > 1) cluster_sync();   // peers' barriers are initialised before any multicast / remote arrive
+  // Programmatic dependent launch (no-ops for a normally launched grid): everything above touched only kernel parameters
+  // and this CTA's own shared memory, so it may run while the previous kernel of the stream drains.  Let OUR dependents be
+  // scheduled as our CTAs retire, then wait for the previous grid to complete (and its writes to be visible) before any
+  // thread reads or writes global memory.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
   const int cta_rank = (CL > 1) ? static_cast<int>(cluster_ctarank()) : 0;
@@ -300,14 +277,13 @@ __global__ void __launch_bounds__(64 + 128 * EG, 1) igemm_kernel(const __grid_co
   const int nx = p.ntaps / ny;
   const int total_k = nx * p.kblocks;                          // groups per tile (each = ny k-iterations of MMAs)
   const int kb_elems = p.row_bytes >> 1;
-  const uint32_t a_tx = static_cast<uint32_t>(p.BD * p.BW * (p.BH * ms + ny - 1)) * p.row_bytes;
-  const uint32_t b_tx = (CG == 2 ? BN / 2 : BN) * p.row_bytes;   // B bytes that land in THIS CTA's smem
 
-  if (warp == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
     // ------------------------------------------------------------ TMA producer (one thread).  The k loop is
     // (tap, kblock)-nested so there is no division, and everything loop-invariant lives in registers: this
     // thread's issue rate bounds the whole pipeline.
-    if (elect_one()) {
+    if (warp == 0 && elect_one()) {
       constexpr uint16_t kMask = static_cast<uint16_t>((1u << CL) - 1u);
       constexpr int kBRows = BN / CL;               // rows of the B tile this CTA fetches (and multicasts)
       const int kps = p.kps, kblocks = p.kblocks, stages = p.stages;
@@ -315,9 +291,10 @@ __global__ void __launch_bounds__(64 + 128 * EG, 1) igemm_kernel(const __grid_co
       const uint32_t smem_base = smem_u32(smem), full0 = smem_u32(full_bar);
       const uint32_t a_sub = static_cast<uint32_t>(p.a_sub_bytes), sub_u = static_cast<uint32_t>(sub_bytes);
       const uint32_t b_sub = static_cast<uint32_t>(p.b_sub_bytes);
-      const uint32_t kit_tx = (CG == 2 ? 2u : 1u) * (a_tx + static_cast<uint32_t>(ny) * b_tx);
-      const uint32_t b_off = (CL > 1 && CG == 1) ? static_cast<uint32_t>(cta_rank * kBRows * p.row_bytes) : 0u;
-      const int b_row = (CG == 2) ? cta_rank * (BN / 2) : ((CL > 1) ? cta_rank * kBRows : 0);
+      const uint32_t a_tx = static_cast<uint32_t>(p.BD * p.BW * (p.BH * MS + ny - 1)) * p.row_bytes;
+      const uint32_t kit_tx = a_tx + static_cast<uint32_t>(ny) * BN * p.row_bytes;
+      const uint32_t b_off = static_cast<uint32_t>(cta_rank * kBRows * p.row_bytes);
+      const int b_row = cta_rank * kBRows;
       const uint64_t mapA_hi = reinterpret_cast<uint64_t>(&p.tmA), mapB_hi = reinterpret_cast<uint64_t>(&p.tmB);
       const uint64_t mapA_lo = reinterpret_cast<uint64_t>(&p.tmA2), mapB_lo = reinterpret_cast<uint64_t>(&p.tmB2);
       constexpr bool split = SPLIT;          // pseudo-taps pick the hi / lo plane of either operand (tap[.][3])
@@ -339,22 +316,22 @@ __global__ void __launch_bounds__(64 + 128 * EG, 1) igemm_kernel(const __grid_co
               n_here = min(kps, left);
               mbar_wait(&empty_bar[stage], phase ^ 1);
               bar = full0 + 8u * stage;
-              if (CG == 1 || cta_rank == 0) mbar_expect_tx_a(bar, n_here * kit_tx);   // CG=2: leader counts both CTAs
+              mbar_expect_tx_a(bar, n_here * kit_tx);
               dst = smem_base + static_cast<uint32_t>(stage) * stage_bytes;
             }
-            if (rank5) tma_a_5d<CG == 2>(dst, mapA, bar, ac, cz, cx, cy, t.b);
-            else tma_a_4d<CG == 2>(dst, mapA, bar, ac, cx, cy, t.b);
+            if (rank5) tma_a_5d(dst, mapA, bar, ac, cz, cx, cy, t.b);
+            else tma_a_4d(dst, mapA, bar, ac, cx, cy, t.b);
             uint32_t bdst = dst + a_sub;
             for (int ky = 0; ky < ny; ++ky) {
               int tap = ky * nx + kx;
               const uint64_t mapB = (split && (p.tap[tap][3] & 2)) ? mapB_lo : mapB_hi;
               if (split) tap = p.tap_b[tap];
-              if constexpr (CL > 1 && CG == 1) {
+              if constexpr (CL > 1) {
                 if (banded) tma_a_3d_mc(bdst + b_off, mapB, bar, kMask, 0, b_row, tap * kblocks + kb);
                 else tma_a_3d_mc(bdst + b_off, mapB, bar, kMask, bk, bn0, tap);
               } else {
-                if (banded) tma_a_3d<CG == 2>(bdst, mapB, bar, 0, b_row, tap * kblocks + kb);
-                else tma_a_3d<CG == 2>(bdst, mapB, bar, bk, bn0, tap);
+                if (banded) tma_a_3d(bdst, mapB, bar, 0, 0, tap * kblocks + kb);
+                else tma_a_3d(bdst, mapB, bar, bk, bn0, tap);
               }
               bdst += b_sub;
             }
@@ -367,310 +344,137 @@ __global__ void __launch_bounds__(64 + 128 * EG, 1) igemm_kernel(const __grid_co
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (one thread; leader CTA only for CG=2)
-    if ((CG == 1 || cta_rank == 0) && elect_one()) {
-      const uint32_t idesc = make_idesc_f16(CG * kTileM, BN, p.ab_fmt);
-      const uint32_t idesc_half = make_idesc_f16(CG * kTileM, BN / 2, p.ab_fmt);   // edge K blocks of a banded filter
-      const bool band_half = p.band_half != 0;
-      const int kblocks = p.kblocks;
-      const int mma_per_kit = p.row_bytes >> 5;  // 32 B (= 16 elements, UMMA_K) per instruction
-      const int kps = p.kps, stages = p.stages;
-      // descriptor = constant high part | (smem address >> 4); all operand buffers are 1024-byte aligned
-      const uint64_t desc_hi = make_smem_desc(0, p.row_bytes);
-      const uint32_t base16 = (smem_u32(smem) & 0x3FFFFu) >> 4;
-      const uint32_t stage16 = static_cast<uint32_t>(stage_bytes) >> 4, sub16 = static_cast<uint32_t>(sub_bytes) >> 4;
-      const uint32_t a16 = static_cast<uint32_t>(p.a_sub_bytes) >> 4, b16 = static_cast<uint32_t>(p.b_sub_bytes) >> 4;
-      const uint32_t ady16 = static_cast<uint32_t>(p.BD * p.BW * p.row_bytes) >> 4;   // one image row of the A halo
-      const uint32_t ams16 = static_cast<uint32_t>(kTileM * p.row_bytes) >> 4;          // one M sub-tile (BH image rows)
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int ct = cl_id; ct < num_ct; ct += ncl) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * ms * BN);
-        uint32_t accum = 0;
-        int kbi = 0;                                // K block (in processing order) of the current group
-        for (int left = total_k; left > 0;) {
-          const int n_here = min(kps, left);
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          uint64_t da = desc_hi | static_cast<uint64_t>(base16 + static_cast<uint32_t>(stage) * stage16);
-          for (int j = 0; j < n_here; ++j) {
-            uint64_t dak = da, dbk = da + a16;
-            // banded filter: an edge K block feeds only half of the N tile -> N = BN/2 MMAs on that half of the accumulator
-            // (its packed tile holds the needed rows first; the very first block of a tile is always a full one)
-            const uint32_t half = band_half ? p.kb_half[kbi] : 0u;
-            const uint32_t id_j = half ? idesc_half : idesc;
-            const uint32_t d_j = d_tmem + (half == 2u ? static_cast<uint32_t>(BN / 2) : 0u);
-            if (++kbi == kblocks) kbi = 0;
-            for (int ky = 0; ky < ny; ++ky) {       // operand ky = the halo shifted down by ky image rows
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                if (k < mma_per_kit) {
-                  umma_f16<CG>(d_j, dak + 2 * k, dbk + 2 * k, id_j, accum);
-                  if constexpr (MS == 2)   // second accumulator, same weight operand
-                    umma_f16<CG>(d_j + BN, dak + ams16 + 2 * k, dbk + 2 * k, id_j, accum);
-                  accum = 1;
-                }
-              }
-              dak += ady16;
-              dbk += b16;
-            }
-            da += sub16;
-          }
-          // frees the smem slot (in every CTA of the cluster: their multicasts write into ours) once these MMAs retire
-          if constexpr (CG == 2) umma_commit<2>(&empty_bar[stage]);
-          else if constexpr (CL == 1) umma_commit<1>(&empty_bar[stage]);
-          else umma_commit_mc(&empty_bar[stage], static_cast<uint16_t>((1u << CL) - 1u));
-          left -= n_here;
-          if (++stage == stages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit<CG>(&tfull_bar[acc]);     // accumulator complete -> epilogue (of both CTAs for CG=2)
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
   } else {
-    // ------------------------------------------------------------ epilogue warps (TMEM lane quadrant = warp % 4)
-    const int quad = warp & 3;
-    const int m = quad * 32 + lane;
+    setmaxnreg_inc<232>();
+    // ------------------------------------------------------------ consumers: MMAs of 64 rows, then their epilogue
+    const int wg = (warp - 4) >> 2;                 // rows [64 wg, 64 wg + 64) of every M sub-tile
+    const int wtid = threadIdx.x - 128 * (1 + wg);
+    const int bf16 = p.ab_fmt;
+    const int kblocks = p.kblocks;
+    const int mma_per_kit = p.row_bytes >> 5;       // 32 B (= 16 elements) per k-step
+    const int kps = p.kps, stages = p.stages;
+    // descriptor = constant high part | (smem address >> 4); all operand buffers are 1024-byte aligned
+    const uint64_t desc_hi = make_smem_desc(0, p.row_bytes);
+    const uint32_t base16 = (smem_u32(smem) & 0x3FFFFu) >> 4;
+    const uint32_t stage16 = static_cast<uint32_t>(stage_bytes) >> 4, sub16 = static_cast<uint32_t>(sub_bytes) >> 4;
+    const uint32_t a16 = static_cast<uint32_t>(p.a_sub_bytes) >> 4, b16 = static_cast<uint32_t>(p.b_sub_bytes) >> 4;
+    const uint32_t ady16 = static_cast<uint32_t>(p.BD * p.BW * p.row_bytes) >> 4;   // one image row of the A halo
+    const uint32_t ams16 = static_cast<uint32_t>(kTileM * p.row_bytes) >> 4;          // one M sub-tile (BH image rows)
+    const uint32_t awg16 = static_cast<uint32_t>(64 * wg * p.row_bytes) >> 4;          // this warpgroup's 64 rows
+    const uint32_t bhalf16 = static_cast<uint32_t>((BN / 2) * p.row_bytes) >> 4;        // rows [BN/2, BN) of a B tile
+    // epilogue mapping: fragment rows fr, fr + 8 (columns fc, fc + 1 of every 8-column block) are written to the staging
+    // panel; thread wtid then reads row er, columns ec..ec+15 of it back and stores them
+    float* stg = stg_all + wg * 64 * kStgStride;
+    const int fr = 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);
+    const int er = wtid / TPR, ec = (wtid % TPR) * 16;
+    const int m = 64 * wg + er;
     const int zl = m % p.BD;
     const int xl = (m / p.BD) % p.BW;
     const int yl = m / (p.BD * p.BW);
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    if constexpr (EG == 2) {
-      // ---------------------------------------------------------- two warp groups, one 64-column panel per tcgen05.ld
-      constexpr int PC = (BN >= 64) ? 64 : BN;        // panel = TMEM load = staging buffer = TMA store box
-      constexpr int NPT = BN / PC;                    // panels per accumulator
-      constexpr int RV = PC / 8;
-      constexpr int NQ = MS * NPT;                    // panels per tile
-      constexpr int PER = NQ >= 2 ? NQ / 2 : NQ;      // panels per group (a lone panel goes to group 0)
-      const int grp = (warp - 2) >> 2;
-      const int q_lo = grp * PER, q_hi = (NQ >= 2) ? q_lo + PER : (grp == 0 ? 1 : 0);
-      const int bar_id = 1 + grp;
-      const uint32_t stg = stg_base + static_cast<uint32_t>(grp) * (kTileM * PC * 2);
-      const bool leader = ((warp - 2) & 3) == 0 && lane == 0;
-      const bool tma_out = p.tma_store != 0;
-      const uint64_t mapO = reinterpret_cast<uint64_t>(&p.tmO);
-      for (int ct = cl_id; ct < num_ct; ct += ncl) {
-        const TileCoord t = decode_tile(p, tile_of(ct), BN);
-        const int x = t.x0 + xl, z = t.z0 + zl;
-        if (p.res_l2_prefetch && warp == 2 && lane == 0) {   // next tile's residual rows: HBM -> L2 a whole tile ahead
-          const uint64_t mapR = reinterpret_cast<uint64_t>(&p.tmR);
-          auto l2_prefetch_tile = [&](const TileCoord& tt) {
-            for (int s = 0; s < ms; ++s)
-#pragma unroll
-              for (int pc = 0; pc < BN; pc += PC) tma_prefetch_l2_4d(mapR, tt.n0 + pc, tt.x0, tt.y0 + s * p.BH, tt.b);
-          };
-          if (ct == cl_id) l2_prefetch_tile(t);
-          if (ct + ncl < num_ct) l2_prefetch_tile(decode_tile(p, tile_of(ct + ncl), BN));
-        }
-        const bool want_pre = p.res_prefetch && !SPLIT && (p.res != nullptr) && !p.res_is_f32 && p.vec_ok && (p.o_nsplit == 0) &&
-                              (t.n0 + BN <= p.n_valid);
-        auto drain = [&](auto pre_tag) {
-          constexpr bool res_pre = decltype(pre_tag)::value;
-          uint4 res[res_pre ? RV : 1];
-#pragma unroll
-          for (int i = 0; i < (res_pre ? RV : 1); ++i) res[i] = make_uint4(0u, 0u, 0u, 0u);
-          auto prefetch_res = [&](int q) {
-            const int y = t.y0 + (q / NPT) * p.BH + yl;
-            if (x < p.W && y < p.H && z < p.D) {
-              const long long o = p.o_base + t.b * p.o_b + y * p.o_y + x * p.o_x + z * p.o_z + t.n0 + (q % NPT) * PC;
-              const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.res) + o);
-#pragma unroll
-              for (int i = 0; i < (res_pre ? RV : 1); ++i) res[i] = __ldg(rp + i);
-            }
-          };
-          if constexpr (res_pre) { if (q_lo < q_hi) prefetch_res(q_lo); }
-          mbar_wait(&tfull_bar[acc], acc_phase);
-          tc_fence_after();
-          auto release = [&]() {     // this warp has read all it will read of the tile's accumulators
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if (CG == 2 && cta_rank != 0) mbar_arrive_cluster(&tempty_bar[acc], 0);   // leader owns the barrier
-              else mbar_arrive(&tempty_bar[acc]);
-            }
-          };
-          if (q_lo >= q_hi) release();
-#pragma unroll 1
-          for (int q = q_lo; q < q_hi; ++q) {
-            const int s = q / NPT, pc = (q % NPT) * PC;
-            const int ys0 = t.y0 + s * p.BH, y = ys0 + yl;
-            const bool row_valid = (x < p.W) && (y < p.H) && (z < p.D);
-            const long long off = p.o_base + t.b * p.o_b + y * p.o_y + x * p.o_x + z * p.o_z;
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) +
-                                   static_cast<uint32_t>((acc * ms + s) * BN + pc);
-            uint32_t r[PC];
-            if constexpr (PC == 64) tmem_ld_32x32b_x64(taddr, r);
-            else if constexpr (PC == 32) tmem_ld_32x32b_x32(taddr, r);
-            else tmem_ld_32x32b_x16(taddr, r);
-            tmem_ld_wait();
-            if (q == q_hi - 1) release();
-            if (!tma_out) {
-#pragma unroll
-              for (int c = 0; c < PC; c += CW) {
-                const int nc = t.n0 + pc + c;
-                const long long offc = p.o_nsplit > 0 ? off + (nc / p.o_nsplit) * p.o_nhi + (nc % p.o_nsplit) - nc : off;
-                epilogue_chunk<CW, SPLIT>(p, r + c, nc, offc, row_valid, 0, 0, 0, 128, res_pre ? res + c / 8 : nullptr, t.b);
-              }
-              if constexpr (res_pre) { if (q + 1 < q_hi) prefetch_res(q + 1); }
-            } else {
-              named_bar_sync(bar_id, 128);               // this group's previous store has finished reading its staging buffer
-#pragma unroll
-              for (int c = 0; c < PC; c += CW)
-                epilogue_chunk<CW, SPLIT>(p, r + c, t.n0 + pc + c, off, row_valid, stg, m, c / 8, PC * 2,
-                                   res_pre ? res + c / 8 : nullptr);
-              if constexpr (res_pre) { if (q + 1 < q_hi) prefetch_res(q + 1); }
-              fence_proxy_async();
-              named_bar_sync(bar_id, 128);               // panel complete and visible to the async proxy
-              if (leader) {
-                const int ncol = t.n0 + pc;
-                if (p.tma_store == 2) tma_store_5d(mapO, stg, ncol % p.o_nsplit, t.x0, ncol / p.o_nsplit, ys0, t.b);
-                else tma_store_4d(mapO, stg, ncol, t.x0, ys0, t.b);
-                tma_store_commit();
-                tma_store_wait_read();
-              }
-            }
-          }
-        };
-        if (want_pre) drain(std::true_type{});
-        else drain(std::false_type{});
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
+    const int bar_id = 1 + wg;
+    float acc[MS][NP][NACC];
+    int stage = 0;
+    uint32_t phase = 0;
+    // frees smem stage s in every CTA of the cluster (their multicasts write into ours) once its MMAs have retired
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) {
+        if constexpr (CL == 1) mbar_arrive(&empty_bar[s]);
+        else
+          for (int c = 0; c < CL; ++c) mbar_arrive_cluster(&empty_bar[s], static_cast<uint32_t>(c));
       }
-      if (p.tma_store && leader) tma_store_wait_all();
-    } else {
+    };
     for (int ct = cl_id; ct < num_ct; ct += ncl) {
+      int prev = -1;                                // stage whose wgmma group may still be in flight
+      uint32_t scale_d = 0;
+      int kbi = 0;                                  // K block (in processing order) of the current group
+      for (int left = total_k; left > 0;) {
+        const int n_here = min(kps, left);
+        mbar_wait(&full_bar[stage], phase);
+        wgmma_fence();
+        uint32_t da = base16 + static_cast<uint32_t>(stage) * stage16;
+        for (int j = 0; j < n_here; ++j) {
+          uint64_t dak = desc_hi | (da + awg16), dbk = desc_hi | (da + a16);
+          // banded filter: an edge K block feeds only half of the N tile -> only that half's MMA (its packed tile holds the
+          // needed rows first; the very first block of a tile is always a full one)
+          const uint32_t half = HALF ? p.kb_half[kbi] : 0u;
+          if (++kbi == kblocks) kbi = 0;
+          for (int ky = 0; ky < ny; ++ky) {       // operand ky = the halo shifted down by ky image rows
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              if (k < mma_per_kit) {
+#pragma unroll
+                for (int s = 0; s < MS; ++s) {
+                  const uint64_t a = dak + s * ams16 + 2 * k, b = dbk + 2 * k;
+                  if constexpr (!HALF) {
+                    wgmma_ss<BN>(acc[s][0], a, b, scale_d, bf16);
+                  } else {
+                    if (half != 2) wgmma_ss<BN / 2>(acc[s][0], a, b, scale_d, bf16);
+                    if (half == 0) wgmma_ss<BN / 2>(acc[s][1], a, b + bhalf16, scale_d, bf16);
+                    else if (half == 2) wgmma_ss<BN / 2>(acc[s][1], a, b, scale_d, bf16);
+                  }
+                }
+                scale_d = 1;
+              }
+            }
+            dak += ady16;
+            dbk += b16;
+          }
+          da += sub16;
+        }
+        // one group stays in flight: the previous stage is released once its MMAs have retired
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) release(prev);
+        prev = stage;
+        left -= n_here;
+        if (++stage == stages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      release(prev);
+      // epilogue: accumulator fragments -> staging panel (SC columns at a time) -> one row per thread -> epilogue_chunk
       const TileCoord t = decode_tile(p, tile_of(ct), BN);
       const int x = t.x0 + xl, z = t.z0 + zl;
-      // TMEM is read SC columns at a time (every tcgen05.ld queues behind the MMAs already issued for the next tile and
-      // costs ~2000 cycles whatever its width -- fewer, wider loads: x128), then drained panel by panel: one panel =
-      // PC columns = one swizzled staging buffer = one TMA store.  A 16-bit residual is fetched one panel AHEAD into
-      // registers (the first panel's before the accumulator-full wait), all 128 bytes of the row at once, so its L2
-      // latency overlaps the store / barrier / next TMEM load instead of stalling every 32-column chunk.
-      constexpr int SC = (BN >= 128) ? 128 : BN;
-      constexpr int PC = (BN >= 64) ? 64 : BN;        // staging panel columns (one TMA store box)
-      constexpr int NPT = BN / PC;                    // panels per accumulator
-      constexpr int RV = PC / 8;                      // 16-byte residual vectors per row and panel
-      const int nq = ms * NPT;
-      const bool tma_out = p.tma_store != 0;
-      const uint64_t mapO = reinterpret_cast<uint64_t>(&p.tmO);
-      // HBM -> L2 prefetch of the residual rows of the NEXT tile of this CTA (and of the first tile at start-up): the
-      // register prefetch below is only one 64-column panel deep, enough for L2 latency but not for DRAM latency.
-      if (p.res_l2_prefetch && warp == 2 && lane == 0) {
-        const uint64_t mapR = reinterpret_cast<uint64_t>(&p.tmR);
-        constexpr int PCR = (BN >= 64) ? 64 : BN;
-        auto l2_prefetch_tile = [&](const TileCoord& tt) {
-          for (int s = 0; s < ms; ++s)
 #pragma unroll
-            for (int pc = 0; pc < BN; pc += PCR) tma_prefetch_l2_4d(mapR, tt.n0 + pc, tt.x0, tt.y0 + s * p.BH, tt.b);
-        };
-        if (ct == cl_id) l2_prefetch_tile(t);
-        if (ct + ncl < num_ct) l2_prefetch_tile(decode_tile(p, tile_of(ct + ncl), BN));
-      }
-      const bool want_pre = p.res_prefetch && !SPLIT && (p.res != nullptr) && !p.res_is_f32 && p.vec_ok && (p.o_nsplit == 0) &&
-                            (t.n0 + BN <= p.n_valid);
-      // Two copies of the drain loop, selected per tile: the one without a residual keeps no prefetch registers alive
-      // (the 1x1 projection kernel is epilogue-bound and measurably slower with them: profiles/r01_ab_oldnew.log).
-      auto drain = [&](auto pre_tag) {
-      constexpr bool res_pre = decltype(pre_tag)::value;
-      uint4 res[res_pre ? RV : 1];
-#pragma unroll
-      for (int i = 0; i < (res_pre ? RV : 1); ++i) res[i] = make_uint4(0u, 0u, 0u, 0u);
-      auto prefetch_res = [&](int q) {                // panel q -> M sub-tile q / NPT, columns (q % NPT) * PC
-        const int y = t.y0 + (q / NPT) * p.BH + yl;
-        if (x < p.W && y < p.H && z < p.D) {
-          const long long o = p.o_base + t.b * p.o_b + y * p.o_y + x * p.o_x + z * p.o_z + t.n0 + (q % NPT) * PC;
-          const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.res) + o);
-#pragma unroll
-          for (int i = 0; i < (res_pre ? RV : 1); ++i) res[i] = __ldg(rp + i);
-        }
-      };
-      if constexpr (res_pre) prefetch_res(0);
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      int q = 0;                                      // running panel index
-#pragma unroll 1
-      for (int s = 0; s < ms; ++s) {                  // M sub-tiles: BH image rows further down, BN TMEM columns further on
-        const int ys0 = t.y0 + s * p.BH, y = ys0 + yl;
-        const bool row_valid = (x < p.W) && (y < p.H) && (z < p.D);
+      for (int s = 0; s < MS; ++s) {
+        const int y = t.y0 + s * p.BH + yl;
+        const bool row_valid = (er < 64) && (x < p.W) && (y < p.H) && (z < p.D);
         const long long off = p.o_base + t.b * p.o_b + y * p.o_y + x * p.o_x + z * p.o_z;
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + static_cast<uint32_t>((acc * ms + s) * BN);
-#pragma unroll 1
-        for (int sc = 0; sc < BN; sc += SC) {
-          uint32_t r[SC];
-          if constexpr (SC == 128) tmem_ld_32x32b_x128(taddr + sc, r);
-          else if constexpr (SC == 64) tmem_ld_32x32b_x64(taddr + sc, r);
-          else if constexpr (SC == 32) tmem_ld_32x32b_x32(taddr + sc, r);
-          else tmem_ld_32x32b_x16(taddr + sc, r);
-          tmem_ld_wait();
-          if (sc + SC >= BN && s == ms - 1) {  // all TMEM reads of this tile's accumulators are done -> hand them back
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if (CG == 2 && cta_rank != 0) mbar_arrive_cluster(&tempty_bar[acc], 0);   // leader owns the barrier
-              else mbar_arrive(&tempty_bar[acc]);
-            }
+#pragma unroll
+        for (int c0 = 0; c0 < BN; c0 += SC) {
+          named_bar_sync(bar_id, 128);              // the previous pass has read the staging panel
+#pragma unroll
+          for (int jj = 0; jj < SC / 8; ++jj) {
+            const int j = c0 / 8 + jj;
+            const float* d = acc[s][j / JP] + 4 * (j % JP);
+            *reinterpret_cast<float2*>(stg + fr * kStgStride + 8 * jj + fc) = make_float2(d[0], d[1]);
+            *reinterpret_cast<float2*>(stg + (fr + 8) * kStgStride + 8 * jj + fc) = make_float2(d[2], d[3]);
           }
+          named_bar_sync(bar_id, 128);
+          if (row_valid) {
+            float a[16];
+            const float4* sp = reinterpret_cast<const float4*>(stg + er * kStgStride + ec);
 #pragma unroll
-          for (int pc = 0; pc < SC; pc += PC) {
-            if (!tma_out) {
-#pragma unroll
-              for (int c = 0; c < PC; c += CW) {
-                const int nc = t.n0 + sc + pc + c;
-                const long long offc = p.o_nsplit > 0 ? off + (nc / p.o_nsplit) * p.o_nhi + (nc % p.o_nsplit) - nc : off;
-                epilogue_chunk<CW, SPLIT>(p, r + pc + c, nc, offc, row_valid, 0, 0, 0, 128, res_pre ? res + c / 8 : nullptr, t.b);
-              }
-              ++q;
-              if constexpr (res_pre) { if (q < nq) prefetch_res(q); }
-            } else {
-              // registers -> swizzled smem -> one TMA store (full 128-byte lines, edges clipped by TMA)
-              named_bar_sync(1, 128);                    // the previous panel's store has finished reading the staging buffer
-#pragma unroll
-              for (int c = 0; c < PC; c += CW)
-                epilogue_chunk<CW, SPLIT>(p, r + pc + c, t.n0 + sc + pc + c, off, row_valid, stg_base, m, c / 8, PC * 2,
-                                   res_pre ? res + c / 8 : nullptr);
-              ++q;
-              if constexpr (res_pre) { if (q < nq) prefetch_res(q); }   // next panel's residual: in flight across the store + barrier
-              fence_proxy_async();
-              named_bar_sync(1, 128);                    // panel complete and visible to the async proxy
-              if (warp == 2 && lane == 0) {
-                const int ncol = t.n0 + sc + pc;
-                if (p.tma_store == 2)   // merged stride-2 transposed conv: n = (ay, ax, co) -> "TMA scatter" into row 2y+ay
-                  tma_store_5d(mapO, stg_base, ncol % p.o_nsplit, t.x0, ncol / p.o_nsplit, ys0, t.b);
-                else
-                  tma_store_4d(mapO, stg_base, ncol, t.x0, ys0, t.b);
-                tma_store_commit();
-                tma_store_wait_read();                   // staging buffer may be overwritten after this
-              }
+            for (int i = 0; i < 4; ++i) {
+              const float4 q = sp[i];
+              a[4 * i] = q.x; a[4 * i + 1] = q.y; a[4 * i + 2] = q.z; a[4 * i + 3] = q.w;
             }
+            const int nc = t.n0 + c0 + ec;
+            const long long offc = p.o_nsplit > 0 ? off + (nc / p.o_nsplit) * p.o_nhi + (nc % p.o_nsplit) - nc : off;
+            epilogue_chunk<16, SPLIT>(p, a, nc, offc, true, t.b);
           }
         }
       }
-      };
-      if (want_pre) drain(std::true_type{});
-      else drain(std::false_type{});
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
-    if (p.tma_store && warp == 2 && lane == 0) tma_store_wait_all();
-    }   // EG == 1
   }
 
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CL > 1) cluster_sync();   // no CTA exits while a peer may still multicast into / commit to it
-  if (warp == 1) tmem_dealloc<CG>(tmem_base, kTmemCols);
+  if constexpr (CL > 1) cluster_sync();   // no CTA exits while a peer may still multicast into / arrive on it
 }
 
 // One explicit instantiation per kernel variant lives in its own object file (rn_igemm_inst.cu compiled with
 // -DRN_BN=.. etc., see the Makefile's VARIANTS list); rn_igemm.cu holds the matching dispatch table.
-template <int BN, int CL, int CG, int MS, int EG, bool SPLIT>
+template <int BN, int CL, int MS, bool SPLIT, bool HALF>
 cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t stream) {
   // cudaFuncSetAttribute is per DEVICE (and per kernel variant): one flag per device ordinal
   static std::atomic<bool> attr_set[kMaxDevices];
@@ -678,7 +482,7 @@ cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t 
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
   if (!attr_set[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(igemm_kernel<BN, CL, CG, MS, EG, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
+    cudaError_t e = cudaFuncSetAttribute(igemm_kernel<BN, CL, MS, SPLIT, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e != cudaSuccess) return e;
     attr_set[dev].store(true, std::memory_order_release);
   }
@@ -686,7 +490,7 @@ cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t 
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(64 + 128 * EG);
+  cfg.blockDim = dim3(kNumThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
@@ -705,7 +509,7 @@ cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t 
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  return cudaLaunchKernelEx(&cfg, igemm_kernel<BN, CL, CG, MS, EG, SPLIT>, p);
+  return cudaLaunchKernelEx(&cfg, igemm_kernel<BN, CL, MS, SPLIT, HALF>, p);
 }
 
 }  // namespace rn

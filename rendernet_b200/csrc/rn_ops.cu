@@ -239,33 +239,25 @@ __global__ void cast_16_to_f32_kernel(const uint16_t* __restrict__ s, float* __r
 
 
 // ------------------------------------------------------------------------------------------ banded conv3d filter
-// Wb[arr][tap=(ky,kx)][i][n'][k = zi_l*Cin + ci]: K block i of the processing order is block kb = order[i] of the band.
+// Wb[tap=(ky,kx)][i][n'][k = zi_l*Cin + ci]: K block i of the processing order is block kb = order[i] of the band.
 // Relative to the N tile's first output depth z0: zi = sz*z0 - pz + kb*(64/Cin) + zi_l, zo = z0 + zo_l
 //   ->  kz = zi - (sz*zo - pz) = kb*(64/Cin) + zi_l - sz*zo_l;  entry = w[ky][kx][kz][ci][co] when 0 <= kz < 3, else 0.
 // Row n' of a tile holds filter row n = zo_l*Cout + co.  Full blocks: n = n'.  Half blocks (they feed only columns
 // [base, base+64) of the tile, base = 0 or 64; rn_igemm.cuh band_layout) keep the needed rows FIRST so that an N = 64 MMA finds
-// them at the start of the operand: arrangement 0 (single CTA holds all 128 rows): n = base + n' for n' < 64;
-// arrangement 1 (cta_group::2, CTA r holds rows [64r, 64r+64) and supplies columns [32r, 32r+32) of the N = 64 MMA):
-// n = base + 32r + i for n' = 64r + i, i < 32.  Unused rows are zero.   (BN = 128, KB = 64; sz = z stride)
+// them at the start of the operand: n = base + n' for n' < 64.  Unused rows are zero.   (BN = 128, KB = 64; sz = z stride)
 __global__ void pack_banded_kernel(const float* __restrict__ w, uint16_t* __restrict__ packed, int Cin, int Cout,
                                    BandLayout L, int sz, int fmt, long long plane) {
   const int kblocks = L.kblocks;
-  const long long per_arr = 9LL * kblocks * 128 * 64;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < 2 * per_arr;
+  const long long total = 9LL * kblocks * 128 * 64;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int arr = static_cast<int>(i / per_arr);
-    const long long r = i - arr * per_arr;
-    const int k = static_cast<int>(r % 64);
-    const int np = static_cast<int>((r / 64) % 128);
-    const int bi = static_cast<int>((r / (64 * 128)) % kblocks);
-    const int tap = static_cast<int>(r / (64LL * 128 * kblocks));
+    const int k = static_cast<int>(i % 64);
+    const int np = static_cast<int>((i / 64) % 128);
+    const int bi = static_cast<int>((i / (64 * 128)) % kblocks);
+    const int tap = static_cast<int>(i / (64LL * 128 * kblocks));
     const int kb = L.order[bi], half = L.half[bi];
     int n = np;
-    if (half != 0) {
-      const int base = half == 2 ? 64 : 0;
-      if (arr == 0) n = np < 64 ? base + np : -1;
-      else n = (np % 64) < 32 ? base + 32 * (np / 64) + (np % 64) : -1;
-    }
+    if (half != 0) n = np < 64 ? (half == 2 ? 64 : 0) + np : -1;
     float v = 0.f;
     if (n >= 0) {
       const int zi_l = k / Cin, ci = k % Cin, zo_l = n / Cout, co = n % Cout;
@@ -1001,7 +993,7 @@ __global__ void phong_kernel(const float* __restrict__ img, const float* __restr
   }
 }
 
-static inline int grid_for(long long n, int block, int cap = 148 * 32) {
+static inline int grid_for(long long n, int block, int cap = 132 * 32) {
   long long g = (n + block - 1) / block;
   return static_cast<int>(g < 1 ? 1 : (g > cap ? cap : g));
 }
@@ -1122,7 +1114,6 @@ static void apply_tuning(rn_conv_desc& d, const rn_tuning* t) {
   d.epi_groups = t->epilogue_groups; d.res_prefetch = t->res_prefetch; d.tma_store = t->tma_store;
 }
 static bool want_yhalo(const rn_tuning* t) { return (t != nullptr && t->yhalo != 0) ? t->yhalo > 0 : tuning().yhalo != 0; }
-static int want_epi_groups(const rn_tuning* t) { return (t != nullptr && t->epilogue_groups != 0) ? t->epilogue_groups : tuning().epi_groups; }
 
 extern "C" int rn_conv2d_same(const void* x, const void* w_packed, const float* bias, const float* alpha, int act,
                               const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H,
@@ -1270,13 +1261,13 @@ extern "C" long long rn_conv3d_banded_bytes(int Cin, int Cout, int sz) {
   if (!banded_ok(Cin, Cout, sz)) return -1;
   const BandLayout L = band_layout(Cin, Cout, sz);
   if (L.kblocks > 8) return -1;
-  return 2LL * 9LL * L.kblocks * 128 * 64 * 2;       // two arrangements (single CTA / CTA pair), 16-bit
+  return 9LL * L.kblocks * 128 * 64 * 2;             // 16-bit
 }
 
 extern "C" int rn_pack_conv3d_banded(const float* w, void* packed, int Cin, int Cout, int sz, int fmt, void* stream) {
   if (!w || !packed || rn_conv3d_banded_bytes(Cin, Cout, sz) < 0 || fmt < 0 || fmt > 2) return -1;
   const BandLayout L = band_layout(Cin, Cout, sz);
-  const long long total = 2LL * 9LL * L.kblocks * 128 * 64;
+  const long long total = 9LL * L.kblocks * 128 * 64;
   pack_banded_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       w, static_cast<uint16_t*>(packed), Cin, Cout, L, sz, fmt, total);
   RN_COUNT_LAUNCH();
@@ -1327,13 +1318,6 @@ extern "C" int rn_conv3d_banded_same(const void* x, const void* w_banded, const 
   }
   apply_tuning(d, tune);
   if (want_yhalo(tune)) d.ny = 3;
-  // With a residual the epilogue is the critical path of these short-K tiles, and the paired (cta_group::2) form couples
-  // the two CTAs' epilogues through the shared accumulator hand-over: multicast clusters of independent CTAs are 17 %
-  // faster there (0.296 vs 0.355 ms), while the PReLU-only convs prefer the pair (0.238 vs 0.270 ms);
-  // profiles/r01_probe_res1_cg.log.  Results are bit-identical either way.
-  // (With two epilogue warp groups the pair form drains fast enough again, so the override only applies to the
-  // single-group configuration.)
-  if (residual != nullptr && want_epi_groups(tune) == 1 && d.cta_group == 0) d.cta_group = 1;
   return rn_conv_igemm(&d, stream);
 }
 

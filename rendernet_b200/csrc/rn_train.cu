@@ -4,7 +4,7 @@
 //   * rn_conv_weight_grad_direct : weight gradient of ANY convolution or transposed convolution of the network (2-D or 3-D, any
 //     stride, TF SAME) as a strided correlation  dW[tap][a][b] = sum_p P[p][a] * Q[p*s + tap - pad][b]  on the CUDA cores, fp32
 //     accumulation.  The thin layers (e_conv1 / e_conv2, the transposed convs) go through it; the wide stride-1 2-D layers and
-//     the depth-folded 3^3 layers use the tcgen05 kernel of rn_wgrad.cu (97 % of the parameters, 90 % of the MACs).
+//     the depth-folded 3^3 layers use the wgmma kernel of rn_wgrad.cu (97 % of the parameters, 90 % of the MACs).
 //   * rn_prelu_alpha_grad        : dL/dalpha[c] = sum_{z<0} g * z  (tools/layer_util.py:27-45, alpha is initialised to 0, so the
 //     pre-activation z cannot be recovered from the stored output and is recomputed by the caller).
 //   * rn_dropout_16              : tf.nn.dropout (x / keep where a counter-based hash of (seed, layer, element) < keep, else 0);
@@ -245,7 +245,7 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
   }
 }
 
-inline int grid_for(long long n, int block, int cap = 148 * 16) {
+inline int grid_for(long long n, int block, int cap = 132 * 16) {
   long long g = (n + block - 1) / block;
   return static_cast<int>(g < 1 ? 1 : (g > cap ? cap : g));
 }
@@ -274,7 +274,7 @@ extern "C" int rn_conv_weight_grad_direct(const void* P, const void* Q, float* d
   p.b_tiles = (Cb + kTile - 1) / kTile;
   p.scale = scale;
   if ((Ca == 8 && Cb == 1) || (Ca == 16 && Cb == 3)) {               // thin layers: per-thread channel blocks, positions across threads
-    long long nsplit = (148LL * 8 + taps - 1) / taps;
+    long long nsplit = (132LL * 8 + taps - 1) / taps;
     const long long maxsplit = (p.npos + 255) / 256;
     if (nsplit > maxsplit) nsplit = maxsplit;
     if (nsplit < 1) nsplit = 1;
@@ -286,7 +286,7 @@ extern "C" int rn_conv_weight_grad_direct(const void* P, const void* Q, float* d
   }
   const long long tiles = taps * p.a_tiles * p.b_tiles;
   const long long nchunks = (p.npos + kChunk - 1) / kChunk;
-  long long nsplit = (148LL * 8 + tiles - 1) / tiles;               // ~8 CTAs per SM in flight
+  long long nsplit = (132LL * 8 + tiles - 1) / tiles;               // ~8 CTAs per SM in flight
   if (nsplit < 1) nsplit = 1;
   if (nsplit > nchunks) nsplit = nchunks;
   if (p.a_tiles * p.b_tiles > 65535) return -2;
@@ -323,7 +323,7 @@ extern "C" int rn_image_loss_grad(const float* img, const float* target, float* 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   cudaError_t e = cudaMemsetAsync(loss, 0, sizeof(double), st);
   if (e != cudaSuccess) return static_cast<int>(e);
-  image_loss_grad_kernel<<<grid_for(n, 256 * 8, 148 * 4), 256, 0, st>>>(img, target, dimg, loss, n, batch, kind);
+  image_loss_grad_kernel<<<grid_for(n, 256 * 8, 132 * 4), 256, 0, st>>>(img, target, dimg, loss, n, batch, kind);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }

@@ -1,18 +1,19 @@
-// rn_wgrad.cu -- weight gradient of a stride-1 SAME 2-D convolution on the 5th-gen tensor cores (backward pass, stage 2;
+// rn_wgrad.cu -- weight gradient of a stride-1 SAME 2-D convolution on the Hopper tensor cores (backward pass, stage 2;
 // the training step of RenderNet_Shader.py:159-167 differentiates every conv filter).
 //
 //   dW[tap][ci][co] = sum over pixels p of  x[p + off(tap)][ci] * g[p][co]              (x = layer input, g = dL/d(conv output))
 //
 // A GEMM per tap with M = ci, N = co and K = pixels.  Both operands are channel-last ([pixel][channel]), i.e. M/N-contiguous:
-// tcgen05.mma reads them as MN-MAJOR operands straight from what TMA delivers -- a box {64 channels, 64 pixels} lands as 64
+// wgmma reads them as MN-MAJOR (transposed) operands straight from what TMA delivers -- a box {64 channels, 64 pixels} lands as 64
 // rows of 128 bytes in the 128-byte swizzle, which is the canonical MN-major layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte
 // units: SBO = 1024 B between 8-pixel groups, LBO = 8192 B between the 64-channel boxes of a tile.  No transposed copy of the
 // activations is ever made.  The tap offset is a shifted TMA coordinate for x (zero fill outside the image = SAME padding).
 //
-// One CTA tile = (tap, 128 input channels, BN output channels), fp32 accumulator in TMEM; the K loop runs over pixel blocks of a
-// slice of the batch (split-K over CTAs when there are fewer tiles than SMs; partial results are combined with fp32 atomics
-// into a zero-initialised dW).  Warp 0 = TMA producer, warp 1 = MMA issuer, warps 2-5 = epilogue.  Exact mode (fmt 2): three
-// passes x_lo.g_hi, x_hi.g_lo, x_hi.g_hi into the same accumulator, corrections first (DESIGN.md §4).
+// One CTA tile = (tap, 128 input channels, BN output channels); the K loop runs over pixel blocks of a slice of the batch
+// (split-K over CTAs when there are fewer tiles than SMs; partial results are combined with fp32 atomics into a
+// zero-initialised dW).  Warpgroup 0 = TMA producer; warpgroups 1 and 2 each own 64 of the 128 input channels: m64nBNk16
+// wgmmas into fp32 register accumulators, then the stores of those rows.  Exact mode (fmt 2): three passes x_lo.g_hi,
+// x_hi.g_lo, x_hi.g_hi into the same accumulator, corrections first (DESIGN.md §4).
 #include <atomic>
 #include <cstdint>
 #include <cstring>
@@ -47,46 +48,38 @@ __device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr) {
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);            // start address
   d |= static_cast<uint64_t>(kBoxBytes >> 4) << 16;                   // LBO: next 64-channel box
   d |= static_cast<uint64_t>(1024 >> 4) << 32;                        // SBO: next group of 8 pixels
-  d |= static_cast<uint64_t>(1) << 46;                                // descriptor version (Blackwell)
-  d |= 2ull << 61;                                                    // SWIZZLE_128B
+  d |= wgmma_layout_code(128) << 62;                                  // SWIZZLE_128B
   return d;
 }
 
 template <int BN>
-__global__ void __launch_bounds__(192, 1) wgrad2d_kernel(const __grid_constant__ WgradParams p) {
+__global__ void __launch_bounds__(384, 1) wgrad2d_kernel(const __grid_constant__ WgradParams p) {
   constexpr int NBOX_B = BN / 64;
   constexpr int kStageBytes = (2 + NBOX_B) * kBoxBytes;
+  constexpr int NACC = BN / 2;                       // accumulator registers per consumer thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + static_cast<size_t>(p.stages) * kStageBytes);
   uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* acc_bar = empty_bar + p.stages;          // accumulator complete
-  uint64_t* free_bar = acc_bar + 1;                  // accumulator drained
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(free_bar + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmX);
     tma_prefetch_desc(&p.tmG);
     if (p.split) { tma_prefetch_desc(&p.tmX2); tma_prefetch_desc(&p.tmG2); }
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(acc_bar, 1);
-    mbar_init(free_bar, 4);
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<1>(tmem_slot, BN < 32 ? 32 : BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int bx = p.W / p.PX, by = p.H / p.PY;
   const int kb_per_img = bx * by;
   const int total_work = p.ntaps * p.m_tiles * p.n_tiles * p.ksplit;
   const int passes = p.split ? 3 : 1;
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
       int stage = 0; uint32_t phase = 0;
       for (int wk = blockIdx.x; wk < total_work; wk += gridDim.x) {
         const int ks = wk % p.ksplit; int t = wk / p.ksplit;
@@ -114,72 +107,60 @@ __global__ void __launch_bounds__(192, 1) wgrad2d_kernel(const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      // M = 128, N = BN, both operands MN-major (bits 15, 16), fp16 in, fp32 accumulate
-      const uint32_t idesc = make_idesc_f16(kWgBM, BN, 0) | (1u << 15) | (1u << 16);
-      int stage = 0; uint32_t phase = 0, free_phase = 0;
-      bool first_tile = true;
-      for (int wk = blockIdx.x; wk < total_work; wk += gridDim.x) {
-        const int ks = wk % p.ksplit;
-        const int b0 = (p.B * ks) / p.ksplit, b1 = (p.B * (ks + 1)) / p.ksplit;
-        const int nkb = (b1 - b0) * kb_per_img * passes;
-        if (!first_tile) { mbar_wait(free_bar, free_phase); free_phase ^= 1; }   // epilogue drained the previous tile
-        first_tile = false;
-        tc_fence_after();
-        uint32_t accum = 0;
-        for (int it = 0; it < nkb; ++it) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a0 = smem_u32(smem + static_cast<size_t>(stage) * kStageBytes);
-          const uint64_t da = make_smem_desc_mn(a0), db = make_smem_desc_mn(a0 + 2 * kBoxBytes);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {           // 64 pixels = 4 x (K = 16); 16 pixel rows = 2048 B further on
-            umma_f16<1>(tmem_base, da + static_cast<uint64_t>(k * (2048 >> 4)), db + static_cast<uint64_t>(k * (2048 >> 4)),
-                        idesc, accum);
-            accum = 1;
-          }
-          umma_commit<1>(&empty_bar[stage]);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit<1>(acc_bar);
-      }
-    }
   } else {
-    const int quad = warp & 3;                   // TMEM lane quadrant
-    const int m = quad * 32 + lane;              // accumulator row = input channel within the tile
-    uint32_t acc_phase = 0;
+    setmaxnreg_inc<232>();
+    // consumer warpgroup wg: input channels [64 wg, 64 wg + 64) of the tile = x box wg; M = 64, N = BN, both MN-major
+    const int wg = (warp - 4) >> 2;
+    const int fr = 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);   // accumulator fragment rows fr, fr+8
+    float acc[NACC];
+    int stage = 0; uint32_t phase = 0;
     for (int wk = blockIdx.x; wk < total_work; wk += gridDim.x) {
-      int t = wk / p.ksplit;
+      const int ks = wk % p.ksplit; int t = wk / p.ksplit;
       const int ni = t % p.n_tiles; t /= p.n_tiles;
       const int mi = t % p.m_tiles; const int tap = t / p.m_tiles;
-      mbar_wait(acc_bar, acc_phase);
-      acc_phase ^= 1;
-      tc_fence_after();
-      float* orow = p.dw + (static_cast<size_t>(tap) * p.Cin + (mi * kWgBM + m)) * p.Cout + ni * BN;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + static_cast<uint32_t>(c0), r);
-        tmem_ld_wait();
+      const int b0 = (p.B * ks) / p.ksplit, b1 = (p.B * (ks + 1)) / p.ksplit;
+      const int nkb = (b1 - b0) * kb_per_img * passes;
+      int prev = -1;                               // stage whose wgmma group may still be in flight
+      uint32_t scale_d = 0;
+      for (int it = 0; it < nkb; ++it) {
+        mbar_wait(&full_bar[stage], phase);
+        wgmma_fence();
+        const uint32_t a0 = smem_u32(smem + static_cast<size_t>(stage) * kStageBytes);
+        const uint64_t da = make_smem_desc_mn(a0 + wg * kBoxBytes), db = make_smem_desc_mn(a0 + 2 * kBoxBytes);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {             // 64 pixels = 4 x (K = 16); 16 pixel rows = 2048 B further on
+          wgmma_ss<BN, 1>(acc, da + static_cast<uint64_t>(k * (2048 >> 4)), db + static_cast<uint64_t>(k * (2048 >> 4)),
+                          scale_d, 0);
+          scale_d = 1;
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        __syncwarp();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == p.stages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      // rows = input channels, columns = output channels: d[4j..4j+1] at (fr, 8j+fc), d[4j+2..4j+3] at (fr+8, 8j+fc)
+      float* orow = p.dw + (static_cast<size_t>(tap) * p.Cin + (mi * kWgBM + 64 * wg + fr)) * p.Cout + ni * BN + fc;
+      const size_t down8 = static_cast<size_t>(8) * p.Cout;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
         if (p.ksplit == 1) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            *reinterpret_cast<float4*>(orow + c0 + i) = make_float4(__uint_as_float(r[i]), __uint_as_float(r[i + 1]),
-                                                                    __uint_as_float(r[i + 2]), __uint_as_float(r[i + 3]));
+          *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(orow + down8 + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) atomicAdd(orow + c0 + i, __uint_as_float(r[i]));
+          atomicAdd(orow + 8 * j, acc[4 * j]);
+          atomicAdd(orow + 8 * j + 1, acc[4 * j + 1]);
+          atomicAdd(orow + down8 + 8 * j, acc[4 * j + 2]);
+          atomicAdd(orow + down8 + 8 * j + 1, acc[4 * j + 3]);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(free_bar);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) tmem_dealloc<1>(tmem_base, BN < 32 ? 32 : BN);
 }
 
 template <int BN>
@@ -189,12 +170,12 @@ static cudaError_t launch_wgrad(const WgradParams& p, int grid, size_t smem, cud
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
   if (!attr_set[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad2d_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
+    cudaError_t e = cudaFuncSetAttribute(wgrad2d_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e != cudaSuccess) return e;
     attr_set[dev].store(true, std::memory_order_release);
   }
   g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  wgrad2d_kernel<BN><<<grid, 192, smem, st>>>(p);
+  wgrad2d_kernel<BN><<<grid, 384, smem, st>>>(p);
   return cudaGetLastError();
 }
 
@@ -243,7 +224,7 @@ extern "C" int rn_conv2d_weight_grad(const void* x, const void* g, float* dw, in
   while (tiles * ksplit < sms && ksplit * 2 <= B) ksplit *= 2;          // fewer tiles than SMs: split the batch over CTAs
   p.ksplit = ksplit;
   const int stage_bytes = (2 + BN / 64) * kBoxBytes;
-  p.stages = (232448 - 1024 - 256) / stage_bytes;
+  p.stages = (kMaxSmem - 1024 - 256) / stage_bytes;
   if (p.stages > 8) p.stages = 8;
   if (p.stages < 2) return -10;
   const size_t smem = static_cast<size_t>(p.stages) * stage_bytes + 1024 + 256;

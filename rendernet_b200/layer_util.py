@@ -1,5 +1,5 @@
 """Drop-in mirror of the reference's tools/layer_util.py (same function names, argument order, defaults and
-variable-scope naming), executing on the sm_100a kernels.  Citations are into /root/reference.
+variable-scope naming), executing on the sm_90a kernels.  Citations are into the reference RenderNet source tree.
 
 Differences that are deliberate and documented:
   * tensors are torch CUDA tensors (16-bit activations, fp32 accumulation) instead of tf.Tensor;

@@ -54,7 +54,7 @@ class PeerImageGather:
     exported to its peers over CUDA IPC at start-up; each step a rank writes its shard into every peer's buffer of that
     parity with plain device-to-device copies (copy engines over NVLink / NVSwitch) on a side stream.
 
-    An alternative to ncclAllGather that leaves all 148 SMs to the persistent convolution kernels of the next step (NCCL's
+    An alternative to ncclAllGather that leaves all SMs to the persistent convolution kernels of the next step (NCCL's
     kernels hold a few SMs while they run); `ShardedRenderEngine(gather="peer")` / `bench.py --gather peer`.
 
     Write-after-read safety across processes: a rank may only overwrite a peer's parity-p buffer with step i+2 after that
@@ -90,7 +90,7 @@ class PeerImageGather:
             self.peers.append(views)
         self.stream = torch.cuda.Stream(device=self.device)
         # one copy stream per destination: a single cudaMemcpyPeer stream moves ~115 GB/s on this fabric (one copy engine), the
-        # world-1 outgoing copies run concurrently on separate engines (profiles/r02_nccl_diag_8gpu.log)
+        # world-1 outgoing copies run concurrently on separate engines
         self.copy_streams = [torch.cuda.Stream(device=self.device) for _ in range(self.world)]
         self.done = torch.cuda.Event()
         self.done.record(torch.cuda.current_stream(self.device))
@@ -171,10 +171,8 @@ class ShardedRenderEngine:
     def __init__(self, engine, gather: str = "nccl_sync", group=None):
         """gather: "nccl_sync" (default) = ncclAllGather on the COMPUTE stream right after the step, straight from the engine's
         output buffer; "nccl" = the same collective on a side stream, overlapped with the next step; "peer" = copy-engine P2P
-        writes (PeerImageGather); "none".  Measured on 8 x B200 (DESIGN.md §7, profiles/r02_scale8*_*.json): all three cost
-        2.5-3.5 ms per step -- the bare 604 MB transfer is 0.94 ms, the rest is every rank waiting, each step, for the slowest of
-        eight power-capped GPUs; overlapping does not hide it because the persistent convolution kernels occupy every SM (NCCL's
-        CTAs only get SMs at kernel boundaries and slow every rank's compute by the same amount).  The stream-ordered form needs
+        writes (PeerImageGather); "none".  Overlapping the gather with the next step cannot hide much because the persistent
+        convolution kernels occupy every SM (NCCL's CTAs only get SMs at kernel boundaries).  The stream-ordered form needs
         no staging copy and no second gathered buffer in flight."""
         if gather not in ("nccl", "nccl_sync", "peer", "none"):
             raise ValueError("gather must be nccl_sync | nccl | peer | none")

@@ -1,4 +1,4 @@
-"""The training step of the Shader network (SURVEY §8 f-4, stage 2) -- RenderNet_Shader.py:154-167 on the B200 path:
+"""The training step of the Shader network (SURVEY §8 f-4, stage 2) -- RenderNet_Shader.py:154-167 on the H100 path:
 
     images_pred = RenderNet(rotated voxels, is_training=True, prob=cfg['keep_prob'])          (:156, dropout after ten layers)
     recon_loss  = BCE (greyscale, :159-161)  |  tf.losses.mean_squared_error (:163)
@@ -6,8 +6,8 @@
     tf.train.AdamOptimizer(learning_rate, beta1=0.5).minimize(recon_loss, global_step)       (:167)
 
 One `ShaderTrainer.step(voxels, view_params, target)` = forward with a tape (tensor-core convolutions, stateless hashed dropout)
--> loss + dL/dimage (rn_image_loss_grad) -> backward walk (rendernet_b200/backward.py: data gradients through the tcgen05
-implicit-GEMM kernel, weight gradients through the tcgen05 weight-gradient kernel / the strided-correlation kernel, bias and
+-> loss + dL/dimage (rn_image_loss_grad) -> backward walk (rendernet_b200/backward.py: data gradients through the wgmma
+implicit-GEMM kernel, weight gradients through the wgmma weight-gradient kernel / the strided-correlation kernel, bias and
 PReLU-slope reductions) -> rn_adam_step on every variable -> the kernel-ready packed copies of the filters are dropped and
 re-packed from the updated fp32 masters at the next forward.
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Timing of the tcgen05 weight-gradient kernel on the full-size trunk layer (3x3 1024->1024 @64x64, B=24): same algorithmic FLOPs
+"""Timing of the wgmma weight-gradient kernel on the full-size trunk layer (3x3 1024->1024 @64x64, B=24): same algorithmic FLOPs
 as the forward conv (1.855 TFLOP).  CUDA events on the launch stream, 10 back-to-back launches after 3 warm-ups."""
 import os, sys
 import torch

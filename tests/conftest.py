@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 # The CUDA extension is built in-tree (git-ignored).  A fresh checkout has no .so yet: build it once (nvcc
-# cross-compiles for sm_100a without a GPU) so that the host-side tests can load the C ABI.
+# cross-compiles for sm_90a without a GPU) so that the host-side tests can load the C ABI.
 _LIB = os.path.join(ROOT, "rendernet_b200", "librendernet_b200.so")
 if not os.path.exists(_LIB):
     import subprocess
@@ -19,7 +19,7 @@ if not os.path.exists(_LIB):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")

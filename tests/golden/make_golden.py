@@ -1,14 +1,14 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz by executing the REFERENCE'S OWN PYTHON SOURCE.
 
-Run in the build container only (needs /root/reference, which does not exist on the
-GPU box):   python tests/golden/make_golden.py
+Needs a checkout of the reference (thunguyenphuoc/RenderNet); the tests only read the
+stored fixtures:   python tests/golden/make_golden.py /path/to/RenderNet
 
 How: TensorFlow-1 is not installable here, so `oracle/tf1_shim.py` registers a NumPy
 stand-in for the ~50 TF primitives the hot path uses; the reference modules
 (`tools/resampling_voxel_grid.py`, `tools/model_util.py`, `tools/layer_util.py`,
 `tools/Phong_shading.py`, `tools/binvox_rw.py`, `RenderNet_demo.py`) are then imported
-unmodified from /root/reference, and the `RenderNet` model function is lifted out of
+unmodified from that checkout, and the `RenderNet` model function is lifted out of
 `RenderNet_Shader.py` with `ast` (that module trains at import time, so it cannot be
 imported) and executed over the shim.  No reference source is copied into this repo.
 
@@ -26,7 +26,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = "/root/reference"
+REF = sys.argv[1] if __name__ == "__main__" and len(sys.argv) > 1 else os.environ.get("RENDERNET_REFERENCE", "")
 sys.path.insert(0, ROOT)
 
 from oracle import tf1_shim  # noqa: E402

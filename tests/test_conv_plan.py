@@ -1,7 +1,7 @@
 """Launch-plan heuristics of the implicit-GEMM convolution (rn_conv_plan: pure host arithmetic, runs without a GPU).
-Pins the decisions the performance work arrived at for the BASELINE-size layers (DESIGN.md §3.1) so that a change to
-the sizing code cannot silently drop the trunk's halo sharing, the banded convs' second accumulator, or the second
-epilogue warp group of the projection unit -- and checks the argument validation of rn_conv_igemm's front end."""
+Pins the decisions the sizing code makes on the H100 (132 SMs, 227 KB of shared memory per block) for the BASELINE-size
+layers (DESIGN.md §3.1) so that a change to it cannot silently drop the banded convs' halo sharing, turn the (slower)
+weight multicast clusters on by default or drop the thin layers' second accumulator -- and checks the argument validation of rn_conv_igemm's front end."""
 import ctypes as C
 
 import pytest
@@ -40,27 +40,27 @@ def plan(ndim=2, B=24, H=64, W=64, D=1, Cin=1024, Cout=1024, cout_pad=None, k=3,
 
 def test_plan_trunk_and_projection():
     p = plan(Cin=1024, Cout=1024, k=3, ny=3)                       # res2 conv: the dominant kernel
-    assert (p["bn"], p["cluster"], p["cta_group"], p["msub"], p["ny"]) == (256, 2, 2, 1, 3)
-    assert (p["tile_w"], p["tile_h"]) == (16, 8) and p["stages"] >= 3 and p["epilogue_mode"] == 1
-    assert p["epilogue_groups"] == 1                               # a second staging buffer would cost the third stage
-    assert p["smem_bytes"] <= 232448 and p["grid"] == 148 and p["tiles"] == 24 * 4 * 8 * 4
-    assert plan(Cin=1024, Cout=1024, k=3, ny=3, residual=True)["epilogue_groups"] == 1
-    q = plan(Cin=1024, Cout=1024, k=1)                             # projection unit: 16 k-blocks per tile, epilogue-bound
-    assert (q["bn"], q["cta_group"], q["epilogue_groups"], q["ny"]) == (256, 2, 2, 1) and q["stages"] >= 3
+    # three full 256-row weight tiles per halo group would leave fewer than 3 stages: one activation load per tap
+    assert (p["bn"], p["cluster"], p["cta_group"], p["msub"], p["ny"]) == (256, 1, 1, 1, 1)
+    assert (p["tile_w"], p["tile_h"]) == (64, 2) and p["stages"] >= 3 and p["epilogue_mode"] == 0
+    assert p["epilogue_groups"] == 2                               # both consumer warpgroups store their own rows
+    assert p["smem_bytes"] <= 232448 and p["grid"] == 132 and p["tiles"] == 24 * 32 * 4
+    q = plan(Cin=1024, Cout=1024, k=1)                             # projection unit: 16 k-blocks per tile
+    assert (q["bn"], q["cluster"], q["ny"]) == (256, 1, 1) and q["stages"] >= 3
     r = plan(H=32, W=32, Cin=512, Cout=512, k=3, ny=3)             # res3
-    assert (r["bn"], r["cta_group"], r["ny"]) == (256, 2, 3) and r["stages"] >= 3
+    assert (r["bn"], r["cluster"]) == (256, 1) and r["stages"] >= 3
 
 
 def test_plan_banded_res1_and_thin_layers():
     # res1: depth-folded 3^3 conv, K per tap = 192 of the 1024 folded channels, N tile 128 (rn_conv3d_banded_same)
     kw = dict(Cin=192, Cout=1024, k=3, ny=3, force_bn=128, x_channels=1024, w_banded=1)
-    p = plan(**kw)
-    assert (p["bn"], p["cta_group"], p["msub"], p["epilogue_groups"], p["ny"]) == (128, 2, 2, 2, 3) and p["stages"] >= 3
-    assert (p["tile_w"], p["tile_h"]) == (16, 8) and p["tiles"] == 24 * 4 * 4 * 8      # 16x16-pixel CTA tiles
-    p1 = plan(cta_group=1, **kw)                                   # unpaired: full weight tile per CTA -> one accumulator
-    assert (p1["cluster"], p1["cta_group"], p1["msub"]) == (2, 1, 1) and p1["stages"] >= 3
+    p = plan(**kw)                                                 # a second accumulator would cost the third stage
+    assert (p["bn"], p["cluster"], p["msub"], p["ny"]) == (128, 1, 1, 3) and p["stages"] >= 3
+    assert (p["tile_w"], p["tile_h"]) == (16, 8) and p["tiles"] == 24 * 4 * 8 * 8      # 16x8-pixel CTA tiles
+    p1 = plan(cluster=2, **kw)                                     # per-call multicast cluster
+    assert (p1["cluster"], p1["msub"], p1["ny"]) == (2, 1, 3) and p1["stages"] >= 3
     assert plan(msub=1, **kw)["msub"] == 1
-    # x-folded e_conv11-like thin layer: N tile 16, two M sub-tiles, one epilogue group per sub-tile
+    # x-folded e_conv11-like thin layer: N tile 16, two M sub-tiles
     t = plan(H=512, W=128, Cin=64, Cout=16, k=1, taps=[(dx, dy, 0) for dy in (-2, -1, 0, 1) for dx in (-1, 0, 1)], ny=4)
     assert (t["bn"], t["cluster"], t["msub"], t["epilogue_groups"], t["ny"]) == (16, 1, 2, 2, 4)
     # tiny image: nothing to pair, halo sharing falls away when the pipeline would starve
@@ -70,8 +70,9 @@ def test_plan_banded_res1_and_thin_layers():
 
 def test_plan_tuning_switches_and_validation():
     # per-call overrides travel in the descriptor (the library has no mutable global state)
-    assert plan(Cin=1024, Cout=1024, k=1, epi_groups=1)["epilogue_groups"] == 1
+    assert plan(Cin=1024, Cout=1024, k=3, ny=3, cluster=4)["cluster"] == 4
     assert plan(Cin=1024, Cout=1024, k=3, ny=3, cta_group=1)["cta_group"] == 1
+    plan(Cin=1024, Cout=1024, k=3, cta_group=2, expect=-22)        # no paired (two-CTA) MMA on sm_90
     assert plan(Cin=1024, Cout=1024, k=3, ny=3, tma_store=-1)["epilogue_mode"] == 0
     assert plan(Cin=1024, Cout=1024, k=3, ny=3, out32=True)["epilogue_mode"] == 0      # fp32 output: direct stores
     plan(Cin=1000, expect=-4)                        # Cin % 16
@@ -85,18 +86,18 @@ def test_plan_tuning_switches_and_validation():
 
 
 def test_plan_exact_mode_split_operands():
-    """RN_FMT_F16X2: every tap becomes 3 pseudo-taps (x_hi.w_hi, x_lo.w_hi, x_hi.w_lo); split kernels exist for CTA pairs or
-    single CTAs with two epilogue groups, direct-store epilogue; the LO-plane offsets are mandatory."""
+    """RN_FMT_F16X2: every tap becomes 3 pseudo-taps (x_hi.w_hi, x_lo.w_hi, x_hi.w_lo); split kernels run on single CTAs
+    (no multicast cluster); the LO-plane offsets are mandatory."""
     planes = dict(fmt=2, x_plane=24 * 64 * 64 * 1024, w_plane=9 * 1024 * 1024, o_plane=24 * 64 * 64 * 1024)
     p = plan(Cin=1024, Cout=1024, k=3, ny=3, **planes)
-    assert (p["bn"], p["cluster"], p["cta_group"], p["epilogue_groups"], p["ny"], p["epilogue_mode"]) == (256, 2, 2, 2, 3, 0)
+    assert (p["bn"], p["cluster"], p["cta_group"], p["epilogue_mode"]) == (256, 1, 1, 0)
     assert p["stages"] >= 3 and p["smem_bytes"] <= 232448
     q = plan(Cin=1024, Cout=1024, k=1, **planes)
-    assert (q["bn"], q["cta_group"], q["epilogue_groups"]) == (256, 2, 2)
+    assert (q["bn"], q["cluster"]) == (256, 1)
     b = plan(Cin=192, Cout=1024, k=3, ny=3, force_bn=128, x_channels=1024, w_banded=1, **planes)
-    assert (b["bn"], b["cta_group"], b["msub"], b["epilogue_groups"], b["ny"]) == (128, 2, 2, 2, 3)
+    assert (b["bn"], b["cluster"], b["msub"], b["ny"]) == (128, 1, 1, 3)
     odd = plan(B=1, H=24, W=8, Cin=64, Cout=256, k=3, fmt=2, x_plane=8 * 24 * 64, w_plane=9 * 256 * 64, o_plane=8 * 24 * 256)
-    assert (odd["cluster"], odd["cta_group"], odd["epilogue_groups"]) in ((1, 1, 2), (2, 2, 2))
+    assert (odd["cluster"], odd["cta_group"]) == (1, 1)
     k4 = plan(Cin=64, Cout=64, k=4, taps=[(kx - 1, ky - 1, 0) for ky in range(4) for kx in range(4)], fmt=2,
               x_plane=24 * 64 * 64 * 64, w_plane=16 * 64 * 64, o_plane=24 * 64 * 64 * 64)       # 16 taps x 3 = 48 pseudo-taps
     assert k4["stages"] >= 2

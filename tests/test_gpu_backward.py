@@ -200,7 +200,7 @@ def test_full_size_input_gradients_match_oracle_autograd(golden_dir, precision):
     e_v, e_r, e_p = _rel_err(dvox, dvox_ref), _rms_err(dvox, dvox_ref), _rel_err(dpose, dpose_ref)
     cos = float((dvox.ravel() * dvox_ref.ravel()).sum() / (np.linalg.norm(dvox) * np.linalg.norm(dvox_ref)))
     print(f"[{precision}] dL/dvox err max {e_v:.2e} rms {e_r:.2e} (cosine {cos:.6f}), dL/dpose {dpose} vs {dpose_ref} rel err {e_p:.2e}")
-    # full-size weight gradients (tcgen05 wgrad kernel, K = 4096 pixels) of a few layers vs autograd
+    # full-size weight gradients (wgmma wgrad kernel, K = 4096 pixels) of a few layers vs autograd
     for n in WGRAD_PROBES:
         got, want = ig.weight_grads[n].cpu().numpy(), dw_ref[n]
         c = float((got.ravel() * want.ravel()).sum() / (np.linalg.norm(got) * np.linalg.norm(want)))
@@ -239,7 +239,7 @@ def test_thin_conv3d_data_gradients_match_autograd():
 # ----------------------------------------------------------------------------------------- stage 2: weight gradients
 @pytest.mark.parametrize("k,cin,cout,hw,B", [(3, 128, 256, 32, 2), (1, 256, 128, 64, 1), (4, 128, 128, 16, 3), (3, 256, 512, 64, 2)])
 def test_conv2d_weight_and_bias_gradients_match_autograd(k, cin, cout, hw, B):
-    """rn_conv2d_weight_grad (tcgen05, MN-major operands straight from the channel-last tensors, K = pixels, split-K over CTAs)
+    """rn_conv2d_weight_grad (wgmma, MN-major operands straight from the channel-last tensors, K = pixels, split-K over CTAs)
     and rn_bias_grad_16 vs torch.autograd on the oracle's conv2d, both precisions.  Exact: 2e-5 of the gradient scale (fp32
     accumulation over up to 8192 pixels); fast: operand rounding, 2e-3."""
     from rendernet_b200 import ops

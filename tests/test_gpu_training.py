@@ -84,7 +84,7 @@ def test_direct_weight_gradient_kernel_matches_autograd(kind, wshape, xshape, st
 
 
 def test_depth_folded_tensor_core_weight_gradient_equals_direct_kernel():
-    """res1 layer, real shape (B=1, 64x64x32, 32 -> 32): the tcgen05 gradient of the depth-folded conv + block-diagonal extraction
+    """res1 layer, real shape (B=1, 64x64x32, 32 -> 32): the wgmma gradient of the depth-folded conv + block-diagonal extraction
     vs the direct kernel vs autograd."""
     from rendernet_b200 import ops
     from rendernet_b200.backward import ShaderInputGradients
@@ -222,7 +222,7 @@ def test_gradients_of_every_variable_match_oracle_autograd(golden_dir, precision
     for k, v in kinds.items():
         print(f"[{precision}] {k}: {len(v)} variables, cosine min {min(c for c, _ in v):.5f} median {np.median([c for c, _ in v]):.5f}, "
               f"norm ratio {min(r for _, r in v):.4f}..{max(r for _, r in v):.4f}")
-    bar = 0.9999 if precision == "exact" else 0.9985         # measured: 1.00000 / 0.99976 (profiles/r02_training_parity.log)
+    bar = 0.9999 if precision == "exact" else 0.9985
     assert c_min > bar, (worst, c_min)
     assert all(abs(r - 1) < (5e-3 if precision == "exact" else 3e-2) for _, r, _ in rows)      # measured: 4e-4 / 5.4e-3
 

@@ -334,13 +334,13 @@ def test_pose_matrix_vjp_matches_finite_differences_host():
 
 
 def test_banded_filter_sizes_and_abi_rejections():
-    """Host-only checks of the C ABI: the banded filter holds two arrangements (single CTA / CTA pair) of 9 x kblocks tiles;
+    """Host-only checks of the C ABI: the banded filter holds 9 x kblocks tiles of 128 x 64;
     geometry the depth-folded form cannot take is rejected before any launch; exact-mode descriptors need their plane offsets."""
     from rendernet_b200._lib import lib
-    assert lib.rn_conv3d_banded_bytes(32, 32, 1) == 2 * 9 * 3 * 128 * 64 * 2        # res1: 3 K blocks
-    assert lib.rn_conv3d_banded_bytes(16, 32, 1) == 2 * 9 * 2 * 128 * 64 * 2        # e_conv3: 2 K blocks
-    assert lib.rn_conv3d_banded_bytes(8, 16, 2) == 2 * 9 * 3 * 128 * 64 * 2         # e_conv2 (z stride 2)
-    assert lib.rn_conv3d_banded_bytes(16, 16, 1) == 2 * 9 * 3 * 128 * 64 * 2        # Texture net res1
+    assert lib.rn_conv3d_banded_bytes(32, 32, 1) == 9 * 3 * 128 * 64 * 2        # res1: 3 K blocks
+    assert lib.rn_conv3d_banded_bytes(16, 32, 1) == 9 * 2 * 128 * 64 * 2        # e_conv3: 2 K blocks
+    assert lib.rn_conv3d_banded_bytes(8, 16, 2) == 9 * 3 * 128 * 64 * 2         # e_conv2 (z stride 2)
+    assert lib.rn_conv3d_banded_bytes(16, 16, 1) == 9 * 3 * 128 * 64 * 2        # Texture net res1
     assert lib.rn_conv3d_banded_bytes(48, 32, 1) == -1 and lib.rn_conv3d_banded_bytes(32, 32, 3) == -1
     assert lib.rn_xfold_factor(16, 512) == 4 and lib.rn_xfold_factor(32, 512) == 2 and lib.rn_xfold_factor(64, 512) == 1
     assert lib.rn_version() >= 100 and lib.rn_launch_count() >= 0
