@@ -260,29 +260,9 @@ class ShaderInputGradients:
                 if res is not None:                            # y = act(conv(x) + res): the gradient flows to res unchanged
                     k = _key(res)
                     grads[k] = ops.bias_act(g, None, None, None, residual=grads[k]) if k in grads else g
-                x, kind, stride = rec["x"], rec["kind"], rec["stride"]
+                x = rec["x"]
                 acc = grads.pop(_key(x), None)                 # gradient already collected for x (fan-out): fused as `residual`
-                if kind == "conv3d" and stride == 2:           # e_conv2: thin, z-strided -> CUDA cores
-                    w32 = rec["w"].to(dev).float().contiguous()
-                    gx = ops.conv3d_backward_data_direct(g, w32, tuple(x.shape), (1, 1, 2))
-                    if acc is not None:
-                        gx = ops.bias_act(gx, None, None, None, residual=acc)
-                else:
-                    L = self._dgrad_layer(rec)
-                    if kind == "conv3d":
-                        gx = ops.conv3d_banded(g, L, residual=acc)
-                    elif kind == "conv2d":
-                        k = int(rec["w"].shape[0])
-                        if k % 2 == 1:
-                            gx = ops.conv2d(g, L, residual=acc)
-                        else:
-                            gx = ops.conv2d_taps(g, L.w, L.bias, L.taps, L.cout, L.cout_pad, fmt, residual=acc,
-                                                 ny=k if L.cin % 64 == 0 else 0)
-                    elif stride == 1:                          # transposed conv, stride 1
-                        gx = ops.conv2d(g, L, residual=acc)
-                    else:                                      # transposed conv, stride 2
-                        gx = ops.conv2d(self._space_to_depth(g), L, residual=acc)
-                grads[_key(x)] = gx
+                grads[_key(x)] = self._data_grad_of(rec, g, acc)
             dvox = dminv = None
             if need_inputs:
                 if dgrid is None:
@@ -294,6 +274,27 @@ class ShaderInputGradients:
         if want_dpose:
             dpose = pose_matrix_jacobian_vjp(self.view_params, dminv.cpu().numpy(), self.size, self.new_size)
         return (dvox.cpu().numpy() if dvox is not None else None), dpose
+
+    def _data_grad_of(self, rec, g, acc=None):
+        """dL/dx of one recorded convolution layer from g = dL/d(its pre-activation) (16-bit, carrying the loss scale); `acc`, a
+        gradient already collected for x at a fan-out, is added to the result (fused as the kernels' `residual` input)."""
+        x, kind, stride = rec["x"], rec["kind"], rec["stride"]
+        if kind == "conv3d" and stride == 2:           # e_conv2: thin, z-strided -> CUDA cores
+            w32 = rec["w"].to(self.store.device).float().contiguous()
+            gx = ops.conv3d_backward_data_direct(g, w32, tuple(x.shape), (1, 1, 2))
+            return gx if acc is None else ops.bias_act(gx, None, None, None, residual=acc)
+        L = self._dgrad_layer(rec)
+        if kind == "conv3d":
+            return ops.conv3d_banded(g, L, residual=acc)
+        if kind == "conv2d":
+            k = int(rec["w"].shape[0])
+            if k % 2 == 1:
+                return ops.conv2d(g, L, residual=acc)
+            return ops.conv2d_taps(g, L.w, L.bias, L.taps, L.cout, L.cout_pad, self.store.fmt, residual=acc,
+                                   ny=k if L.cin % 64 == 0 else 0)
+        if stride == 1:                                # transposed conv, stride 1
+            return ops.conv2d(g, L, residual=acc)
+        return ops.conv2d(self._space_to_depth(g), L, residual=acc)      # transposed conv, stride 2
 
     # ------------------------------------------------------------------------------------------- weight gradients
     def _weight_grads_of(self, rec, g, inv: float, tensor_core: bool):

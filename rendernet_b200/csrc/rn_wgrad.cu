@@ -10,8 +10,8 @@
 // activations is ever made.  The tap offset is a shifted TMA coordinate for x (zero fill outside the image = SAME padding).
 //
 // One CTA tile = (tap, 128 input channels, BN output channels); the K loop runs over pixel blocks of a slice of the batch
-// (split-K over CTAs when there are fewer tiles than SMs; partial results are combined with fp32 atomics into a
-// zero-initialised dW).  Warpgroup 0 = TMA producer; warpgroups 1 and 2 each own 64 of the 128 input channels: m64nBNk16
+// (split-K over CTAs when there are fewer tiles than SMs or a slice would exceed kWgMaxChainPixels; partial results are
+// combined with fp32 atomics into a zero-initialised dW).  Warpgroup 0 = TMA producer; warpgroups 1 and 2 each own 64 of the 128 input channels: m64nBNk16
 // wgmmas into fp32 register accumulators, then the stores of those rows.  Exact mode (fmt 2): three passes x_lo.g_hi,
 // x_hi.g_lo, x_hi.g_hi into the same accumulator, corrections first (DESIGN.md §4).
 #include <atomic>
@@ -42,6 +42,7 @@ struct alignas(64) WgradParams {
 
 constexpr int kWgBM = 128;                 // input channels per tile (2 boxes of 64)
 constexpr int kBoxBytes = 64 * 128;        // one TMA box: 64 pixels x 64 channels x 2 B
+constexpr int kWgMaxChainPixels = 4096;    // pixels one CTA accumulates in a single wgmma chain (when the batch can be split)
 
 __device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr) {
   uint64_t d = 0;
@@ -74,7 +75,10 @@ __global__ void __launch_bounds__(384, 1) wgrad2d_kernel(const __grid_constant__
 
   const int bx = p.W / p.PX, by = p.H / p.PY;
   const int kb_per_img = bx * by;
-  const int total_work = p.ntaps * p.m_tiles * p.n_tiles * p.ksplit;
+  // batch slice ks is the slowest index: CTAs running at the same time work on different output tiles (no atomics on the same
+  // addresses) of the same images (shared in L2)
+  const int tiles = p.ntaps * p.m_tiles * p.n_tiles;
+  const int total_work = tiles * p.ksplit;
   const int passes = p.split ? 3 : 1;
 
   if (warp < 4) {
@@ -82,7 +86,7 @@ __global__ void __launch_bounds__(384, 1) wgrad2d_kernel(const __grid_constant__
     if (warp == 0 && elect_one()) {
       int stage = 0; uint32_t phase = 0;
       for (int wk = blockIdx.x; wk < total_work; wk += gridDim.x) {
-        const int ks = wk % p.ksplit; int t = wk / p.ksplit;
+        const int ks = wk / tiles; int t = wk % tiles;
         const int ni = t % p.n_tiles; t /= p.n_tiles;
         const int mi = t % p.m_tiles; const int tap = t / p.m_tiles;
         const int b0 = (p.B * ks) / p.ksplit, b1 = (p.B * (ks + 1)) / p.ksplit;
@@ -115,7 +119,7 @@ __global__ void __launch_bounds__(384, 1) wgrad2d_kernel(const __grid_constant__
     float acc[NACC];
     int stage = 0; uint32_t phase = 0;
     for (int wk = blockIdx.x; wk < total_work; wk += gridDim.x) {
-      const int ks = wk % p.ksplit; int t = wk / p.ksplit;
+      const int ks = wk / tiles; int t = wk % tiles;
       const int ni = t % p.n_tiles; t /= p.n_tiles;
       const int mi = t % p.m_tiles; const int tap = t / p.m_tiles;
       const int b0 = (p.B * ks) / p.ksplit, b1 = (p.B * (ks + 1)) / p.ksplit;
@@ -222,6 +226,11 @@ extern "C" int rn_conv2d_weight_grad(const void* x, const void* g, float* dw, in
   const int sms = num_sms();
   int ksplit = 1;
   while (tiles * ksplit < sms && ksplit * 2 <= B) ksplit *= 2;          // fewer tiles than SMs: split the batch over CTAs
+  // The tensor core truncates its fp32 accumulator once per k-step, so one long wgmma chain shrinks its sum by ~1.6e-8 per step
+  // (trunk layer, B = 24 in one chain: 6144 steps, a bias of -9.9e-5).  Cap a CTA's chain at kWgMaxChainPixels (256 steps,
+  // bias ~ -4e-6) by splitting the batch further; the slices are summed by round-to-nearest fp32 atomics.
+  const long long chain_split = (static_cast<long long>(B) * H * W + kWgMaxChainPixels - 1) / kWgMaxChainPixels;
+  if (ksplit < chain_split) ksplit = static_cast<int>(chain_split < B ? chain_split : B);
   p.ksplit = ksplit;
   const int stage_bytes = (2 + BN / 64) * kBoxBytes;
   p.stages = (kMaxSmem - 1024 - 256) / stage_bytes;

@@ -183,3 +183,44 @@ def test_dropout_is_refused_outside_the_training_path_and_gradient_allreduce_is_
         tf.nn.dropout(x, 0.75)
     g = {"a": torch.ones(3), "b": torch.zeros(2, 2)}
     assert all_reduce_gradients(g) is g and torch.equal(g["a"], torch.ones(3))
+
+
+def test_frozen_kink_prelu_reproduces_the_oracle_with_its_own_masks():
+    """oracle.frozen_kinks, which the whole-network gradient tests use to give the oracle the device's PReLU branches: on a
+    narrow Shader net, masks taken from the oracle's own pre-activations reproduce its image and the autograd gradients of all
+    variables bit for bit (the two forms differ only at a pre-activation of exactly 0, where there is none here), and a mask of
+    the wrong shape or a slope it does not know is an error."""
+    from oracle.frozen_kinks import kink_flips, prelu_kinks
+    W = orc.init_shader_weights(seed=4, width=8, depth=8, alpha_range=(-0.2, 0.3), bias_jitter=0.05)   # 64 features: e_conv10 -> 1
+    x = torch.from_numpy(np.random.default_rng(0).random((2, 8, 8, 32, 1)).astype(np.float32))
+    G = torch.from_numpy(np.random.default_rng(1).standard_normal((2, 32, 32, 3)).astype(np.float32))
+
+    def run(masks=None, record=None):
+        Wt = {n: torch.tensor(v, requires_grad=True) for n, v in W.items()}
+        with prelu_kinks(Wt, masks=masks, record=record):
+            img = orc.rendernet_shader(x, Wt)
+        grads = torch.autograd.grad((img * G).sum(), [Wt[n] for n in sorted(Wt)])
+        return img.detach(), dict(zip(sorted(Wt), grads))
+
+    plain = orc.prelu
+    signs = {}
+    img0, g0 = run(record=signs)
+    assert len(signs) == 36                                   # every PReLU of the graph, projection unit included
+    plain_img = orc.rendernet_shader(x, W)
+    assert torch.equal(img0, plain_img)                       # recording changes nothing
+    img1, g1 = run(masks=signs)
+    assert kink_flips(signs, signs) == (0, sum(int(m.numel()) for m in signs.values()))
+    assert torch.equal(img1, img0)
+    assert all(torch.equal(g1[n], g0[n]) for n in g0), [n for n in g0 if not torch.equal(g1[n], g0[n])][:3]
+    flipped = {n: m.clone() for n, m in signs.items()}
+    flipped["encoder/e_conv5/alpha"].view(-1)[:7] ^= True
+    img2, g2 = run(masks=flipped)
+    assert not torch.equal(img2, img0) or not torch.equal(g2["encoder/e_conv5/alpha"], g0["encoder/e_conv5/alpha"])
+    bad = dict(signs)
+    bad["encoder/e_conv3/alpha"] = bad["encoder/e_conv3/alpha"][:1]
+    with pytest.raises(ValueError):
+        run(masks=bad)
+    with pytest.raises(KeyError):
+        with prelu_kinks({}, masks={}):
+            orc.rendernet_shader(x, W)
+    assert orc.prelu is plain
