@@ -121,6 +121,64 @@ def test_resampler_against_float64_bruteforce():
     assert worst < 2e-4, worst
 
 
+def test_device_cell_resampler_matches_golden(golden_dir):
+    """oracle/resample_cells.py, the float64 resampler the backward tests differentiate: its emulated fp32 sample coordinates
+    equal np.matmul's bit for bit, and its output matches the fixtures everywhere, the knife-edge points of the axis-aligned
+    poses included (inside/outside decided by one ulp).  Inside the cube only fp32-vs-float64 weight rounding separates them;
+    outside, the fixtures hold the reference's clamped-corner cancellation noise where the resampler writes 0 (DESIGN §4)."""
+    from oracle import resample_cells as rc
+    g = _g(golden_dir, "resample.npz")
+    cases = [("small_vox", "small_pose", "small_out", 16, 32, False), ("small_vox", "small_pose", "small_net_in", 16, 32, True),
+             ("axis_vox", "axis_pose", "axis_out", 16, 32, False), (None, "chair_pose", None, 64, 128, True)]
+    for vk, pk, ok, S, N, transform in cases:
+        vox = _chair(golden_dir) if vk is None else g[vk]
+        if ok is None:
+            want = np.zeros(N ** 3, np.float32)
+            want[g["chair_nz_idx"]] = g["chair_nz_val"]
+        else:
+            want = g[ok]
+        want = want.reshape(vox.shape[0], N, N, N, vox.shape[-1])
+        R, Sm = orc.rotation_around_grid_centroid(g[pk])
+        minv = orc.inverse_total_matrix(R, Sm, S, N)
+        grid = rc.output_grid(N, transform)
+        c = rc.sample_coords(minv, grid)
+        assert np.array_equal(c, np.matmul(minv, grid.astype(np.float32)[None]))
+        inside = ((c >= 0) & (c < S - 1)).all(1).reshape(vox.shape[0], N, N, N)
+        got = rc.resample(torch.from_numpy(vox.astype(np.float64)), torch.from_numpy(minv.astype(np.float64)), N, transform).numpy()
+        err = np.abs(got - want).max(-1)
+        assert err[inside].max() < 1e-6 and err[~inside].max() < 5e-5, (ok, err[inside].max(), err[~inside].max())
+        if vk == "axis_vox":
+            edge = (np.minimum(np.abs(c), np.abs(c - (S - 1))).min(1) < 1e-4).reshape(inside.shape)
+            assert (edge & inside).sum() > 500 and (edge & ~inside).sum() > 500       # both sides of the border are pinned
+            f64 = rc.resample(torch.from_numpy(vox.astype(np.float64)), torch.from_numpy(minv.astype(np.float64)), N, transform,
+                              device_cells=False).numpy()
+            assert np.abs(f64 - want).max() > 0.5              # float64 coordinates decide some knife edges the other way
+
+
+def test_device_cell_coordinates_round_once():
+    """The fp32 emulation of oracle/resample_cells.py rounds each fused multiply-add once, as fmaf does, also where going
+    through float64 would round twice: 2^30 + (64 + 2^-24) lies just above the fp32 halfway point 2^30 + 64."""
+    from fractions import Fraction
+    from oracle import resample_cells as rc
+
+    def round32(v):                                        # nearest fp32 to the exact value v, ties to the even significand
+        r = np.float32(float(v))
+        near = [np.nextafter(r, np.float32(-np.inf)), r, np.nextafter(r, np.float32(np.inf))]
+        return min(near, key=lambda f: (abs(Fraction(float(f)) - v), int(np.array(f).view(np.uint32)) & 1))
+
+    a, c = np.float32(16519105 * 2.0 ** -24), np.float32(2.0 ** 30)          # a * 65 = 64 + 2^-24 exactly
+    for s in (1, -1):
+        got = rc._fma32(np.array([s * a]), 65.0, np.array([s * c]))[0]
+        assert got == round32(Fraction(float(s * a)) * 65 + Fraction(float(s * c))) == np.float32(s * (2.0 ** 30 + 128))
+    rng = np.random.default_rng(0)
+    a = (rng.uniform(-1, 1, 3000) * np.exp2(rng.integers(-40, 6, 3000))).astype(np.float32)
+    c = (rng.uniform(-1, 1, 3000) * np.exp2(rng.integers(-5, 11, 3000))).astype(np.float32)
+    b = rng.integers(0, 128, 3000).astype(np.float64)
+    got = rc._fma32(a, b, c)
+    want = np.array([round32(Fraction(float(x)) * int(y) + Fraction(float(z))) for x, y, z in zip(a, b, c)], np.float32)
+    assert np.array_equal(got, want)
+
+
 def test_axis_transform_definition():
     t = np.arange(2 * 3 * 4 * 5 * 1, dtype=np.float32).reshape(2, 3, 4, 5, 1)
     n = orc.transform_voxel_to_match_image(t)
