@@ -30,6 +30,7 @@ try:  # torch is only needed for the conv stack
 except Exception:  # pragma: no cover
     torch = None
     F = None
+_F32 = torch.float32 if torch is not None else None   # default arithmetic type of the conv stack
 
 
 # ----------------------------------------------------------------------------------
@@ -195,9 +196,10 @@ def _t(x):
     return x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
 
 
-def conv3d(x, w, b=None, stride=(1, 1, 1)):
-    """tf.nn.conv3d SAME + bias (layer_util.py:228-265).  x [B,D0,D1,D2,Cin], w [k0,k1,k2,Cin,Cout]."""
-    x = _t(x).float(); w = _t(w).float()
+def conv3d(x, w, b=None, stride=(1, 1, 1), dtype=_F32):
+    """tf.nn.conv3d SAME + bias (layer_util.py:228-265).  x [B,D0,D1,D2,Cin], w [k0,k1,k2,Cin,Cout].
+    dtype: arithmetic type (torch.float64 gives a high-precision reference of the same op)."""
+    x = _t(x).to(dtype); w = _t(w).to(dtype)
     xs = x.permute(0, 4, 1, 2, 3)
     pads = []
     for d in (2, 1, 0):  # F.pad wants last dim first
@@ -206,7 +208,7 @@ def conv3d(x, w, b=None, stride=(1, 1, 1)):
     y = F.conv3d(F.pad(xs, pads), w.permute(4, 3, 0, 1, 2).contiguous(), stride=tuple(stride))
     y = y.permute(0, 2, 3, 4, 1)
     if b is not None:
-        y = y + _t(b).float()
+        y = y + _t(b).to(dtype)
     return y.contiguous()
 
 
@@ -241,31 +243,31 @@ def conv2d_transpose(x, w, b=None, stride=(1, 1)):
     return y.contiguous()
 
 
-def conv3d_transpose(x, w, b=None, stride=(1, 1, 1)):
-    """tf.nn.conv3d_transpose SAME (layer_util.py:269-309).  w [k0,k1,k2,Cout,Cin]."""
-    x = _t(x).float(); w = _t(w).float()
+def conv3d_transpose(x, w, b=None, stride=(1, 1, 1), dtype=_F32):
+    """tf.nn.conv3d_transpose SAME (layer_util.py:269-309).  w [k0,k1,k2,Cout,Cin]; dtype as in conv3d."""
+    x = _t(x).to(dtype); w = _t(w).to(dtype)
     B, D0, D1, D2, _ = x.shape
     full = F.conv_transpose3d(x.permute(0, 4, 1, 2, 3), w.permute(4, 3, 0, 1, 2).contiguous(), stride=tuple(stride))
     pb = [max(w.shape[d] - stride[d], 0) // 2 for d in range(3)]
     y = full[:, :, pb[0]:pb[0] + D0 * stride[0], pb[1]:pb[1] + D1 * stride[1], pb[2]:pb[2] + D2 * stride[2]]
     y = y.permute(0, 2, 3, 4, 1)
     if b is not None:
-        y = y + _t(b).float()
+        y = y + _t(b).to(dtype)
     return y.contiguous()
 
 
-def fully_connected(x, w, b=None):
-    """layer_util.py:311-343."""
-    y = _t(x).float() @ _t(w).float()
+def fully_connected(x, w, b=None, dtype=_F32):
+    """layer_util.py:311-343; dtype as in conv3d."""
+    y = _t(x).to(dtype) @ _t(w).to(dtype)
     if b is not None:
-        y = y + _t(b).float()
+        y = y + _t(b).to(dtype)
     return y
 
 
-def prelu(x, alpha):
-    """layer_util.py:27-45: max(0,x) + alpha*min(0,x), alpha per last-axis channel."""
-    x = _t(x).float(); a = _t(np.asarray(alpha, np.float32)) if not isinstance(alpha, torch.Tensor) else alpha.float()
-    return torch.clamp(x, min=0) + a * torch.clamp(x, max=0)
+def prelu(x, alpha, dtype=_F32):
+    """layer_util.py:27-45: max(0,x) + alpha*min(0,x), alpha per last-axis channel; dtype as in conv3d."""
+    x = _t(x).to(dtype); a = _t(np.asarray(alpha, np.float32)) if not isinstance(alpha, torch.Tensor) else alpha
+    return torch.clamp(x, min=0) + a.to(dtype) * torch.clamp(x, max=0)
 
 
 def projection_unit(x, w, b, alpha):
@@ -553,20 +555,23 @@ def init_texture_weights(seed: int = 0, alpha_range=(0.0, 0.0), gain: float = 1.
     return W
 
 
-def decoder_texture(z_in, W):
-    """RenderNet_Texture_Face_Normal.py:34-46: FC 199->32^3*4, T-conv 4^3 s1 4->4, T-conv 4^3 s2 4->8, conv 4^3 8->4."""
+def decoder_texture(z_in, W, dtype=_F32):
+    """RenderNet_Texture_Face_Normal.py:34-46: FC 199->32^3*4, T-conv 4^3 s1 4->4, T-conv 4^3 s2 4->8, conv 4^3 8->4.
+    z_in is taken as float32 (what the model is fed); dtype is the arithmetic type, as in conv3d."""
     te = "texture_encoder"
     g = lambda n: W[n]
     z = _t(np.asarray(z_in, np.float32))
-    zP = prelu(fully_connected(z, g(f"{te}/e_tex_fc1/fully_connected/weights"), g(f"{te}/e_tex_fc1/fully_connected/biases")),
-               g(f"{te}/e_tex_fc1/alpha"))
+    zP = prelu(fully_connected(z, g(f"{te}/e_tex_fc1/fully_connected/weights"), g(f"{te}/e_tex_fc1/fully_connected/biases"),
+                               dtype), g(f"{te}/e_tex_fc1/alpha"), dtype)
     x = zP.reshape(z.shape[0], 32, 32, 32, 4)
     c0 = prelu(conv3d_transpose(x, g(f"{te}/e_tex_conv0/conv3d_transpose/weights"),
-                                g(f"{te}/e_tex_conv0/conv3d_transpose/biases"), (1, 1, 1)), g(f"{te}/e_tex_conv0/alpha"))
+                                g(f"{te}/e_tex_conv0/conv3d_transpose/biases"), (1, 1, 1), dtype),
+               g(f"{te}/e_tex_conv0/alpha"), dtype)
     c1 = prelu(conv3d_transpose(c0, g(f"{te}/e_tex_conv1/conv3d_transpose/weights"),
-                                g(f"{te}/e_tex_conv1/conv3d_transpose/biases"), (2, 2, 2)), g(f"{te}/e_tex_conv1/alpha"))
-    c2 = prelu(conv3d(c1, g(f"{te}/e_tex_conv2/conv3d/weights"), g(f"{te}/e_tex_conv2/conv3d/biases"), (1, 1, 1)),
-               g(f"{te}/e_tex_conv2/alpha"))
+                                g(f"{te}/e_tex_conv1/conv3d_transpose/biases"), (2, 2, 2), dtype),
+               g(f"{te}/e_tex_conv1/alpha"), dtype)
+    c2 = prelu(conv3d(c1, g(f"{te}/e_tex_conv2/conv3d/weights"), g(f"{te}/e_tex_conv2/conv3d/biases"), (1, 1, 1), dtype),
+               g(f"{te}/e_tex_conv2/alpha"), dtype)
     return c2
 
 

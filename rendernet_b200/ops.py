@@ -667,25 +667,38 @@ def bias_act(x, bias: Optional[torch.Tensor], alpha: Optional[torch.Tensor], act
 
 # --------------------------------------------------------------------------------------- texture decoder (config 4)
 def fully_connected(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], alpha: Optional[torch.Tensor],
-                    want32: bool = True, dtype: torch.dtype = torch.float16) -> torch.Tensor:
-    """y = prelu(x @ w + bias; alpha).  x [B,K] fp32, w [K,N] fp32 (TF layout) -> [B,N] fp32 (or 16-bit)."""
+                    want32: bool = True, dtype: torch.dtype = torch.float16, fmt: Optional[int] = None):
+    """y = prelu(x @ w + bias; alpha).  x [B,K] fp32, w [K,N] fp32 (TF layout) -> [B,N] fp32, or 16-bit in the format
+    `fmt` or else `dtype` picks (fmt 2: fp16 hi/lo pair, returned as Split16)."""
     x = _cuda(x, torch.float32)
     w = _cuda(w, torch.float32)
     B, K = x.shape
     N = w.shape[1]
-    out = torch.empty((B, N), device=x.device, dtype=torch.float32 if want32 else dtype)
+    fmt = fmt_of(dtype) if fmt is None else int(fmt)
+    out = (torch.empty((B, N), device=x.device, dtype=torch.float32) if want32
+           else _alloc16((B, N), fmt, torch.bfloat16 if fmt == 1 else torch.float16, x.device))
     check(lib.rn_fully_connected(x.data_ptr(), w.data_ptr(), _ptr(bias), _ptr(alpha), None if want32 else out.data_ptr(),
-                                 out.data_ptr() if want32 else None, B, K, N, fmt_of(dtype), _stream()),
+                                 out.data_ptr() if want32 else None, B, K, N, fmt, _stream()),
           "rn_fully_connected")
-    return out
+    return out if want32 else _wrap16(out, fmt)
 
 
-def conv3d_small(x: torch.Tensor, w_tf: torch.Tensor, bias: Optional[torch.Tensor], alpha: Optional[torch.Tensor],
-                 stride: int, transposed: bool, want32: bool = True, dtype: torch.dtype = torch.float16) -> torch.Tensor:
-    """Thin (<= 8 channel) conv3d / conv3d_transpose, TF SAME, + bias + PReLU.  x [B,H,W,D,Cin] fp32 or 16-bit;
-    w_tf fp32 [k,k,k,Cin,Cout] (forward) or [k,k,k,Cout,Cin] (transposed)."""
+def conv3d_small(x, w_tf: torch.Tensor, bias: Optional[torch.Tensor], alpha: Optional[torch.Tensor],
+                 stride: int, transposed: bool, want32: bool = True, dtype: torch.dtype = torch.float16,
+                 fmt: Optional[int] = None):
+    """Thin (<= 8 channel) conv3d / conv3d_transpose, TF SAME, + bias + PReLU.  x [B,H,W,D,Cin] fp32, 16-bit or Split16;
+    w_tf fp32 [k,k,k,Cin,Cout] (forward) or [k,k,k,Cout,Cin] (transposed).  The kernel reads and writes ONE 16-bit format:
+    a 16-bit x sets it (a 16-bit output then has x's format); for an fp32 x, `fmt` or else `dtype` picks the output's."""
     x = _cuda(x)
     w_tf = _cuda(w_tf, torch.float32)
+    x_is_f32 = isinstance(x, torch.Tensor) and x.dtype == torch.float32
+    if not x_is_f32:
+        fx = 2 if isinstance(x, Split16) else fmt_of(x.dtype)
+        if fmt is not None and int(fmt) != fx:
+            raise TypeError(f"conv3d_small: a 16-bit input of format {fx} gives output format {fx}, not {fmt}")
+        fmt = fx
+    elif fmt is None:
+        fmt = fmt_of(dtype)
     B, H, W, D, Cin = x.shape
     k = w_tf.shape[0]
     Cout = w_tf.shape[3] if transposed else w_tf.shape[4]
@@ -693,12 +706,12 @@ def conv3d_small(x: torch.Tensor, w_tf: torch.Tensor, bias: Optional[torch.Tenso
         oshape = (B, H * stride, W * stride, D * stride, Cout)
     else:
         oshape = (B, -(-H // stride), -(-W // stride), -(-D // stride), Cout)
-    out = torch.empty(oshape, device=x.device, dtype=torch.float32 if want32 else dtype)
-    check(lib.rn_conv3d_small(x.data_ptr(), 1 if x.dtype == torch.float32 else 0, w_tf.data_ptr(), _ptr(bias),
+    out = (torch.empty(oshape, device=x.device, dtype=torch.float32) if want32
+           else _alloc16(oshape, fmt, torch.bfloat16 if fmt == 1 else torch.float16, x.device))
+    check(lib.rn_conv3d_small(x.data_ptr(), 1 if x_is_f32 else 0, w_tf.data_ptr(), _ptr(bias),
                               _ptr(alpha), None if want32 else out.data_ptr(), out.data_ptr() if want32 else None,
-                              B, H, W, D, Cin, Cout, k, stride, 1 if transposed else 0,
-                              fmt_of(dtype if x.dtype == torch.float32 else x.dtype), _stream()), "rn_conv3d_small")
-    return out
+                              B, H, W, D, Cin, Cout, k, stride, 1 if transposed else 0, fmt, _stream()), "rn_conv3d_small")
+    return out if want32 else _wrap16(out, fmt)
 
 
 def concat_channels(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:

@@ -341,3 +341,21 @@ def test_texture_model_matches_reference_python(golden_dir):
     img, nrm = orc.rendernet_texture(x5, W)
     assert np.abs(img.numpy() - g["image"]).max() < 5e-6
     assert np.abs(nrm.numpy() - g["normal"]).max() < 5e-6
+
+
+def test_texture_decoder_float64_matches_float32_and_reference_python(golden_dir):
+    """decoder_texture(dtype=torch.float64) -- the reference tests/test_gpu_texture.py holds the CUDA decoder to -- runs the same
+    SAME-padding and transposed-conv code as the fp32 oracle pinned above, in float64.  Measured (max error / max |float64|):
+    vs the fp32 oracle 1.3e-6, vs the fixture's every-4th-voxel sample 1.5e-7 (the fixture is fp32); the sum over all voxels is
+    2.4e-10 of the fixture's sum of |values|."""
+    g = _g(golden_dir, "texture_patch.npz")
+    W = orc.init_texture_weights(seed=int(g["weight_seed"]), alpha_range=tuple(g["alpha_range"]),
+                                 gain=float(g["gain"]), bias_jitter=float(g["bias_jitter"]))
+    t32 = orc.decoder_texture(g["z_in"], W)
+    t64 = orc.decoder_texture(g["z_in"], W, dtype=torch.float64)
+    assert t32.dtype == torch.float32 and t64.dtype == torch.float64 and t64.shape == t32.shape == (1, 64, 64, 64, 4)
+    t64 = t64.numpy()
+    scale = np.abs(t64).max()
+    assert np.abs(t64 - t32.numpy()).max() < 4e-6 * scale
+    assert np.abs(t64[:, ::4, ::4, ::4] - g["decoder_sub"]).max() < 5e-7 * scale
+    assert abs(t64.sum() - float(g["decoder_sum"])) < 1e-9 * float(g["decoder_abs_sum"])
