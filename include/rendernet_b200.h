@@ -286,6 +286,31 @@ int rn_conv3d_backward_data_direct(const void* g16, const float* w, void* dx16, 
  * them first.  Points outside the cube contribute nothing (the forward writes exact zeros there).  C = 1 or 4. */
 int rn_resample_backward_f32(const float* vox, const float* minv, const float* gout, float* dvox, float* dminv, int B, int C,
                              int size, int new_size, int transform, void* stream);
+/* Backward of rn_resample5_conv1_fused's input chain (Texture net, RenderNet_Texture_Face_Normal.py:155-179 /
+ * Reconstruct_RenderNet_Face.py:367-378: two axis-transformed resamplings with one pose, concatenated): gout = dL/d(concat)
+ * [B,new,new,new,5] fp32 -> dvox [B,size^3,1] (channel 0), dtex [B,size^3,4] (channels 1..4, 16-byte aligned) and dminv
+ * [B,3,4] (all five channels), each ACCUMULATED into (zero them first) and each may be NULL.  Sample coordinates and in/out
+ * decisions are the forward kernel's. */
+int rn_resample5_backward_f32(const float* vox, const float* tex, const float* minv, const float* gout, float* dvox, float* dtex,
+                              float* dminv, int B, int size, int new_size, void* stream);
+/* fp32 PReLU derivative (texture decoder, tools/layer_util.py:27-45): out[i] = g[i] * (z[i] > 0 ? 1 : alpha[i % C]) with z the
+ * PRE-activation (slopes may be negative). */
+int rn_prelu_backward_f32(const float* g, const float* z, const float* alpha, float* out, long long n, int C, void* stream);
+/* Data gradient of rn_fully_connected (tools/layer_util.py:311-343): dx[b][k] = sum_n g[b][n] w[k][n], g fp32 [B,N], w fp32 TF
+ * layout [K,N] (16-byte aligned, N % 4 == 0), B <= 32.  Split over N with a fixed-order second stage (no float atomics: the
+ * result is reproducible bit for bit); `work` holds rn_fully_connected_backward_workspace(B, K, N) floats. */
+/* Face reconstruction objective (Reconstruct_RenderNet_Face.py:372-383) over TensorFlow's Phong composite
+ * (tools/Phong_shading.py:24-113, tf_phong_composite; not the NumPy composite rn_phong_composite implements): shade =
+ * tf_phong_composite(normal, light_dir, light_col, ambient, k_diffuse, black_background, with_mask), loss[b] += mean_{h,w,c}
+ * (target - albedo * shade)^2, and in the same pass d_albedo, d_normal (fp32 [B,H,W,3], overwritten) and d_light_dir [B,3]
+ * (ACCUMULATED into: zero it first; may be NULL).  loss (double [B]) is accumulated into as well.  TF-1 gradient conventions:
+ * tf.maximum passes where x >= y, clip_by_value where lo <= x <= hi, d|x|/dx = x/|x|.  light_dir, light_col [B,3]. */
+int rn_phong_recon_loss_grad(const float* albedo, const float* normal, const float* target, const float* light_dir,
+                             const float* light_col, float ambient, float k_diffuse, int black_background, int with_mask,
+                             double* loss, float* d_albedo, float* d_normal, float* d_light_dir, int B, int H, int W,
+                             void* stream);
+long long rn_fully_connected_backward_workspace(int B, int K, int N);
+int rn_fully_connected_backward_data(const float* g, const float* w, float* work, float* dx, int B, int K, int N, void* stream);
 
 /* ---- backward pass, stage 2: weight gradients (training step, RenderNet_Shader.py:159-167) -------------------------------
  * dW of a stride-1 SAME conv2d (slim.conv2d / layer_util.conv2d, tools/layer_util.py:147-184) on the tensor cores:

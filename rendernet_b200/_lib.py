@@ -84,6 +84,11 @@ SIGNATURES = {
     "rn_sigmoid_backward": (_i, [_vp, _vp, _vp, _ll, _i, _i, _f, _i, _vp]),
     "rn_conv3d_backward_data_direct": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp]),
     "rn_resample_backward_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "rn_resample5_backward_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "rn_prelu_backward_f32": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _vp]),
+    "rn_fully_connected_backward_workspace": (_ll, [_i, _i, _i]),
+    "rn_fully_connected_backward_data": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "rn_phong_recon_loss_grad": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "rn_conv2d_weight_grad": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "rn_bias_grad_16": (_i, [_vp, _vp, _ll, _i, _i, _vp]),
     "rn_conv_weight_grad_direct": (_i, [_vp, _vp, _vp] + [_i] * 22 + [_f, _vp]),

@@ -22,6 +22,12 @@ realised layer appends (kind, input, filter, activation, residual, output).  `ba
     are mapped to (azimuth, elevation, scale) on the host by differentiating the reference's matrix construction
     (tools/resampling_voxel_grid.py:515-602) -- a 3 -> 12 map, float64.
 
+The Texture+Normal network (TextureInputGradients) walks the same tape the same way.  Its two heads both read enc5_skip, a
+fan-out like the residual adds.  Its input chain is two resamplings (geometry C = 1, decoded texture C = 4) concatenated into
+e_conv1: rn_resample5_backward_f32 splits dL/d(concat) into dL/dvoxels, dL/d(texture volume) and dL/dM^-1, and dL/d(texture
+volume) continues, in fp32, through the texture decoder (rn_prelu_backward_f32, rn_conv3d_small, rn_fully_connected_backward_data)
+to dL/d(texture vector).
+
 Gradients travel in the activations' 16-bit format (fp16, or fp16 hi/lo pairs in the exact mode) with a loss scale to keep
 them inside fp16's range; they are un-scaled when they leave the tensor-core part (fp32 from there on).
 """
@@ -37,7 +43,7 @@ from . import ops
 from . import tfcompat as tf
 from .RenderNet_Shader import RenderNet
 from .engine import pose_to_matrix
-from .resampling_voxel_grid import ResampledGrid
+from .resampling_voxel_grid import ConcatResampledGrid, ResampledGrid
 
 
 def _key(t) -> int:
@@ -70,21 +76,18 @@ def pose_matrix_jacobian_vjp(view_params: np.ndarray, dminv: np.ndarray, size: i
     return vp.grad.numpy()
 
 
-class ShaderInputGradients:
-    """Forward + input-gradient backward of the Shader network for a fixed batch size.
 
-        ig = ShaderInputGradients(weights, batch=1, precision="exact")
-        img = ig.forward(voxels, view_params)                 # [B,512,512,3] fp32 on the device (tape recorded)
-        dvox, dpose = ig.backward(dL_dimg)                    # [B,64,64,64,1], [B,3] fp32 (NumPy)
 
-    `weights`: {tf variable name: array} or None (seeded reference initialisers)."""
+class _InputGradients:
+    """What the Shader and the Texture+Normal input gradients share: the variable store, the per-layer data-gradient filters
+    and the reverse walk over the tape (`_reverse_walk`).  A subclass records the tape in `forward` and differentiates, in
+    `_input_chain`, the fused resample + e_conv1 record that starts its network."""
 
-    def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str = "exact", is_greyscale: bool = False,
-                 size: int = 64, new_size: int = 128, loss_scale: float = 4096.0, seed: int = 0, device: str = "cuda"):
+    def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str, size: int, new_size: int,
+                 loss_scale: float, seed: int, device: str):
         if not torch.cuda.is_available():
-            raise RuntimeError("ShaderInputGradients needs a CUDA device (no CPU fallback)")
+            raise RuntimeError(f"{type(self).__name__} needs a CUDA device (no CPU fallback)")
         self.B, self.size, self.new_size = batch, size, new_size
-        self.is_greyscale = is_greyscale
         self.loss_scale = float(loss_scale)
         self.device = torch.device(device)
         self.store = tf.VariableStore(precision=precision, device=str(self.device) if self.device.index is not None else "cuda",
@@ -94,23 +97,7 @@ class ShaderInputGradients:
                 tf.load_weight_dict(weights)
         self._dgrad_cache: Dict[object, object] = {}
         self.tape = None
-        self.img = None
-
-    # ------------------------------------------------------------------------------------------- forward
-    def forward(self, voxels, view_params) -> torch.Tensor:
-        dev = self.store.device
-        self.view_params = np.asarray(view_params, np.float32)
-        self.vox = torch.as_tensor(np.asarray(voxels, np.float32)).reshape(self.B, self.size, self.size, self.size, 1).to(dev)
-        self.minv = torch.from_numpy(pose_to_matrix(self.view_params, self.size, self.new_size)).to(dev)
-        self.tape = []
-        self.store.tape = self.tape
-        try:
-            with tf.use_store(self.store):
-                grid = ResampledGrid(self.vox, self.minv, self.new_size, transform=True)
-                self.img = RenderNet(grid, is_training=False, is_greyscale=self.is_greyscale)
-        finally:
-            self.store.tape = None
-        return self.img
+        self.last_dgrid = None
 
     # ------------------------------------------------------------------------------------------- packed gradient filters
     def _zeros(self, n):
@@ -199,81 +186,94 @@ class ShaderInputGradients:
             self._dgrad_cache[key] = a
         return a
 
-    # ------------------------------------------------------------------------------------------- backward
-    def backward(self, dimg, want_dvox: bool = True, want_dpose: bool = True, want_weight_grads: bool = False,
-                 tensor_core_wgrad: bool = True):
-        """dimg: dL/dimg [B,512,512,3|1] (NumPy or tensor).  Returns (dL/dvoxels [B,S,S,S,1] or None, dL/dview_params [B,3] or None).
-        want_weight_grads: also fills `self.weight_grads` {variable name: fp32 device tensor in the variable's TF layout} for EVERY
-        variable the forward pass used -- filters (wgmma weight-gradient kernel for the wide stride-1 2-D layers and, depth-folded,
-        the 3^3 layers; the strided-correlation kernel rn_conv_weight_grad_direct for the thin / strided / transposed ones), biases
-        and PReLU slopes (pre-activation recomputed: alpha starts at 0, tools/layer_util.py:38).  tensor_core_wgrad=False sends
-        every filter through the direct kernel (cross-check)."""
-        if self.tape is None:
-            raise RuntimeError("call forward() first")
-        dev = self.store.device
+    def _w32(self, w):
+        """fp32 device copy of a recorded filter (cached per variable)."""
+        key = ("w32", w._rn_name)
+        d = self._dgrad_cache.get(key)
+        if d is None:
+            d = w.to(device=self.store.device, dtype=torch.float32).contiguous()
+            self._dgrad_cache[key] = d
+        return d
+
+    # ------------------------------------------------------------------------------------------- reverse walk
+    def _reverse_walk(self, grads, want_weight_grads: bool, tensor_core_wgrad: bool):
+        """Walk the tape backwards from `grads` {_key(output): dL/doutput}.  16-bit layers take and give gradients carrying the
+        loss scale; the fused input record goes to `_input_chain`; the texture decoder's fp32 layers (records "conv_small",
+        "fc"), which come after it in the walk, take and give unscaled fp32 gradients."""
         fmt = self.store.fmt
-        dimg = torch.as_tensor(np.asarray(dimg, np.float32) if not isinstance(dimg, torch.Tensor) else dimg).to(dev).float()
-        if tuple(dimg.shape) != tuple(self.img.shape):
-            raise ValueError(f"dimg shape {tuple(dimg.shape)} != image shape {tuple(self.img.shape)}")
-        grads = {_key(self.img): dimg.contiguous()}
-        dgrid = None
-        self.weight_grads = {}
         inv = 1.0 / self.loss_scale
-        need_inputs = want_dvox or want_dpose
-        with torch.cuda.device(self.device), tf.use_store(self.store):
-            for rec in reversed(self.tape):
-                y = rec["y"]
-                g = grads.pop(_key(y), None)
-                if g is None:
-                    continue                                   # no gradient reaches this layer
-                if tuple(g.shape) != tuple(y.shape):           # the consumer saw a reshaped view (projection unit: [..,D,C] -> [..,D*C])
-                    g = g.reshape(tuple(y.shape))
-                if rec["op"] == "dropout":                     # d(x * mask / keep) = g * mask / keep: the same stateless kernel
-                    grads[_key(rec["x"])] = ops.dropout(g, rec["keep"], rec["seed"], rec["salt"])
-                    continue
-                act = rec["act"]
-                if act == "sigmoid":
-                    co = int(y.shape[-1])
-                    g = ops.sigmoid_backward(g, y, ops.round_up(co, 16), self.loss_scale, fmt)
-                elif act == "prelu":
-                    alpha = rec["alpha"]
-                    a_dev = self._alpha(alpha, int(y.shape[-1]))
-                    sign_src = y                    # the stored output tells the side of the kink as long as every slope is >= 0
-                    if not isinstance(alpha, str) and (want_weight_grads or self._has_negative_slope(alpha, a_dev)):
-                        # Re-run the layer without its PReLU to get the pre-activation z: dL/dalpha = sum_{z<0} g*z needs it (alpha
-                        # starts at 0), and so does the derivative itself once a slope is negative (y = alpha*z > 0 for z < 0;
-                        # Adam's first step already makes half of the slopes negative).
-                        sign_src = rec["rerun"]()
-                        if want_weight_grads:
-                            self.weight_grads[alpha._rn_name] = ops.prelu_alpha_grad(g, sign_src, inv)
-                    g = ops.prelu_backward(g, sign_src, a_dev)
-                if want_weight_grads:
-                    self._weight_grads_of(rec, g, inv, tensor_core_wgrad)
-                if rec["op"] == "resample_conv1":              # e_conv1 (5^3 s2, 1 -> 8) fused with the resampler in the forward pass
-                    if need_inputs:
-                        N = self.new_size
-                        w32 = rec["w"].to(dev).float().contiguous()
-                        dgrid = ops.conv3d_backward_data_direct(g, w32, (self.B, N, N, N, 1), rec["stride"], want32=True,
-                                                                out_scale=inv)
-                    continue
-                res = rec.get("residual")
-                if res is not None:                            # y = act(conv(x) + res): the gradient flows to res unchanged
-                    k = _key(res)
-                    grads[k] = ops.bias_act(g, None, None, None, residual=grads[k]) if k in grads else g
-                x = rec["x"]
-                acc = grads.pop(_key(x), None)                 # gradient already collected for x (fan-out): fused as `residual`
-                grads[_key(x)] = self._data_grad_of(rec, g, acc)
-            dvox = dminv = None
-            if need_inputs:
-                if dgrid is None:
-                    raise RuntimeError("the tape holds no fused resample + e_conv1 record (is this the Shader path?)")
-                dvox, dminv = ops.resample_backward(self.vox, self.minv, dgrid, True, want_dvox, want_dpose)
-            torch.cuda.synchronize()
-        self.last_dgrid = dgrid
-        dpose = None
-        if want_dpose:
-            dpose = pose_matrix_jacobian_vjp(self.view_params, dminv.cpu().numpy(), self.size, self.new_size)
-        return (dvox.cpu().numpy() if dvox is not None else None), dpose
+        for rec in reversed(self.tape):
+            y = rec["y"]
+            g = grads.pop(_key(y), None)
+            if g is None:
+                continue                                   # no gradient reaches this layer
+            if tuple(g.shape) != tuple(y.shape):           # the consumer saw a reshaped view (projection unit: [..,D,C] -> [..,D*C])
+                g = g.reshape(tuple(y.shape))
+            op = rec["op"]
+            if op == "copy":                               # a device copy made on the way into the resampler (_to_cuda_f32)
+                k = _key(rec["x"])
+                grads[k] = grads[k] + g if k in grads else g
+                continue
+            if op == "dropout":                            # d(x * mask / keep) = g * mask / keep: the same stateless kernel
+                grads[_key(rec["x"])] = ops.dropout(g, rec["keep"], rec["seed"], rec["salt"])
+                continue
+            if op in ("conv_small", "fc"):
+                self._decoder_step(rec, g, grads)
+                continue
+            act = rec["act"]
+            if act == "sigmoid":
+                co = int(y.shape[-1])
+                g = ops.sigmoid_backward(g, y, ops.round_up(co, 16), self.loss_scale, fmt)
+            elif act == "prelu":
+                alpha = rec["alpha"]
+                a_dev = self._alpha(alpha, int(y.shape[-1]))
+                sign_src = y                    # the stored output tells the side of the kink as long as every slope is >= 0
+                if not isinstance(alpha, str) and (want_weight_grads or self._has_negative_slope(alpha, a_dev)):
+                    # Re-run the layer without its PReLU to get the pre-activation z: dL/dalpha = sum_{z<0} g*z needs it (alpha
+                    # starts at 0), and so does the derivative itself once a slope is negative (y = alpha*z > 0 for z < 0;
+                    # Adam's first step already makes half of the slopes negative).
+                    sign_src = rec["rerun"]()
+                    if want_weight_grads:
+                        self.weight_grads[alpha._rn_name] = ops.prelu_alpha_grad(g, sign_src, inv)
+                g = ops.prelu_backward(g, sign_src, a_dev)
+            if want_weight_grads:
+                self._weight_grads_of(rec, g, inv, tensor_core_wgrad)
+            if op in ("resample_conv1", "resample5_conv1"):   # e_conv1 fused with the resampler(s) in the forward pass
+                self._input_chain(rec, g, grads)
+                continue
+            res = rec.get("residual")
+            if res is not None:                            # y = act(conv(x) + res): the gradient flows to res unchanged
+                k = _key(res)
+                grads[k] = ops.bias_act(g, None, None, None, residual=grads[k]) if k in grads else g
+            x = rec["x"]
+            acc = grads.pop(_key(x), None)                 # gradient already collected for x (fan-out): fused as `residual`
+            grads[_key(x)] = self._data_grad_of(rec, g, acc)
+
+    def _input_chain(self, rec, g, grads):
+        raise NotImplementedError
+
+    def _decoder_step(self, rec, g, grads):
+        """One texture-decoder layer (fp32, unscaled).  PReLU: once a layer has a negative slope the side of the kink comes from
+        the pre-activation (re-run without the activation): pretrained decoder slopes may be negative.  The data gradients need no kernel of their own: TF defines conv3d_transpose as the
+        input gradient of conv3d with the same filter array and padding, so the gradient of a conv3d is rn_conv3d_small
+        transposed on that array, the gradient of a conv3d_transpose is rn_conv3d_small forward on it (same stride), and the
+        gradient of fully_connected is rn_fully_connected_backward_data."""
+        act = rec["act"]
+        if act == "prelu":
+            alpha = rec["alpha"]
+            a_dev = self._alpha(alpha, int(rec["y"].shape[-1]))
+            # with every slope >= 0 the output's sign is the pre-activation's (z <= 0 -> y = alpha z <= 0), as in the trunk
+            neg = not isinstance(alpha, str) and self._has_negative_slope(alpha, a_dev)
+            g = ops.prelu_backward_f32(g, rec["rerun"]() if neg else rec["y"], a_dev)
+        elif act is not None:
+            raise NotImplementedError(f"no backward for a fused {act} on a texture-decoder layer")
+        w32 = self._w32(rec["w"])
+        if rec["op"] == "fc":
+            dx = ops.fully_connected_backward_data(g, w32)
+        else:
+            dx = ops.conv3d_small(g, w32, None, None, int(rec["stride"]), not rec["transposed"], want32=True)
+        k = _key(rec["x"])
+        grads[k] = grads[k] + dx if k in grads else dx
 
     def _data_grad_of(self, rec, g, acc=None):
         """dL/dx of one recorded convolution layer from g = dL/d(its pre-activation) (16-bit, carrying the loss scale); `acc`, a
@@ -346,3 +346,193 @@ class ShaderInputGradients:
             wg[w._rn_name] = d.permute(0, 1, 3, 2).contiguous()
         else:
             raise NotImplementedError(f"no weight-gradient path for {kind}")
+
+
+class ShaderInputGradients(_InputGradients):
+    """Forward + input-gradient backward of the Shader network for a fixed batch size.
+
+        ig = ShaderInputGradients(weights, batch=1, precision="exact")
+        img = ig.forward(voxels, view_params)                 # [B,512,512,3] fp32 on the device (tape recorded)
+        dvox, dpose = ig.backward(dL_dimg)                    # [B,64,64,64,1], [B,3] fp32 (NumPy)
+
+    `weights`: {tf variable name: array} or None (seeded reference initialisers)."""
+
+    def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str = "exact", is_greyscale: bool = False,
+                 size: int = 64, new_size: int = 128, loss_scale: float = 4096.0, seed: int = 0, device: str = "cuda"):
+        super().__init__(weights, batch, precision, size, new_size, loss_scale, seed, device)
+        self.is_greyscale = is_greyscale
+        self.img = None
+
+    # ------------------------------------------------------------------------------------------- forward
+    def forward(self, voxels, view_params) -> torch.Tensor:
+        dev = self.store.device
+        self.view_params = np.asarray(view_params, np.float32)
+        self.vox = torch.as_tensor(np.asarray(voxels, np.float32)).reshape(self.B, self.size, self.size, self.size, 1).to(dev)
+        self.minv = torch.from_numpy(pose_to_matrix(self.view_params, self.size, self.new_size)).to(dev)
+        self.tape = []
+        self.store.tape = self.tape
+        try:
+            with tf.use_store(self.store):
+                grid = ResampledGrid(self.vox, self.minv, self.new_size, transform=True)
+                self.img = RenderNet(grid, is_training=False, is_greyscale=self.is_greyscale)
+        finally:
+            self.store.tape = None
+        return self.img
+
+    # ------------------------------------------------------------------------------------------- backward
+    def backward(self, dimg, want_dvox: bool = True, want_dpose: bool = True, want_weight_grads: bool = False,
+                 tensor_core_wgrad: bool = True):
+        """dimg: dL/dimg [B,512,512,3|1] (NumPy or tensor).  Returns (dL/dvoxels [B,S,S,S,1] or None, dL/dview_params [B,3] or None).
+        want_weight_grads: also fills `self.weight_grads` {variable name: fp32 device tensor in the variable's TF layout} for EVERY
+        variable the forward pass used -- filters (wgmma weight-gradient kernel for the wide stride-1 2-D layers and, depth-folded,
+        the 3^3 layers; the strided-correlation kernel rn_conv_weight_grad_direct for the thin / strided / transposed ones), biases
+        and PReLU slopes (pre-activation recomputed: alpha starts at 0, tools/layer_util.py:38).  tensor_core_wgrad=False sends
+        every filter through the direct kernel (cross-check)."""
+        if self.tape is None:
+            raise RuntimeError("call forward() first")
+        dev = self.store.device
+        dimg = torch.as_tensor(np.asarray(dimg, np.float32) if not isinstance(dimg, torch.Tensor) else dimg).to(dev).float()
+        if tuple(dimg.shape) != tuple(self.img.shape):
+            raise ValueError(f"dimg shape {tuple(dimg.shape)} != image shape {tuple(self.img.shape)}")
+        grads = {_key(self.img): dimg.contiguous()}
+        self._dgrid = None
+        self.weight_grads = {}
+        self._need_inputs = want_dvox or want_dpose
+        with torch.cuda.device(self.device), tf.use_store(self.store):
+            self._reverse_walk(grads, want_weight_grads, tensor_core_wgrad)
+            dgrid = self._dgrid
+            dvox = dminv = None
+            if self._need_inputs:
+                if dgrid is None:
+                    raise RuntimeError("the tape holds no fused resample + e_conv1 record (is this the Shader path?)")
+                dvox, dminv = ops.resample_backward(self.vox, self.minv, dgrid, True, want_dvox, want_dpose)
+            torch.cuda.synchronize()
+        self.last_dgrid = dgrid
+        dpose = None
+        if want_dpose:
+            dpose = pose_matrix_jacobian_vjp(self.view_params, dminv.cpu().numpy(), self.size, self.new_size)
+        return (dvox.cpu().numpy() if dvox is not None else None), dpose
+
+    def _input_chain(self, rec, g, grads):
+        """e_conv1 (5^3 s2, 1 -> 8) fused with the resampler: its data gradient dL/dgrid, fp32 and un-scaled."""
+        if rec["op"] != "resample_conv1":
+            raise RuntimeError(f"a Shader tape cannot hold a {rec['op']} record")
+        if self._need_inputs:
+            N = self.new_size
+            w32 = rec["w"].to(self.store.device).float().contiguous()
+            self._dgrid = ops.conv3d_backward_data_direct(g, w32, (self.B, N, N, N, 1), rec["stride"], want32=True,
+                                                          out_scale=1.0 / self.loss_scale)
+
+
+class TextureInputGradients(_InputGradients):
+    """Forward + input-gradient backward of the Texture+Normal network (texture decoder -> two resamplings -> concat ->
+    RenderNet; RenderNet_Texture_Face_Normal.py:155-179) for a fixed batch size: the gradients face reconstruction descends
+    (Reconstruct_RenderNet_Face.py:383-412).
+
+        tig = TextureInputGradients(weights, batch=5, precision="exact")
+        albedo, normal = tig.forward(voxels, texture, view_params)        # [B,512,512,3] fp32 each, on the device
+        dvox, dtex, dpose = tig.backward(dL_dalbedo, dL_dnormal)          # [B,64,64,64,1], [B,199], [B,3] fp32 (NumPy)
+
+    model="texture": RenderNet_Texture_Face_Normal's decoder_texture + RenderNet, `weights` {tf variable name: array} or None
+    (seeded initialisers).  model="pretrained": Reconstruct_RenderNet_Face's texture_decoder_pretrained + RenderNet_pretrained
+    (ReLU residual blocks), `weights` the npz-keyed dictionary those functions read."""
+
+    def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str = "exact", model: str = "texture",
+                 size: int = 64, new_size: int = 128, loss_scale: float = 4096.0, seed: int = 0, device: str = "cuda"):
+        if model not in ("texture", "pretrained"):
+            raise ValueError(f"model must be 'texture' or 'pretrained', not {model!r}")
+        if model == "pretrained" and weights is None:
+            raise ValueError("model='pretrained' builds its variables from the npz-keyed weight dictionary: pass one")
+        super().__init__(weights if model == "texture" else None, batch, precision, size, new_size, loss_scale, seed, device)
+        self.model = model
+        self.weight_dict = weights if model == "pretrained" else None
+        self.albedo = self.normal = None
+
+    def forward(self, voxels, texture, view_params):
+        """voxels [B,64,64,64,1], texture [B,199], view_params [B,3] -> (albedo, normal), fp32 [B,512,512,3] on the device."""
+        from .RenderNet_Texture_Face_Normal import RenderNet as RenderNetTexture, decoder_texture
+        from .Reconstruct_RenderNet_Face import RenderNet_pretrained, texture_decoder_pretrained
+        dev = self.store.device
+        self.view_params = np.asarray(view_params, np.float32)
+        self.vox = torch.as_tensor(np.asarray(voxels, np.float32)).reshape(self.B, self.size, self.size, self.size, 1).to(dev)
+        self.tex_in = torch.as_tensor(np.asarray(texture, np.float32)).reshape(self.B, -1).to(dev).contiguous()
+        self.minv = torch.from_numpy(pose_to_matrix(self.view_params, self.size, self.new_size)).to(dev)
+        self.tape = []
+        self.store.tape = self.tape
+        try:
+            with tf.use_store(self.store):
+                if self.model == "texture":
+                    self.tex3d = tf.realize(decoder_texture(self.tex_in))
+                else:
+                    self.tex3d = tf.realize(texture_decoder_pretrained(self.tex_in, self.weight_dict))
+                # both resamplings stay deferred: resample x2 + axis transform + concat + e_conv1 run as one kernel, whose
+                # record holds the very tensors (geometry, decoded texture) the backward scatters into
+                grid = ConcatResampledGrid(ResampledGrid(self.vox, self.minv, self.new_size, transform=True),
+                                           ResampledGrid(self.tex3d, self.minv, self.new_size, transform=True))
+                if self.model == "texture":
+                    self.albedo, self.normal = RenderNetTexture(grid, is_training=False)
+                else:
+                    self.albedo, self.normal = RenderNet_pretrained(grid, self.weight_dict)
+        finally:
+            self.store.tape = None
+        return self.albedo, self.normal
+
+    def backward(self, d_albedo, d_normal, want_dvox: bool = True, want_dtex: bool = True, want_dpose: bool = True,
+                 want_weight_grads: bool = False):
+        """d_albedo, d_normal: dL/d(albedo), dL/d(normal map) [B,512,512,3] (NumPy or tensor; None = zero).  Returns
+        (dL/dvoxels [B,64,64,64,1], dL/dtexture [B,199], dL/dview_params [B,3]) as fp32 NumPy arrays, each None unless asked for."""
+        if want_weight_grads:
+            raise NotImplementedError("TextureInputGradients differentiates the inputs only: no weight gradients for the "
+                                      "Texture+Normal network")
+        if self.tape is None:
+            raise RuntimeError("call forward() first")
+        dev = self.store.device
+        grads = {}
+        for out, d in ((self.albedo, d_albedo), (self.normal, d_normal)):
+            if d is None:
+                continue
+            d = torch.as_tensor(np.asarray(d, np.float32) if not isinstance(d, torch.Tensor) else d).to(dev).float()
+            if tuple(d.shape) != tuple(out.shape):
+                raise ValueError(f"output gradient shape {tuple(d.shape)} != output shape {tuple(out.shape)}")
+            grads[_key(out)] = d.contiguous()
+        self._want = (want_dvox, want_dtex, want_dpose)
+        self._dvox = self._dminv = None
+        self._dtex_reached = False
+        self.last_dgrid = None
+        dtex = None
+        with torch.cuda.device(self.device), tf.use_store(self.store):
+            if grads and (want_dvox or want_dtex or want_dpose):
+                self._reverse_walk(grads, False, True)
+                if want_dtex:
+                    dtex = grads.pop(_key(self.tex_in), None)
+                    if dtex is None and self._dtex_reached:
+                        raise RuntimeError("dL/d(texture volume) was computed but never reached the texture vector: the tape "
+                                           "lost the link between the resampler and the texture decoder")
+            torch.cuda.synchronize()
+        B, S = self.B, self.size
+        dvox = dpose = None
+        if want_dvox:
+            dvox = self._dvox.cpu().numpy() if self._dvox is not None else np.zeros((B, S, S, S, 1), np.float32)
+        if want_dtex:
+            dtex = dtex.cpu().numpy() if dtex is not None else np.zeros(tuple(self.tex_in.shape), np.float32)
+        if want_dpose:
+            dminv = self._dminv.cpu().numpy() if self._dminv is not None else np.zeros((B, 3, 4), np.float32)
+            dpose = pose_matrix_jacobian_vjp(self.view_params, dminv, self.size, self.new_size)
+        return dvox, dtex, dpose
+
+    def _input_chain(self, rec, g, grads):
+        """e_conv1 (5^3 s2, 5 -> 8) fused with both resamplings: dL/d(concat) [B,N,N,N,5] fp32 from the thin data-gradient
+        kernel, then rn_resample5_backward_f32 -> dvox, dM^-1 and dL/d(decoded texture), which continues into the decoder."""
+        if rec["op"] != "resample5_conv1":
+            raise RuntimeError(f"a Texture tape cannot hold a {rec['op']} record")
+        want_dvox, want_dtex, want_dpose = self._want
+        grid = rec["grid"]
+        N = self.new_size
+        dgrid = ops.conv3d_backward_data_direct(g, self._w32(rec["w"]), (self.B, N, N, N, 5), rec["stride"], want32=True,
+                                                out_scale=1.0 / self.loss_scale)
+        self.last_dgrid = dgrid
+        self._dvox, dtex, self._dminv = ops.resample5_backward(grid.geom.voxel, grid.tex.voxel, grid.minv, dgrid, want_dvox,
+                                                               want_dtex, want_dpose)
+        if dtex is not None:
+            grads[_key(grid.tex.voxel)] = dtex
+            self._dtex_reached = True

@@ -303,9 +303,11 @@ def fully_connected(input_, output_size, reuse=False, scope='fully_connected', i
                                 _alpha_arg(alpha, None) if act == "prelu" else None, want32=True)
         if act not in (None, "prelu") or residual is not None:
             raise NotImplementedError("fully_connected: only a fused PReLU epilogue is supported")
+        _record(op="fc", x=xt, w=matrix, b=b, act=act, alpha=alpha, y=y,
+                rerun=lambda: ops.fully_connected(xt, wd, _dev_vec(b) if b is not None else None, None, want32=True))
         return y
 
-    return Deferred(run, (xin.shape[0], int(output_size)), torch.float32)
+    return Deferred(run, (xin.shape[0], int(matrix.shape[1])), torch.float32)   # an initializer's width wins (:337)
 
 
 # ------------------------------------------------------------------------------------------ slim look-alikes
@@ -457,10 +459,14 @@ def _deferred_small3d(x, w, b, stride, transposed):
         xt = realize(xin)
         if not xt.is_cuda:
             xt = xt.to(_store().device)
-        y = ops.conv3d_small(xt.contiguous(), _dev_f32(w), _dev_vec(b) if b is not None else None,
+        xt = xt.contiguous()
+        y = ops.conv3d_small(xt, _dev_f32(w), _dev_vec(b) if b is not None else None,
                              _alpha_arg(alpha, cout) if act == "prelu" else None, stride, transposed, want32=True)
         if act not in (None, "prelu") or residual is not None:
             raise NotImplementedError("thin conv3d: only a fused PReLU epilogue is supported")
+        _record(op="conv_small", transposed=transposed, stride=stride, x=xt, w=w, b=b, act=act, alpha=alpha, y=y,
+                rerun=lambda: ops.conv3d_small(xt, _dev_f32(w), _dev_vec(b) if b is not None else None, None, stride,
+                                               transposed, want32=True))     # the pre-activation z
         return y
 
     return Deferred(run, oshape, torch.float32)
@@ -507,8 +513,19 @@ def _deferred_direct3d(x, w, b, stride):
             # Texture net: resample (C=1) + resample (C=4) + concat + e_conv1 + bias + PReLU in one kernel
             bd = _dev_vec(b) if b is not None else torch.zeros(cout, device=wd.device, dtype=torch.float32)
             ad = _alpha_arg(alpha, cout) if act == "prelu" else None
-            return ops.resample5_conv1(xin.geom.voxel, xin.tex.voxel, xin.minv, xin.new_size, wd, bd, ad, tf.COMPUTE_DTYPE,
-                                       fmt=_store().fmt)
+
+            def z5():
+                return ops.resample5_conv1(xin.geom.voxel, xin.tex.voxel, xin.minv, xin.new_size, wd, bd, None, tf.COMPUTE_DTYPE,
+                                           fmt=_store().fmt)
+            if act == "prelu" and _store().tape is not None and _store().keep_preact and not isinstance(alpha, str):
+                z = z5()
+                y = ops.bias_act(z, None, _dev_vec(alpha), "prelu")         # training step: keep z (see _deferred_conv.run)
+                _record(op="resample5_conv1", grid=xin, w=w, b=b, act=act, alpha=alpha, stride=list(stride), y=y, rerun=lambda: z)
+                return y
+            y = ops.resample5_conv1(xin.geom.voxel, xin.tex.voxel, xin.minv, xin.new_size, wd, bd, ad, tf.COMPUTE_DTYPE,
+                                    fmt=_store().fmt)
+            _record(op="resample5_conv1", grid=xin, w=w, b=b, act=act, alpha=alpha, stride=list(stride), y=y, rerun=z5)
+            return y
         xt = realize(xin)
         if not xt.is_cuda:
             xt = xt.to(_store().device)

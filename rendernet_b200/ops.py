@@ -799,6 +799,76 @@ def resample_backward(vox: torch.Tensor, minv: torch.Tensor, gout: torch.Tensor,
     return dvox, dminv
 
 
+def resample5_backward(vox: torch.Tensor, tex: torch.Tensor, minv: torch.Tensor, gout: torch.Tensor, want_dvox: bool = True,
+                       want_dtex: bool = True, want_dminv: bool = True):
+    """Backward of `resample5_conv1`'s input chain (rn_resample5_backward_f32): gout = dL/d(concat) fp32 [B,N,N,N,5] ->
+    (dvox [B,S,S,S,1], dtex [B,S,S,S,4], dminv [B,3,4]), fp32, each None unless asked for."""
+    vox, tex, minv, gout = (_cuda(t, torch.float32) for t in (vox, tex, minv, gout))
+    B, S = vox.shape[0], vox.shape[1]
+    N = gout.shape[1]
+    if (tuple(vox.shape) != (B, S, S, S, 1) or tuple(tex.shape) != (B, S, S, S, 4) or tuple(minv.shape) != (B, 3, 4)
+            or tuple(gout.shape) != (B, N, N, N, 5)):
+        raise ValueError(f"resample5_backward: unsupported shapes {tuple(vox.shape)}, {tuple(tex.shape)}, {tuple(gout.shape)}")
+    dvox = torch.zeros_like(vox) if want_dvox else None
+    dtex = torch.zeros_like(tex) if want_dtex else None
+    dminv = torch.zeros_like(minv) if want_dminv else None
+    check(lib.rn_resample5_backward_f32(vox.data_ptr(), tex.data_ptr(), minv.data_ptr(), gout.data_ptr(), _ptr(dvox), _ptr(dtex),
+                                        _ptr(dminv), B, S, N, _stream()), "rn_resample5_backward_f32")
+    return dvox, dtex, dminv
+
+
+def prelu_backward_f32(g: torch.Tensor, z: torch.Tensor, alpha: torch.Tensor) -> torch.Tensor:
+    """dL/dz = g * (z > 0 ? 1 : alpha[c]) on fp32 tensors (rn_prelu_backward_f32); z is the pre-activation, alpha fp32 [C]."""
+    g, z = _cuda(g, torch.float32), _cuda(z, torch.float32)
+    if tuple(g.shape) != tuple(z.shape):
+        raise ValueError(f"prelu_backward_f32: g {tuple(g.shape)} and z {tuple(z.shape)} differ")
+    C_ = g.shape[-1]
+    alpha = _cuda(alpha.to(device=g.device, dtype=torch.float32))
+    if alpha.numel() < C_:
+        raise ValueError(f"prelu_backward_f32: {alpha.numel()} slopes for {C_} channels")
+    out = torch.empty_like(g)
+    check(lib.rn_prelu_backward_f32(g.data_ptr(), z.data_ptr(), alpha.data_ptr(), out.data_ptr(), g.numel(), C_, _stream()),
+          "rn_prelu_backward_f32")
+    return out
+
+
+def fully_connected_backward_data(g: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
+    """dx = g @ w.T (rn_fully_connected_backward_data): g fp32 [B,N], w fp32 [K,N] (TF layout) -> fp32 [B,K], reproducible bit
+    for bit (fixed-order split-N reduction)."""
+    g, w = _cuda(g, torch.float32), _cuda(w, torch.float32)
+    B, N = g.shape
+    K = w.shape[0]
+    if tuple(w.shape) != (K, N):
+        raise ValueError(f"fully_connected_backward_data: w {tuple(w.shape)} does not match g {tuple(g.shape)}")
+    work = torch.empty(int(lib.rn_fully_connected_backward_workspace(B, K, N)), device=g.device, dtype=torch.float32)
+    dx = torch.empty((B, K), device=g.device, dtype=torch.float32)
+    check(lib.rn_fully_connected_backward_data(g.data_ptr(), w.data_ptr(), work.data_ptr(), dx.data_ptr(), B, K, N, _stream()),
+          "rn_fully_connected_backward_data")
+    return dx
+
+
+def phong_recon_loss_grad(albedo: torch.Tensor, normal: torch.Tensor, target: torch.Tensor, light_dir: torch.Tensor,
+                          light_col: torch.Tensor, ambient: float = 0.0, k_diffuse: float = 1.0, black_background: bool = False,
+                          with_mask: bool = True):
+    """Face reconstruction objective (rn_phong_recon_loss_grad): loss[b] = mean (target - albedo * tf_phong_composite(normal,
+    light_dir, light_col, ...))^2 and its gradients.  albedo, normal, target fp32 [B,H,W,3]; light_dir, light_col [B,3] (or [1,3]).
+    Returns (loss fp64 [B], d_albedo, d_normal fp32 [B,H,W,3], d_light_dir fp32 [B,3])."""
+    albedo, normal, target = (_cuda(t, torch.float32) for t in (albedo, normal, target))
+    B, H, W, C3 = albedo.shape
+    if C3 != 3 or tuple(normal.shape) != tuple(albedo.shape) or tuple(target.shape) != tuple(albedo.shape):
+        raise ValueError(f"phong_recon_loss_grad: shapes {tuple(albedo.shape)}, {tuple(normal.shape)}, {tuple(target.shape)}")
+    ld, lc = (_cuda(t.to(device=albedo.device, dtype=torch.float32).reshape(-1, 3).expand(B, 3).contiguous(), torch.float32)
+              for t in (light_dir, light_col))
+    loss = torch.zeros(B, device=albedo.device, dtype=torch.float64)
+    d_albedo, d_normal = torch.empty_like(albedo), torch.empty_like(albedo)
+    d_light = torch.zeros((B, 3), device=albedo.device, dtype=torch.float32)
+    check(lib.rn_phong_recon_loss_grad(albedo.data_ptr(), normal.data_ptr(), target.data_ptr(), ld.data_ptr(), lc.data_ptr(),
+                                       float(ambient), float(k_diffuse), 1 if black_background else 0, 1 if with_mask else 0,
+                                       loss.data_ptr(), d_albedo.data_ptr(), d_normal.data_ptr(), d_light.data_ptr(), B, H, W,
+                                       _stream()), "rn_phong_recon_loss_grad")
+    return loss, d_albedo, d_normal, d_light
+
+
 def conv2d_weight_grad(x, g, kh: int, kw: int) -> torch.Tensor:
     """dW of a stride-1 SAME conv2d on the tensor cores (rn_conv2d_weight_grad): x 16-bit [B,H,W,Cin] (layer input), g 16-bit
     [B,H,W,Cout] (gradient of the conv output), same 16-bit format -> fp32 [kh,kw,Cin,Cout] (TF filter layout)."""

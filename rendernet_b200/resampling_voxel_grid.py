@@ -14,6 +14,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .tfcompat import get_store
 
 
 def _np32(x) -> np.ndarray:
@@ -136,7 +137,12 @@ def _to_cuda_f32(x) -> torch.Tensor:
         x = x.realize()
     if not isinstance(x, torch.Tensor):
         x = torch.from_numpy(np.ascontiguousarray(np.asarray(x, dtype=np.float32)))
-    return x.to(device="cuda", dtype=torch.float32).contiguous()
+    y = x.to(device="cuda", dtype=torch.float32).contiguous()
+    if y.data_ptr() != x.data_ptr():
+        tape = get_store().tape
+        if tape is not None:                        # backward.py follows tensors by storage address: map the copy to its source
+            tape.append(dict(op="copy", x=x, y=y))
+    return y
 
 
 def tf_resampling(voxel_array, transformation_matrix, params=None, Scale_matrix=None, size=64, new_size=128):
