@@ -38,6 +38,7 @@ extern "C" {
 #define RN_ACT_NONE 0
 #define RN_ACT_PRELU 1   /* max(0,x) + alpha[c]*min(0,x)    tools/layer_util.py:27-45 */
 #define RN_ACT_SIGMOID 2 /* tf.nn.sigmoid                   RenderNet_Shader.py:127,130 */
+#define RN_ACT_ELU 3     /* tf.nn.elu: x < 0 ? exp(x) - 1 : x   Reconstruct_RenderNet_Face.py:48-69 (rn_conv3d_f32 only) */
 
 int rn_version(void);
 const char* rn_error_string(int code);
@@ -311,6 +312,22 @@ int rn_phong_recon_loss_grad(const float* albedo, const float* normal, const flo
                              void* stream);
 long long rn_fully_connected_backward_workspace(int B, int K, int N);
 int rn_fully_connected_backward_data(const float* g, const float* w, float* work, float* dx, int B, int K, int N, void* stream);
+
+/* ---- face-reconstruction shape decoder (Reconstruct_RenderNet_Face.py:31-75, decoder_3d_pretrained) --------------------------
+ * fp32 conv3d / conv3d_transpose with a cubic k = 4 kernel, TF SAME, any channel count up to 512, B <= 32, x [B,H,W,D,Cin] and
+ * out channel-last, out = act(conv + bias) with act RN_ACT_NONE / RN_ACT_ELU / RN_ACT_SIGMOID (bias may be NULL).  Replaces
+ * the reference's conv3d_transpose k4 s2 + tf.nn.elu (g_conv1..4, :47-69) and conv3d_transpose k4 s1 + tf.nn.sigmoid (g_conv5,
+ * :71-74).  transposed = 1: filter [4,4,4,Cout,Cin], out [B,sH,sW,sD,Cout]; transposed = 0: tf.nn.conv3d, filter [4,4,4,Cin,Cout],
+ * out [B,ceil(H/s),...,Cout] -- which is also the data gradient of the transposed conv on the same filter array (TF defines
+ * conv3d_transpose as conv3d's input gradient).  Implicit GEMM on the CUDA cores; a stride-2 transposed conv runs as its 8 output
+ * phases.  Small-M shapes split K; `work` must then hold rn_conv3d_f32_workspace(...) floats (0 = no workspace needed, may be
+ * NULL).  No float atomics: the result is reproducible bit for bit.  rc -2: unsupported geometry. */
+long long rn_conv3d_f32_workspace(int B, int H, int W, int D, int Cin, int Cout, int stride, int transposed);
+int rn_conv3d_f32(const float* x, const float* w, const float* bias, float* out, float* work, int B, int H, int W, int D, int Cin,
+                  int Cout, int k, int stride, int transposed, int act, void* stream);
+/* fp32 activation derivative from the activation's OUTPUT y (n elements): act RN_ACT_ELU -> TF-1 EluGrad, y < 0 ? g * (y + 1) : g;
+ * RN_ACT_SIGMOID -> SigmoidGrad, g * y * (1 - y) (rn_sigmoid_backward writes 16-bit only). */
+int rn_act_backward_f32(const float* g, const float* y, float* out, long long n, int act, void* stream);
 
 /* ---- backward pass, stage 2: weight gradients (training step, RenderNet_Shader.py:159-167) -------------------------------
  * dW of a stride-1 SAME conv2d (slim.conv2d / layer_util.conv2d, tools/layer_util.py:147-184) on the tensor cores:

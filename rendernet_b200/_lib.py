@@ -88,6 +88,9 @@ SIGNATURES = {
     "rn_prelu_backward_f32": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _vp]),
     "rn_fully_connected_backward_workspace": (_ll, [_i, _i, _i]),
     "rn_fully_connected_backward_data": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "rn_conv3d_f32_workspace": (_ll, [_i] * 8),
+    "rn_conv3d_f32": (_i, [_vp, _vp, _vp, _vp, _vp] + [_i] * 10 + [_vp]),
+    "rn_act_backward_f32": (_i, [_vp, _vp, _vp, _ll, _i, _vp]),
     "rn_phong_recon_loss_grad": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "rn_conv2d_weight_grad": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "rn_bias_grad_16": (_i, [_vp, _vp, _ll, _i, _i, _vp]),

@@ -28,6 +28,11 @@ e_conv1: rn_resample5_backward_f32 splits dL/d(concat) into dL/dvoxels, dL/d(tex
 volume) continues, in fp32, through the texture decoder (rn_prelu_backward_f32, rn_conv3d_small, rn_fully_connected_backward_data)
 to dL/d(texture vector).
 
+The face-reconstruction shape decoder (ShapeDecoderGradients, Reconstruct_RenderNet_Face.decoder_3d_pretrained) is walked the same
+way, in fp32: ELU / sigmoid derivatives from the stored outputs (rn_act_backward_f32), each conv3d_transpose's data gradient a
+conv3d on the same filter array (rn_conv3d_f32), the FC's rn_fully_connected_backward_data, down to dL/dlatent.  The voxel grid is
+the seam between it and TextureInputGradients; dL/dvoxels can stay on the device between the two.
+
 Gradients travel in the activations' 16-bit format (fp16, or fp16 hi/lo pairs in the exact mode) with a loss scale to keep
 them inside fp16's range; they are un-scaled when they leave the tensor-core part (fp32 from there on).
 """
@@ -217,7 +222,7 @@ class _InputGradients:
             if op == "dropout":                            # d(x * mask / keep) = g * mask / keep: the same stateless kernel
                 grads[_key(rec["x"])] = ops.dropout(g, rec["keep"], rec["seed"], rec["salt"])
                 continue
-            if op in ("conv_small", "fc"):
+            if op in ("conv_small", "conv_f32", "fc"):
                 self._decoder_step(rec, g, grads)
                 continue
             act = rec["act"]
@@ -253,11 +258,13 @@ class _InputGradients:
         raise NotImplementedError
 
     def _decoder_step(self, rec, g, grads):
-        """One texture-decoder layer (fp32, unscaled).  PReLU: once a layer has a negative slope the side of the kink comes from
-        the pre-activation (re-run without the activation): pretrained decoder slopes may be negative.  The data gradients need no kernel of their own: TF defines conv3d_transpose as the
-        input gradient of conv3d with the same filter array and padding, so the gradient of a conv3d is rn_conv3d_small
-        transposed on that array, the gradient of a conv3d_transpose is rn_conv3d_small forward on it (same stride), and the
-        gradient of fully_connected is rn_fully_connected_backward_data."""
+        """One layer of the texture decoder or the shape decoder (fp32, unscaled).  PReLU: once a layer has a negative slope the
+        side of the kink comes from the pre-activation (re-run without the activation): pretrained decoder slopes may be negative.
+        ELU and sigmoid (shape decoder): TF-1's EluGrad / SigmoidGrad from the stored output (rn_act_backward_f32).  The data
+        gradients need no kernel of their own: TF defines conv3d_transpose as the input gradient of conv3d with the same filter
+        array and padding, so the gradient of a conv3d is the transposed conv on that array, the gradient of a conv3d_transpose
+        is the forward conv on it (same stride) -- rn_conv3d_small for the thin layers, rn_conv3d_f32 for the wide ones -- and
+        the gradient of fully_connected is rn_fully_connected_backward_data."""
         act = rec["act"]
         if act == "prelu":
             alpha = rec["alpha"]
@@ -265,11 +272,15 @@ class _InputGradients:
             # with every slope >= 0 the output's sign is the pre-activation's (z <= 0 -> y = alpha z <= 0), as in the trunk
             neg = not isinstance(alpha, str) and self._has_negative_slope(alpha, a_dev)
             g = ops.prelu_backward_f32(g, rec["rerun"]() if neg else rec["y"], a_dev)
+        elif act in ("elu", "sigmoid"):
+            g = ops.act_backward_f32(g, rec["y"], act)
         elif act is not None:
-            raise NotImplementedError(f"no backward for a fused {act} on a texture-decoder layer")
+            raise NotImplementedError(f"no backward for a fused {act} on a decoder layer")
         w32 = self._w32(rec["w"])
         if rec["op"] == "fc":
             dx = ops.fully_connected_backward_data(g, w32)
+        elif rec["op"] == "conv_f32":
+            dx = ops.conv3d_f32(g, w32, None, int(rec["stride"]), not rec["transposed"])
         else:
             dx = ops.conv3d_small(g, w32, None, None, int(rec["stride"]), not rec["transposed"], want32=True)
         k = _key(rec["x"])
@@ -449,12 +460,16 @@ class TextureInputGradients(_InputGradients):
         self.albedo = self.normal = None
 
     def forward(self, voxels, texture, view_params):
-        """voxels [B,64,64,64,1], texture [B,199], view_params [B,3] -> (albedo, normal), fp32 [B,512,512,3] on the device."""
+        """voxels [B,64,64,64,1], texture [B,199], view_params [B,3] -> (albedo, normal), fp32 [B,512,512,3] on the device.
+        voxels may be a CUDA tensor (e.g. the shape decoder's output): it is used in place, without a host round trip."""
         from .RenderNet_Texture_Face_Normal import RenderNet as RenderNetTexture, decoder_texture
         from .Reconstruct_RenderNet_Face import RenderNet_pretrained, texture_decoder_pretrained
         dev = self.store.device
         self.view_params = np.asarray(view_params, np.float32)
-        self.vox = torch.as_tensor(np.asarray(voxels, np.float32)).reshape(self.B, self.size, self.size, self.size, 1).to(dev)
+        if isinstance(voxels, torch.Tensor) and voxels.is_cuda:
+            self.vox = voxels.to(device=dev, dtype=torch.float32).reshape(self.B, self.size, self.size, self.size, 1).contiguous()
+        else:
+            self.vox = torch.as_tensor(np.asarray(voxels, np.float32)).reshape(self.B, self.size, self.size, self.size, 1).to(dev)
         self.tex_in = torch.as_tensor(np.asarray(texture, np.float32)).reshape(self.B, -1).to(dev).contiguous()
         self.minv = torch.from_numpy(pose_to_matrix(self.view_params, self.size, self.new_size)).to(dev)
         self.tape = []
@@ -478,9 +493,10 @@ class TextureInputGradients(_InputGradients):
         return self.albedo, self.normal
 
     def backward(self, d_albedo, d_normal, want_dvox: bool = True, want_dtex: bool = True, want_dpose: bool = True,
-                 want_weight_grads: bool = False):
+                 want_weight_grads: bool = False, dvox_on_device: bool = False):
         """d_albedo, d_normal: dL/d(albedo), dL/d(normal map) [B,512,512,3] (NumPy or tensor; None = zero).  Returns
-        (dL/dvoxels [B,64,64,64,1], dL/dtexture [B,199], dL/dview_params [B,3]) as fp32 NumPy arrays, each None unless asked for."""
+        (dL/dvoxels [B,64,64,64,1], dL/dtexture [B,199], dL/dview_params [B,3]) as fp32 NumPy arrays, each None unless asked for.
+        dvox_on_device: dL/dvoxels stays a CUDA tensor (for ShapeDecoderGradients.backward)."""
         if want_weight_grads:
             raise NotImplementedError("TextureInputGradients differentiates the inputs only: no weight gradients for the "
                                       "Texture+Normal network")
@@ -511,7 +527,9 @@ class TextureInputGradients(_InputGradients):
             torch.cuda.synchronize()
         B, S = self.B, self.size
         dvox = dpose = None
-        if want_dvox:
+        if want_dvox and dvox_on_device:
+            dvox = self._dvox if self._dvox is not None else torch.zeros((B, S, S, S, 1), device=dev, dtype=torch.float32)
+        elif want_dvox:
             dvox = self._dvox.cpu().numpy() if self._dvox is not None else np.zeros((B, S, S, S, 1), np.float32)
         if want_dtex:
             dtex = dtex.cpu().numpy() if dtex is not None else np.zeros(tuple(self.tex_in.shape), np.float32)
@@ -536,3 +554,51 @@ class TextureInputGradients(_InputGradients):
         if dtex is not None:
             grads[_key(grid.tex.voxel)] = dtex
             self._dtex_reached = True
+
+
+class ShapeDecoderGradients(_InputGradients):
+    """Forward + latent gradient of the face-reconstruction shape decoder (Reconstruct_RenderNet_Face.decoder_3d_pretrained,
+    reference :31-75) for a fixed batch size: the first link of `tf.gradients(recon_loss, initial_vector)` (:402).
+
+        sdg = ShapeDecoderGradients(weight_dict_decoder, batch=5)
+        vox = sdg.forward(latent)                 # [B,64,64,64,1] fp32 on the device (tape recorded)
+        dlatent = sdg.backward(dvox)              # [B,200] fp32 (NumPy); dvox NumPy or a CUDA tensor
+
+    Every layer is fp32 on the CUDA cores (rn_fully_connected, rn_conv3d_f32), whatever the Texture+Normal network's precision,
+    so the object has no precision of its own.  `weight_dict`: the decoder's npz-keyed arrays (g_zP_g_gc1_weights, ...)."""
+
+    def __init__(self, weight_dict: Dict[str, np.ndarray], batch: int, device: str = "cuda"):
+        super().__init__(None, batch, "exact", 64, 128, 1.0, 0, device)
+        self.weight_dict = weight_dict
+        self.vox = None
+
+    def forward(self, latent) -> torch.Tensor:
+        from .Reconstruct_RenderNet_Face import decoder_3d_pretrained
+        dev = self.store.device
+        lat = latent if isinstance(latent, torch.Tensor) else torch.as_tensor(np.asarray(latent, np.float32))
+        self.latent = lat.to(device=dev, dtype=torch.float32).reshape(self.B, -1).contiguous()
+        self.tape = []
+        self.store.tape = self.tape
+        try:
+            with torch.cuda.device(self.device), tf.use_store(self.store):
+                self.vox = tf.realize(decoder_3d_pretrained(self.latent, self.weight_dict))
+        finally:
+            self.store.tape = None
+        return self.vox
+
+    def backward(self, dvox) -> np.ndarray:
+        """dvox: dL/dvoxels [B,64,64,64,1] -> dL/dlatent [B,200] fp32 (NumPy)."""
+        if self.tape is None:
+            raise RuntimeError("call forward() first")
+        dev = self.store.device
+        d = torch.as_tensor(np.asarray(dvox, np.float32) if not isinstance(dvox, torch.Tensor) else dvox).to(dev).float()
+        if tuple(d.shape) != tuple(self.vox.shape):
+            raise ValueError(f"dvox shape {tuple(d.shape)} != voxel shape {tuple(self.vox.shape)}")
+        grads = {_key(self.vox): d.contiguous()}
+        with torch.cuda.device(self.device), tf.use_store(self.store):
+            self._reverse_walk(grads, False, True)
+            dz = grads.pop(_key(self.latent), None)
+            if dz is None:
+                raise RuntimeError("the shape decoder's tape lost the link between the voxels and the latent vector")
+            out = dz.cpu().numpy()
+        return out

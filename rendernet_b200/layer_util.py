@@ -264,7 +264,7 @@ def conv3d_transpose(x, num_output, kernel_size=(4, 4), stride=(1, 1), pad='SAME
                      scope="conv3d_transpose", trainable=True, weight_initializer=None, bias_initializer=None,
                      weight_initializer_type=None):
     """layer_util.py:269-309: tf.nn.conv3d_transpose SAME, out = in*stride, filter [k,k,k,Cout,Cin] (texture
-    decoder, BASELINE config 4).  Thin channels -> CUDA-core kernel, fp32 storage."""
+    decoder, BASELINE config 4; shape decoder).  Thin channels (<= 8) -> rn_conv3d_small; wider -> rn_conv3d_f32; fp32 storage."""
     _check_same(pad)
     if len(set(stride)) != 1 or len(set(kernel_size)) != 1:
         raise NotImplementedError("conv3d_transpose: cubic kernels / isotropic strides only")
@@ -275,6 +275,8 @@ def conv3d_transpose(x, num_output, kernel_size=(4, 4), stride=(1, 1), pad='SAME
         b = None
         if if_bias:
             b = bias_variable([int(num_output)], trainable=trainable, bias_initializer=bias_initializer)
+    if max(cin, int(num_output)) > 8:
+        return _deferred_f32_3d(x, w, b, int(stride[0]), True)
     return _deferred_small3d(x, w, b, int(stride[0]), True)
 
 
@@ -472,6 +474,32 @@ def _deferred_small3d(x, w, b, stride, transposed):
     return Deferred(run, oshape, torch.float32)
 
 
+def _deferred_f32_3d(x, w, b, stride, transposed):
+    """conv3d / conv3d_transpose with more than 8 channels and a 4^3 kernel (the shape decoder, Reconstruct_RenderNet_Face.py:31-75):
+    rn_conv3d_f32, fp32 storage, + bias + a fused tf.nn.elu / tf.nn.sigmoid."""
+    xin = x
+    cout = int(w.shape[3] if transposed else w.shape[4])
+    if tuple(int(v) for v in w.shape[:3]) != (4, 4, 4):
+        raise NotImplementedError(f"conv3d with {tuple(w.shape)} filters has no kernel (k = 4 only above 8 channels)")
+    if transposed:
+        oshape = (x.shape[0], x.shape[1] * stride, x.shape[2] * stride, x.shape[3] * stride, cout)
+    else:
+        oshape = (x.shape[0], -(-x.shape[1] // stride), -(-x.shape[2] // stride), -(-x.shape[3] // stride), cout)
+
+    def run(act, alpha, residual, want32):
+        if act not in (None, "elu", "sigmoid") or residual is not None:
+            raise NotImplementedError("fp32 conv3d: only a fused tf.nn.elu / tf.nn.sigmoid epilogue is supported")
+        xt = realize(xin)
+        if not isinstance(xt, torch.Tensor):
+            xt = torch.as_tensor(np.asarray(xt, np.float32))
+        xt = xt.to(device=_store().device, dtype=torch.float32).contiguous()
+        y = ops.conv3d_f32(xt, _dev_f32(w), _dev_vec(b) if b is not None else None, stride, transposed, act)
+        _record(op="conv_f32", transposed=transposed, stride=stride, x=xt, w=w, b=b, act=act, alpha=None, y=y)
+        return y
+
+    return Deferred(run, oshape, torch.float32)
+
+
 _DIRECT3D = {(1, 8, 5): True, (5, 8, 5): True, (2, 8, 3): True, (8, 16, 3): False, (8, 8, 3): False}  # needs fp32 input?
 
 
@@ -480,6 +508,8 @@ def _deferred_direct3d(x, w, b, stride):
     if key not in _DIRECT3D:
         if len(set(stride)) != 1:
             raise NotImplementedError(f"conv3d {key} with stride {stride} has no kernel")
+        if max(key[0], key[1]) > 8:
+            return _deferred_f32_3d(x, w, b, int(stride[0]), False)
         return _deferred_small3d(x, w, b, int(stride[0]), False)
     xin = x
     oshape = (x.shape[0], -(-x.shape[1] // stride[0]), -(-x.shape[2] // stride[1]), -(-x.shape[3] // stride[2]),

@@ -714,6 +714,54 @@ def conv3d_small(x, w_tf: torch.Tensor, bias: Optional[torch.Tensor], alpha: Opt
     return out if want32 else _wrap16(out, fmt)
 
 
+ACT_ELU = 3
+_ACT_F32 = {None: ACT_NONE, "none": ACT_NONE, "elu": ACT_ELU, "sigmoid": ACT_SIGMOID}
+
+
+def conv3d_f32(x: torch.Tensor, w_tf: torch.Tensor, bias: Optional[torch.Tensor], stride: int, transposed: bool,
+               act: Optional[str] = None) -> torch.Tensor:
+    """fp32 conv3d / conv3d_transpose, cubic k = 4, TF SAME, any channel count (rn_conv3d_f32: the shape decoder's layers and
+    their data gradients), + bias, then act None / "elu" / "sigmoid".  x fp32 [B,H,W,D,Cin]; w_tf fp32 [4,4,4,Cin,Cout] (forward)
+    or [4,4,4,Cout,Cin] (transposed).  Reproducible bit for bit."""
+    x, w_tf = _cuda(x, torch.float32), _cuda(w_tf, torch.float32)
+    if act not in _ACT_F32:
+        raise ValueError(f"conv3d_f32: activation {act!r} is not one of {sorted(k for k in _ACT_F32 if k)}")
+    B, H, W, D, Cin = (int(v) for v in x.shape)
+    if tuple(w_tf.shape[:3]) != (4, 4, 4):
+        raise ValueError(f"conv3d_f32: cubic k = 4 filters only, got {tuple(w_tf.shape)}")
+    wc = int(w_tf.shape[4] if transposed else w_tf.shape[3])
+    if wc != Cin:
+        raise ValueError(f"conv3d_f32: filter {tuple(w_tf.shape)} does not take {Cin} input channels")
+    Cout = int(w_tf.shape[3] if transposed else w_tf.shape[4])
+    s = int(stride)
+    oshape = (B, H * s, W * s, D * s, Cout) if transposed else (B, -(-H // s), -(-W // s), -(-D // s), Cout)
+    tr = 1 if transposed else 0
+    nwork = int(lib.rn_conv3d_f32_workspace(B, H, W, D, Cin, Cout, s, tr))
+    if nwork < 0:
+        check(int(nwork), "rn_conv3d_f32_workspace")
+    work = torch.empty(nwork, device=x.device, dtype=torch.float32) if nwork > 0 else None
+    if bias is not None:
+        bias = _cuda(bias, torch.float32)
+    out = torch.empty(oshape, device=x.device, dtype=torch.float32)
+    check(lib.rn_conv3d_f32(x.data_ptr(), w_tf.data_ptr(), _ptr(bias), out.data_ptr(), _ptr(work), B, H, W, D, Cin, Cout, 4, s, tr,
+                            _ACT_F32[act], _stream()), "rn_conv3d_f32")
+    return out
+
+
+def act_backward_f32(g: torch.Tensor, y: torch.Tensor, act: str) -> torch.Tensor:
+    """dL/dz from dL/dy and the activation's output y, fp32 (rn_act_backward_f32): "elu" -> y < 0 ? g (y + 1) : g (TF-1 EluGrad),
+    "sigmoid" -> g y (1 - y)."""
+    g, y = _cuda(g, torch.float32), _cuda(y, torch.float32)
+    if tuple(g.shape) != tuple(y.shape):
+        raise ValueError(f"act_backward_f32: g {tuple(g.shape)} and y {tuple(y.shape)} differ")
+    if act not in ("elu", "sigmoid"):
+        raise ValueError(f"act_backward_f32: no derivative for {act!r}")
+    out = torch.empty_like(g)
+    check(lib.rn_act_backward_f32(g.data_ptr(), y.data_ptr(), out.data_ptr(), g.numel(), _ACT_F32[act], _stream()),
+          "rn_act_backward_f32")
+    return out
+
+
 def concat_channels(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     """tf.concat([a, b], axis=-1) for fp32 channel-last tensors."""
     a = _cuda(a, torch.float32)

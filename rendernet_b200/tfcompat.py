@@ -1,6 +1,6 @@
 """GPU-backed stand-in for the handful of TensorFlow-1 idioms the reference's *model functions* use
 (RenderNet_Shader.py:32-131, tools/layer_util.py): variable scopes, `tf.get_variable`, `tf.add`,
-`tf.cast`, `tf.nn.dropout/sigmoid/relu`, `tf.cond`, `slim.conv2d(_transpose)`.
+`tf.cast`, `tf.nn.dropout/sigmoid/relu/elu`, `tf.cond`, `slim.conv2d(_transpose)`.
 
 Design: the reference builds a TF graph node by node; TF then runs each node as its own kernel.  Here
 each convolution call returns a *deferred* tensor (`Deferred`) whose epilogue is still open, so that the
@@ -322,6 +322,15 @@ class _NN:
             x.want32 = True            # the network output is float32 like the reference's
             return x
         return ops.bias_act(realize(x), None, None, "sigmoid", want32=True)
+
+    @staticmethod
+    def elu(x, name=None):
+        """tf.nn.elu (Reconstruct_RenderNet_Face.py:48-69), fused into the epilogue of the fp32 convolution that produces x."""
+        if isinstance(x, Deferred) and x.open and x.act is None and x.residual is None:
+            x.act = "elu"
+            return x
+        raise NotImplementedError("tf.nn.elu runs in the epilogue of the shape decoder's fp32 convolutions: apply it to an "
+                                  "unrealised conv3d / conv3d_transpose output")
 
     @staticmethod
     def relu(x):
