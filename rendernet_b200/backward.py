@@ -34,7 +34,10 @@ conv3d on the same filter array (rn_conv3d_f32), the FC's rn_fully_connected_bac
 the seam between it and TextureInputGradients; dL/dvoxels can stay on the device between the two.
 
 Gradients travel in the activations' 16-bit format (fp16, or fp16 hi/lo pairs in the exact mode) with a loss scale to keep
-them inside fp16's range; they are un-scaled when they leave the tensor-core part (fp32 from there on).
+them inside fp16's range; they are un-scaled when they leave the tensor-core part (fp32 from there on).  By default the scale
+is chosen per backward call (choose_loss_scale): the power of two that brings the largest |g * s(1 - s)| at the output heads
+to LOSS_SCALE_TARGET.  A power of two keeps every step of the walk exact under the scaling, so the result does not depend on
+the magnitude of dL/d(output) as long as nothing leaves fp16's range (DESIGN §4).
 """
 from __future__ import annotations
 
@@ -81,6 +84,46 @@ def pose_matrix_jacobian_vjp(view_params: np.ndarray, dminv: np.ndarray, size: i
     return vp.grad.numpy()
 
 
+# Where the adaptive loss scale puts the largest 16-bit gradient of the output heads.  On its way into the network the largest
+# gradient grows by up to 21x (the training walk's e_conv2 / e_conv3, dropout 0.75; 5.4x without dropout; measured with
+# scripts/grad_range.py, DESIGN §4): 2^9 keeps the largest interior gradient 6x below fp16's largest value, 65504.
+LOSS_SCALE_TARGET = 2.0 ** 9
+# An output gradient that still overflows is walked again at a 16x lower scale, at most this many times.
+OVERFLOW_RETRIES = 3
+
+
+def choose_loss_scale(amax: float, target: float = LOSS_SCALE_TARGET) -> float:
+    """The loss scale 2^floor(log2(target / amax)) for a backward walk whose largest scaled output-head gradient |g s (1 - s)|
+    is `amax`: scale * amax lies in (target / 2, target].  A power of two, within [2^-126, 2^126] (scale and 1 / scale are
+    normal fp32 numbers); amax = 0 (nothing to scale) gives 1.  A non-finite amax raises FloatingPointError."""
+    amax, target = float(amax), float(target)
+    if not (math.isfinite(target) and target > 0.0):
+        raise ValueError(f"the loss-scale target must be a positive finite number, not {target}")
+    if not math.isfinite(amax):
+        raise FloatingPointError(f"the output gradient is not finite (max |g s(1-s)| = {amax})")
+    if amax <= 0.0:
+        return 1.0
+    e = math.floor(math.log2(target) - math.log2(amax))
+    while math.ldexp(amax, e) > target:            # log2 is rounded: settle the floor exactly
+        e -= 1
+    while math.ldexp(amax, e + 1) <= target:
+        e += 1
+    return math.ldexp(1.0, max(-126, min(126, e)))
+
+
+def _loss_scale_mode(loss_scale) -> Optional[float]:
+    """None or "auto": the scale is chosen per backward call (returns None); a number: that fixed scale."""
+    if loss_scale is None or (isinstance(loss_scale, str) and loss_scale == "auto"):
+        return None
+    v = float(loss_scale)
+    if not (math.isfinite(v) and v > 0.0):
+        raise ValueError(f"loss_scale must be None, 'auto' or a positive finite number, not {loss_scale!r}")
+    return v
+
+
+def _all_finite(tensors) -> bool:
+    ts = [t for t in tensors if t is not None]
+    return not ts or bool(torch.stack([torch.isfinite(t).all() for t in ts]).all().item())
 
 
 class _InputGradients:
@@ -89,11 +132,14 @@ class _InputGradients:
     `_input_chain`, the fused resample + e_conv1 record that starts its network."""
 
     def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str, size: int, new_size: int,
-                 loss_scale: float, seed: int, device: str):
+                 loss_scale, seed: int, device: str):
         if not torch.cuda.is_available():
             raise RuntimeError(f"{type(self).__name__} needs a CUDA device (no CPU fallback)")
         self.B, self.size, self.new_size = batch, size, new_size
-        self.loss_scale = float(loss_scale)
+        self.loss_scale = _loss_scale_mode(loss_scale)     # None: chosen per backward call, with headroom target scale_target
+        self.scale_target = LOSS_SCALE_TARGET
+        self.overflow_retries = OVERFLOW_RETRIES
+        self.last_loss_scale = None                        # the scale the last walk used
         self.device = torch.device(device)
         self.store = tf.VariableStore(precision=precision, device=str(self.device) if self.device.index is not None else "cuda",
                                       seed=seed)
@@ -201,12 +247,41 @@ class _InputGradients:
         return d
 
     # ------------------------------------------------------------------------------------------- reverse walk
-    def _reverse_walk(self, grads, want_weight_grads: bool, tensor_core_wgrad: bool):
+    def _choose_scale(self, grads) -> float:
+        """The fixed loss scale, or choose_loss_scale of max |g s (1 - s)| over the sigmoid heads that `grads` reaches."""
+        if self.loss_scale is not None:
+            return self.loss_scale
+        amax = None
+        for rec in self.tape:
+            y = rec["y"]
+            if rec["op"] in ("conv_small", "conv_f32", "fc") or rec.get("act") != "sigmoid" or _key(y) not in grads:
+                continue
+            g = grads[_key(y)].reshape(tuple(y.shape))
+            a = torch.amax(torch.abs(g * y * (1.0 - y)))
+            amax = a if amax is None else torch.maximum(amax, a)
+        return 1.0 if amax is None else choose_loss_scale(amax.item(), self.scale_target)
+
+    def _walk_checked(self, walk):
+        """Run walk(shrink) -> the tensors it returns; shrink multiplies the chosen loss scale.  A non-finite result (an fp16
+        overflow inside the walk) raises FloatingPointError with a fixed scale; an adaptive scale is retried 16x lower, at
+        most `overflow_retries` times."""
+        shrink = 1.0
+        for _ in range(self.overflow_retries + 1):
+            if _all_finite(walk(shrink)):
+                return
+            if self.loss_scale is not None:
+                break
+            shrink /= 16.0
+        raise FloatingPointError(f"gradient overflow in the 16-bit backward pass at loss scale {self.last_loss_scale:g}")
+
+    def _reverse_walk(self, grads, want_weight_grads: bool, tensor_core_wgrad: bool, shrink: float = 1.0):
         """Walk the tape backwards from `grads` {_key(output): dL/doutput}.  16-bit layers take and give gradients carrying the
-        loss scale; the fused input record goes to `_input_chain`; the texture decoder's fp32 layers (records "conv_small",
-        "fc"), which come after it in the walk, take and give unscaled fp32 gradients."""
+        loss scale (`_choose_scale` times `shrink`, kept in last_loss_scale); the fused input record goes to `_input_chain`; the
+        texture decoder's fp32 layers (records "conv_small", "fc"), which come after it in the walk, take and give unscaled fp32
+        gradients."""
         fmt = self.store.fmt
-        inv = 1.0 / self.loss_scale
+        self.last_loss_scale = scale = self._choose_scale(grads) * shrink
+        inv = 1.0 / scale
         for rec in reversed(self.tape):
             y = rec["y"]
             g = grads.pop(_key(y), None)
@@ -228,7 +303,7 @@ class _InputGradients:
             act = rec["act"]
             if act == "sigmoid":
                 co = int(y.shape[-1])
-                g = ops.sigmoid_backward(g, y, ops.round_up(co, 16), self.loss_scale, fmt)
+                g = ops.sigmoid_backward(g, y, ops.round_up(co, 16), scale, fmt)
             elif act == "prelu":
                 alpha = rec["alpha"]
                 a_dev = self._alpha(alpha, int(y.shape[-1]))
@@ -366,10 +441,12 @@ class ShaderInputGradients(_InputGradients):
         img = ig.forward(voxels, view_params)                 # [B,512,512,3] fp32 on the device (tape recorded)
         dvox, dpose = ig.backward(dL_dimg)                    # [B,64,64,64,1], [B,3] fp32 (NumPy)
 
-    `weights`: {tf variable name: array} or None (seeded reference initialisers)."""
+    `weights`: {tf variable name: array} or None (seeded reference initialisers).  `loss_scale`: None / "auto" chooses it per
+    call (choose_loss_scale; an overflow is retried at a lower scale); a number fixes it (an overflow raises
+    FloatingPointError)."""
 
     def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str = "exact", is_greyscale: bool = False,
-                 size: int = 64, new_size: int = 128, loss_scale: float = 4096.0, seed: int = 0, device: str = "cuda"):
+                 size: int = 64, new_size: int = 128, loss_scale=None, seed: int = 0, device: str = "cuda"):
         super().__init__(weights, batch, precision, size, new_size, loss_scale, seed, device)
         self.is_greyscale = is_greyscale
         self.img = None
@@ -405,19 +482,29 @@ class ShaderInputGradients(_InputGradients):
         dimg = torch.as_tensor(np.asarray(dimg, np.float32) if not isinstance(dimg, torch.Tensor) else dimg).to(dev).float()
         if tuple(dimg.shape) != tuple(self.img.shape):
             raise ValueError(f"dimg shape {tuple(dimg.shape)} != image shape {tuple(self.img.shape)}")
-        grads = {_key(self.img): dimg.contiguous()}
-        self._dgrid = None
-        self.weight_grads = {}
+        dimg = dimg.contiguous()
         self._need_inputs = want_dvox or want_dpose
-        with torch.cuda.device(self.device), tf.use_store(self.store):
-            self._reverse_walk(grads, want_weight_grads, tensor_core_wgrad)
+        out = {}
+
+        def walk(shrink):
+            self._dgrid = None
+            self.weight_grads = {}
+            self._reverse_walk({_key(self.img): dimg}, want_weight_grads, tensor_core_wgrad, shrink)
             dgrid = self._dgrid
             dvox = dminv = None
             if self._need_inputs:
                 if dgrid is None:
                     raise RuntimeError("the tape holds no fused resample + e_conv1 record (is this the Shader path?)")
                 dvox, dminv = ops.resample_backward(self.vox, self.minv, dgrid, True, want_dvox, want_dpose)
+            out.update(dgrid=dgrid, dvox=dvox, dminv=dminv)
+            # every path of the walk reaches e_conv1's filter gradient: an overflow anywhere makes it non-finite
+            first = next((g for n, g in self.weight_grads.items() if n.endswith("e_conv1/e_conv1/weights")), None)
+            return dvox, dminv, first
+
+        with torch.cuda.device(self.device), tf.use_store(self.store):
+            self._walk_checked(walk)
             torch.cuda.synchronize()
+        dgrid, dvox, dminv = out["dgrid"], out["dvox"], out["dminv"]
         self.last_dgrid = dgrid
         dpose = None
         if want_dpose:
@@ -432,7 +519,7 @@ class ShaderInputGradients(_InputGradients):
             N = self.new_size
             w32 = rec["w"].to(self.store.device).float().contiguous()
             self._dgrid = ops.conv3d_backward_data_direct(g, w32, (self.B, N, N, N, 1), rec["stride"], want32=True,
-                                                          out_scale=1.0 / self.loss_scale)
+                                                          out_scale=1.0 / self.last_loss_scale)
 
 
 class TextureInputGradients(_InputGradients):
@@ -446,10 +533,10 @@ class TextureInputGradients(_InputGradients):
 
     model="texture": RenderNet_Texture_Face_Normal's decoder_texture + RenderNet, `weights` {tf variable name: array} or None
     (seeded initialisers).  model="pretrained": Reconstruct_RenderNet_Face's texture_decoder_pretrained + RenderNet_pretrained
-    (ReLU residual blocks), `weights` the npz-keyed dictionary those functions read."""
+    (ReLU residual blocks), `weights` the npz-keyed dictionary those functions read.  `loss_scale` as in ShaderInputGradients."""
 
     def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str = "exact", model: str = "texture",
-                 size: int = 64, new_size: int = 128, loss_scale: float = 4096.0, seed: int = 0, device: str = "cuda"):
+                 size: int = 64, new_size: int = 128, loss_scale=None, seed: int = 0, device: str = "cuda"):
         if model not in ("texture", "pretrained"):
             raise ValueError(f"model must be 'texture' or 'pretrained', not {model!r}")
         if model == "pretrained" and weights is None:
@@ -512,19 +599,29 @@ class TextureInputGradients(_InputGradients):
                 raise ValueError(f"output gradient shape {tuple(d.shape)} != output shape {tuple(out.shape)}")
             grads[_key(out)] = d.contiguous()
         self._want = (want_dvox, want_dtex, want_dpose)
-        self._dvox = self._dminv = None
-        self._dtex_reached = False
-        self.last_dgrid = None
-        dtex = None
+        out = {}
+
+        def walk(shrink):
+            self._dvox = self._dminv = None
+            self._dtex_reached = False
+            self.last_dgrid = None
+            g = dict(grads)
+            self._reverse_walk(g, False, True, shrink)
+            dtex = None
+            if want_dtex:
+                dtex = g.pop(_key(self.tex_in), None)
+                if dtex is None and self._dtex_reached:
+                    raise RuntimeError("dL/d(texture volume) was computed but never reached the texture vector: the tape "
+                                       "lost the link between the resampler and the texture decoder")
+            out["dtex"] = dtex
+            return self._dvox, dtex, self._dminv
+
+        out["dtex"] = self._dvox = self._dminv = self.last_dgrid = None
         with torch.cuda.device(self.device), tf.use_store(self.store):
             if grads and (want_dvox or want_dtex or want_dpose):
-                self._reverse_walk(grads, False, True)
-                if want_dtex:
-                    dtex = grads.pop(_key(self.tex_in), None)
-                    if dtex is None and self._dtex_reached:
-                        raise RuntimeError("dL/d(texture volume) was computed but never reached the texture vector: the tape "
-                                           "lost the link between the resampler and the texture decoder")
+                self._walk_checked(walk)
             torch.cuda.synchronize()
+        dtex = out["dtex"]
         B, S = self.B, self.size
         dvox = dpose = None
         if want_dvox and dvox_on_device:
@@ -547,7 +644,7 @@ class TextureInputGradients(_InputGradients):
         grid = rec["grid"]
         N = self.new_size
         dgrid = ops.conv3d_backward_data_direct(g, self._w32(rec["w"]), (self.B, N, N, N, 5), rec["stride"], want32=True,
-                                                out_scale=1.0 / self.loss_scale)
+                                                out_scale=1.0 / self.last_loss_scale)
         self.last_dgrid = dgrid
         self._dvox, dtex, self._dminv = ops.resample5_backward(grid.geom.voxel, grid.tex.voxel, grid.minv, dgrid, want_dvox,
                                                                want_dtex, want_dpose)
@@ -568,7 +665,7 @@ class ShapeDecoderGradients(_InputGradients):
     so the object has no precision of its own.  `weight_dict`: the decoder's npz-keyed arrays (g_zP_g_gc1_weights, ...)."""
 
     def __init__(self, weight_dict: Dict[str, np.ndarray], batch: int, device: str = "cuda"):
-        super().__init__(None, batch, "exact", 64, 128, 1.0, 0, device)
+        super().__init__(None, batch, "exact", 64, 128, 1.0, 0, device)          # fp32 walk: the scale is never applied
         self.weight_dict = weight_dict
         self.vox = None
 

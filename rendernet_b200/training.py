@@ -39,7 +39,10 @@ class ShaderTrainer(ShaderInputGradients):
         weights = tr.state_dict()                                                                      # {tf name: ndarray}
 
     learning_rate / decay_steps / keep_prob default to config_RenderNet.json (e_eta 1e-5, 100000, 1.0); beta1 = 0.5 as in
-    RenderNet_Shader.py:167, beta2 / epsilon are TF's defaults.  data_parallel=True (one process per GPU under torchrun, same
+    RenderNet_Shader.py:167, beta2 / epsilon are TF's defaults.  loss_scale=None (default) chooses the 16-bit gradients' scale
+    per step below the headroom target `scale_target`; an fp16 overflow halves that target and redoes the step with the same
+    dropout masks, and `growth_interval` overflow-free steps double it again, up to its initial value.  A fixed loss_scale is
+    halved on overflow instead.  data_parallel=True (one process per GPU under torchrun, same
     initial weights / seed on every rank; the rank is mixed into the dropout-mask seed): gradients are averaged over the
     ranks before Adam (rendernet_b200.parallel.all_reduce_gradients; its bucketing is tested on a 2-process gloo group, the
     multi-GPU step itself has not been run on GPUs in round 2)."""
@@ -47,10 +50,16 @@ class ShaderTrainer(ShaderInputGradients):
     def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str = "exact", is_greyscale: bool = False,
                  keep_prob: float = 1.0, learning_rate: float = 1e-5, decay_steps: int = 100000, decay_rate: float = 0.96,
                  beta1: float = 0.5, beta2: float = 0.999, epsilon: float = 1e-8, loss: Optional[str] = None,
-                 size: int = 64, new_size: int = 128, loss_scale: float = 4096.0, seed: int = 0, device: str = "cuda",
+                 size: int = 64, new_size: int = 128, loss_scale=None, seed: int = 0, device: str = "cuda",
                  data_parallel: bool = False):
         super().__init__(weights, batch, precision=precision, is_greyscale=is_greyscale, size=size, new_size=new_size,
                          loss_scale=loss_scale, seed=seed, device=device)
+        # dynamic loss scaling lives in step(): an overflow halves the headroom target (or a fixed scale) and redoes the step;
+        # after growth_interval steps without one the target doubles again, up to where it started
+        self.overflow_retries = 0
+        self.growth_interval = 1000
+        self._target_ceiling = self.scale_target
+        self._steps_since_overflow = 0
         self.data_parallel = bool(data_parallel)      # one process per GPU, `batch` items each: gradients averaged over the ranks
         if not 0.0 < keep_prob <= 1.0:
             raise ValueError("keep_prob must be in (0, 1]")
@@ -133,11 +142,8 @@ class ShaderTrainer(ShaderInputGradients):
         tgt = tgt.to(device=img.device, dtype=torch.float32).reshape(tuple(img.shape)).contiguous()
         with torch.cuda.device(self.device):
             loss, dimg = ops.image_loss_grad(img.contiguous(), tgt, self.loss_kind)
+        # an fp16 overflow in the walk raises FloatingPointError (overflow_retries = 0: step() chooses the next scale)
         self.backward(dimg, want_dvox=False, want_dpose=False, want_weight_grads=True)
-        # a 16-bit gradient that overflowed the loss scale turns into inf / NaN and reaches the first layer through every path
-        first = next((g for n, g in self.weight_grads.items() if n.endswith("e_conv1/e_conv1/weights")), None)
-        if first is not None and not bool(torch.isfinite(first).all().item()):
-            raise FloatingPointError(f"gradient overflow in the 16-bit backward pass at loss_scale={self.loss_scale:g}")
         missing = sorted(set(self.store.vars) - set(self.weight_grads))
         if missing:
             raise RuntimeError(f"{len(missing)} variables received no gradient, e.g. {missing[:3]}")
@@ -159,9 +165,18 @@ class ShaderTrainer(ShaderInputGradients):
                 overflow = bool(flag.item() > 0)
             if not overflow:
                 break
-            self.loss_scale *= 0.5
+            self._steps_since_overflow = 0
+            if self.loss_scale is None:
+                self.scale_target *= 0.5
+            else:
+                self.loss_scale *= 0.5
         else:
-            raise FloatingPointError("the backward pass overflows even at a loss scale of %g" % self.loss_scale)
+            raise FloatingPointError("the backward pass overflows even at a loss scale of %g" % self.last_loss_scale)
+        self._steps_since_overflow += 1
+        if (self.loss_scale is None and self._steps_since_overflow >= self.growth_interval
+                and self.scale_target < self._target_ceiling):
+            self.scale_target *= 2.0
+            self._steps_since_overflow = 0
         if dp:
             # data-parallel step: every rank holds the same variables and its own `batch` items; the mean loss over the global
             # batch is the mean of the per-rank means, so the gradients are averaged (NCCL all-reduce, bucketed) before Adam

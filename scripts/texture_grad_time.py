@@ -73,7 +73,7 @@ def run(W, label):
             g16 = ops.cast_to_16(torch.randn(B, 64, 64, 64, 8, device=dev), fmt=fmt)
             w32 = tig._w32(rec["w"])
             t_conv1 = timed(lambda: ops.conv3d_backward_data_direct(g16, w32, (B, 128, 128, 128, 5), (2, 2, 2), want32=True,
-                                                                    out_scale=1.0 / tig.loss_scale))
+                                                                    out_scale=1.0 / tig.last_loss_scale))
             dgrid = torch.randn(B, 128, 128, 128, 5, device=dev)
             minv = torch.from_numpy(pose_to_matrix(poses, 64, 128)).to(dev)
             t_res = timed(lambda: ops.resample5_backward(tig.vox, tig.tex3d, minv, dgrid))
