@@ -352,6 +352,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
     const int bf16 = p.ab_fmt;
     const int kblocks = p.kblocks;
     const int mma_per_kit = p.row_bytes >> 5;       // 32 B (= 16 elements) per k-step
+    const bool wide_k1 = ny == 1 && mma_per_kit == 4;
     const int kps = p.kps, stages = p.stages;
     // descriptor = constant high part | (smem address >> 4); all operand buffers are 1024-byte aligned
     const uint64_t desc_hi = make_smem_desc(0, p.row_bytes);
@@ -399,6 +400,18 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
           // needed rows first; the very first block of a tile is always a full one)
           const uint32_t half = HALF ? p.kb_half[kbi] : 0u;
           if (++kbi == kblocks) kbi = 0;
+          // One A tile and one B tile of 128-byte rows (no halo sharing; the trunk and most other layers): the four k16 steps
+          // are issued back to back from a fully unrolled loop, without the runtime ky / k-step loop and its predicates between
+          // the wgmmas.  Same MMAs in the same order as the general loop below, so the results are bit-identical.
+          if (!HALF && wide_k1) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+#pragma unroll
+              for (int s = 0; s < MS; ++s) wgmma_ss<BN>(acc[s][0], dak + s * ams16 + 2 * k, dbk + 2 * k, k == 0 ? scale_d : 1u, bf16);
+            scale_d = 1;
+            da += sub16;
+            continue;
+          }
           for (int ky = 0; ky < ny; ++ky) {       // operand ky = the halo shifted down by ky image rows
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
