@@ -348,13 +348,32 @@ int rn_bias_grad_16(const void* g, float* db, long long npix, int C, int fmt, vo
  * slim.conv2d): P = dL/d(conv output), Q = the layer's input, (pd,ph,pw) = TF SAME pad-before -> dW[tap][co][ci].  Transposed
  * conv (slim.conv2d_transpose, RenderNet_Shader.py:106-129; o = i*s + k - pb): P = the layer's input, Q = dL/d(output)
  * -> dW[tap][ci][co].  P is [B,Dp,Hp,Wp,Cap] with Ca <= Cap channels used, Q [B,Dq,Hq,Wq,Cbp]; fmtP / fmtQ: RN_FMT_F16,
- * RN_FMT_BF16, RN_FMT_F16X2 or 3 = fp32.  dW fp32, overwritten. */
+ * RN_FMT_BF16, RN_FMT_F16X2 or 3 = fp32.  dW fp32, overwritten.  (Ca,Cb) = (8,1), (16,3), (4,4), (4,8), (8,5) -- e_conv1 and
+ * e_conv11 of the Shader; e_tex_conv0, e_tex_conv1 / e_tex_conv2 (fp32 P and Q, RenderNet_Texture_Face_Normal.py:39-44) and
+ * e_conv1 (:51-52) of the Texture+Normal network -- run a thin kernel with the whole Ca x Cb block per thread. */
 int rn_conv_weight_grad_direct(const void* P, const void* Q, float* dW, int B, int Dp, int Hp, int Wp, int Ca, int Cap, int Dq,
                                int Hq, int Wq, int Cb, int Cbp, int kd, int kh, int kw, int sd, int sh, int sw, int pd, int ph,
                                int pw, int fmtP, int fmtQ, float scale, void* stream);
 /* PReLU slope gradient (tools/layer_util.py:27-45: y = max(0,z) + alpha*min(0,z)): dalpha[c] = scale * sum_{z<0} g*z over the
  * n elements (channel-last, n % C == 0) of g = dL/dy and the PRE-activation z, both 16-bit in `fmt`; dalpha fp32 [C], overwritten. */
 int rn_prelu_alpha_grad(const void* g, const void* z, float* dalpha, long long n, int C, int fmt, float scale, void* stream);
+/* Parameter gradient of the Texture+Normal network's FC + PReLU (e_tex_fc1, RenderNet_Texture_Face_Normal.py:37-38:
+ * y = prelu(x W + b; alpha), tools/layer_util.py:27-45,311-343) in one pass: x fp32 [B,K] (the texture vectors), gy = dL/dy,
+ * z = x W + b (pre-activation), both fp32 [B,N], alpha [N] ->
+ *   gz[b][n] = gy * (z > 0 ? 1 : alpha[n])          (may be NULL: not written)
+ *   dw[k][n] = sum_b x[b][k] gz[b][n]               (TF layout [K,N])
+ *   db[n]    = sum_b gz[b][n],   dalpha[n] = sum_{b: z<0} gy[b][n] z[b][n]
+ * all overwritten.  B <= 32 (rc -2), N % 4 == 0 and 16-byte aligned rows (rc -3).  Sums over b in a fixed order, no atomics:
+ * reproducible bit for bit. */
+int rn_fully_connected_param_grad(const float* x, const float* gy, const float* z, const float* alpha, float* gz, float* dw,
+                                  float* db, float* dalpha, int B, int K, int N, void* stream);
+/* fp32 PReLU derivative with the bias and slope gradients of a thin texture-decoder conv (e_tex_conv0..2,
+ * RenderNet_Texture_Face_Normal.py:39-44, conv3d(_transpose) + bias + prelu): gy = dL/dy, z = pre-activation, channel-last
+ * fp32 [n], C = 4 or 8 (rc -2), 16-byte aligned -> gz = gy * (z > 0 ? 1 : alpha[c]) [n], db[c] = sum gz, dalpha[c] =
+ * sum_{z<0} gy * z, all overwritten.  Register partials, one fp32 atomic per CTA and channel (db / dalpha: summation order
+ * varies between runs; gz is exact). */
+int rn_prelu_grad_f32(const float* gy, const float* z, const float* alpha, float* gz, float* db, float* dalpha, long long n, int C,
+                      void* stream);
 /* tf.nn.dropout (RenderNet_Shader.py:39...123): out[i] = x[i] / keep where hash(seed, salt, i) < keep * 2^32, else 0 (16-bit in
  * `fmt`, out may alias x).  Stateless: the same call on the gradient is the backward pass; rn_dropout_mask_host reproduces the
  * mask on the host (1 = kept).  salt = index of the dropout call within the step. */

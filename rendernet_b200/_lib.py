@@ -96,6 +96,8 @@ SIGNATURES = {
     "rn_bias_grad_16": (_i, [_vp, _vp, _ll, _i, _i, _vp]),
     "rn_conv_weight_grad_direct": (_i, [_vp, _vp, _vp] + [_i] * 22 + [_f, _vp]),
     "rn_prelu_alpha_grad": (_i, [_vp, _vp, _vp, _ll, _i, _i, _f, _vp]),
+    "rn_fully_connected_param_grad": (_i, [_vp] * 8 + [_i, _i, _i, _vp]),
+    "rn_prelu_grad_f32": (_i, [_vp] * 6 + [_ll, _i, _vp]),
     "rn_dropout_16": (_i, [_vp, _vp, _ll, _f, C.c_uint, C.c_uint, _i, _vp]),
     "rn_dropout_mask_host": (_i, [_vp, _ll, _f, C.c_uint, C.c_uint]),
     "rn_image_loss_grad": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),

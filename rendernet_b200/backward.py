@@ -298,7 +298,7 @@ class _InputGradients:
                 grads[_key(rec["x"])] = ops.dropout(g, rec["keep"], rec["seed"], rec["salt"])
                 continue
             if op in ("conv_small", "conv_f32", "fc"):
-                self._decoder_step(rec, g, grads)
+                self._decoder_step(rec, g, grads, want_weight_grads)
                 continue
             act = rec["act"]
             if act == "sigmoid":
@@ -332,15 +332,23 @@ class _InputGradients:
     def _input_chain(self, rec, g, grads):
         raise NotImplementedError
 
-    def _decoder_step(self, rec, g, grads):
+    def _decoder_step(self, rec, g, grads, want_weight_grads: bool = False):
         """One layer of the texture decoder or the shape decoder (fp32, unscaled).  PReLU: once a layer has a negative slope the
         side of the kink comes from the pre-activation (re-run without the activation): pretrained decoder slopes may be negative.
         ELU and sigmoid (shape decoder): TF-1's EluGrad / SigmoidGrad from the stored output (rn_act_backward_f32).  The data
         gradients need no kernel of their own: TF defines conv3d_transpose as the input gradient of conv3d with the same filter
         array and padding, so the gradient of a conv3d is the transposed conv on that array, the gradient of a conv3d_transpose
         is the forward conv on it (same stride) -- rn_conv3d_small for the thin layers, rn_conv3d_f32 for the wide ones -- and
-        the gradient of fully_connected is rn_fully_connected_backward_data."""
+        the gradient of fully_connected is rn_fully_connected_backward_data.
+
+        want_weight_grads (Texture+Normal training, PReLU layers only): the pre-activation (kept on the tape, or re-run) gives
+        dL/dz, db and dalpha in one pass (rn_prelu_grad_f32; the FC's rn_fully_connected_param_grad, which also gives dW), the
+        filter gradient comes from the thin correlation kernel (fp32 operands).  The gradients reaching the decoder are unscaled
+        fp32, so no 1/scale is applied.  The FC's data gradient -- dL/d(texture vector), an input of the network -- is skipped."""
         act = rec["act"]
+        if want_weight_grads:
+            self._decoder_weight_step(rec, g, grads)
+            return
         if act == "prelu":
             alpha = rec["alpha"]
             a_dev = self._alpha(alpha, int(rec["y"].shape[-1]))
@@ -359,6 +367,32 @@ class _InputGradients:
         else:
             dx = ops.conv3d_small(g, w32, None, None, int(rec["stride"]), not rec["transposed"], want32=True)
         k = _key(rec["x"])
+        grads[k] = grads[k] + dx if k in grads else dx
+
+    def _decoder_weight_step(self, rec, g, grads):
+        alpha, w, b, x = rec["alpha"], rec["w"], rec["b"], rec["x"]
+        if rec["act"] != "prelu" or isinstance(alpha, str) or b is None or rec["op"] not in ("fc", "conv_small"):
+            raise NotImplementedError(f"no weight gradients for a decoder {rec['op']} record with act {rec['act']!r}")
+        wg = self.weight_grads
+        z = rec["rerun"]()
+        a_dev = self._alpha(alpha, int(rec["y"].shape[-1]))
+        if rec["op"] == "fc":
+            _, wg[w._rn_name], wg[b._rn_name], wg[alpha._rn_name] = ops.fully_connected_param_grad(x, g, z, a_dev)
+            return
+        g, wg[b._rn_name], wg[alpha._rn_name] = ops.prelu_grad_f32(g, z, a_dev)
+        s = int(rec["stride"])
+        ks = tuple(int(v) for v in w.shape[:3])
+        if rec["transposed"]:                  # filter [k,k,k,co,ci]; o = i*s + k - pb: P = the layer's input, Q = dL/dz
+            co, ci = int(w.shape[3]), int(w.shape[4])
+            pad = tuple(ops.same_pad_before(int(x.shape[1 + i]) * s, ks[i], s) for i in range(3))
+            d = ops.conv_weight_grad_direct(x, g, ks, (s, s, s), pad, Ca=ci, Cb=co)                  # [k,k,k,ci,co]
+        else:                                  # filter [k,k,k,ci,co]: P = dL/dz, Q = the layer's input
+            ci, co = int(w.shape[3]), int(w.shape[4])
+            pad = tuple(ops.same_pad_before(int(x.shape[1 + i]), ks[i], s) for i in range(3))
+            d = ops.conv_weight_grad_direct(g, x, ks, (s, s, s), pad, Ca=co, Cb=ci)                  # [k,k,k,co,ci]
+        wg[w._rn_name] = d.permute(0, 1, 2, 4, 3).contiguous()
+        dx = ops.conv3d_small(g, self._w32(w), None, None, s, not rec["transposed"], want32=True)
+        k = _key(x)
         grads[k] = grads[k] + dx if k in grads else dx
 
     def _data_grad_of(self, rec, g, acc=None):
@@ -390,9 +424,15 @@ class _InputGradients:
         cout = int(w.shape[2]) if rec.get("kind") == "conv2d_transpose" else int(w.shape[-1])
         if b is not None:
             wg[b._rn_name] = ops.bias_grad(g)[:cout] * inv          # g may carry zero-padded channels (e_conv11: 3 of 16)
-        if rec["op"] == "resample_conv1":
-            # e_conv1 read the resampled grid straight out of the fused kernel: materialise it once for the correlation
-            q = ops.resample(rec["grid"].voxel, rec["grid"].minv, self.new_size, True)
+        if rec["op"] in ("resample_conv1", "resample5_conv1"):
+            # e_conv1 read the resampled grid straight out of the fused kernel: materialise it once for the correlation (the
+            # standalone resampler is bit-identical to the fused one); Texture+Normal: geometry and decoded texture, concatenated
+            grid = rec["grid"]
+            if rec["op"] == "resample_conv1":
+                q = ops.resample(grid.voxel, grid.minv, self.new_size, True)
+            else:
+                q = ops.concat_channels(ops.resample(grid.geom.voxel, grid.minv, self.new_size, True),
+                                        ops.resample(grid.tex.voxel, grid.minv, self.new_size, True))
             st = tuple(int(v) for v in rec["stride"])
             ks = tuple(int(v) for v in w.shape[:3])
             pad = tuple(ops.same_pad_before(self.new_size, ks[i], st[i]) for i in range(3))
@@ -549,8 +589,17 @@ class TextureInputGradients(_InputGradients):
     def forward(self, voxels, texture, view_params):
         """voxels [B,64,64,64,1], texture [B,199], view_params [B,3] -> (albedo, normal), fp32 [B,512,512,3] on the device.
         voxels may be a CUDA tensor (e.g. the shape decoder's output): it is used in place, without a host round trip."""
-        from .RenderNet_Texture_Face_Normal import RenderNet as RenderNetTexture, decoder_texture
-        from .Reconstruct_RenderNet_Face import RenderNet_pretrained, texture_decoder_pretrained
+        self._set_inputs(voxels, texture, view_params)
+        self.tape = []
+        self.store.tape = self.tape
+        try:
+            with tf.use_store(self.store):
+                self._record_network(is_training=False, prob=1.0)
+        finally:
+            self.store.tape = None
+        return self.albedo, self.normal
+
+    def _set_inputs(self, voxels, texture, view_params):
         dev = self.store.device
         self.view_params = np.asarray(view_params, np.float32)
         if isinstance(voxels, torch.Tensor) and voxels.is_cuda:
@@ -559,25 +608,23 @@ class TextureInputGradients(_InputGradients):
             self.vox = torch.as_tensor(np.asarray(voxels, np.float32)).reshape(self.B, self.size, self.size, self.size, 1).to(dev)
         self.tex_in = torch.as_tensor(np.asarray(texture, np.float32)).reshape(self.B, -1).to(dev).contiguous()
         self.minv = torch.from_numpy(pose_to_matrix(self.view_params, self.size, self.new_size)).to(dev)
-        self.tape = []
-        self.store.tape = self.tape
-        try:
-            with tf.use_store(self.store):
-                if self.model == "texture":
-                    self.tex3d = tf.realize(decoder_texture(self.tex_in))
-                else:
-                    self.tex3d = tf.realize(texture_decoder_pretrained(self.tex_in, self.weight_dict))
-                # both resamplings stay deferred: resample x2 + axis transform + concat + e_conv1 run as one kernel, whose
-                # record holds the very tensors (geometry, decoded texture) the backward scatters into
-                grid = ConcatResampledGrid(ResampledGrid(self.vox, self.minv, self.new_size, transform=True),
-                                           ResampledGrid(self.tex3d, self.minv, self.new_size, transform=True))
-                if self.model == "texture":
-                    self.albedo, self.normal = RenderNetTexture(grid, is_training=False)
-                else:
-                    self.albedo, self.normal = RenderNet_pretrained(grid, self.weight_dict)
-        finally:
-            self.store.tape = None
-        return self.albedo, self.normal
+
+    def _record_network(self, is_training: bool, prob: float):
+        """Decoder -> two deferred resamplings -> RenderNet under the current store and tape (is_training / prob: dropout)."""
+        from .RenderNet_Texture_Face_Normal import RenderNet as RenderNetTexture, decoder_texture
+        from .Reconstruct_RenderNet_Face import RenderNet_pretrained, texture_decoder_pretrained
+        if self.model == "texture":
+            self.tex3d = tf.realize(decoder_texture(self.tex_in))
+        else:
+            self.tex3d = tf.realize(texture_decoder_pretrained(self.tex_in, self.weight_dict))
+        # both resamplings stay deferred: resample x2 + axis transform + concat + e_conv1 run as one kernel, whose
+        # record holds the very tensors (geometry, decoded texture) the backward scatters into
+        grid = ConcatResampledGrid(ResampledGrid(self.vox, self.minv, self.new_size, transform=True),
+                                   ResampledGrid(self.tex3d, self.minv, self.new_size, transform=True))
+        if self.model == "texture":
+            self.albedo, self.normal = RenderNetTexture(grid, prob=prob, is_training=is_training)
+        else:
+            self.albedo, self.normal = RenderNet_pretrained(grid, self.weight_dict)
 
     def backward(self, d_albedo, d_normal, want_dvox: bool = True, want_dtex: bool = True, want_dpose: bool = True,
                  want_weight_grads: bool = False, dvox_on_device: bool = False):
@@ -585,8 +632,8 @@ class TextureInputGradients(_InputGradients):
         (dL/dvoxels [B,64,64,64,1], dL/dtexture [B,199], dL/dview_params [B,3]) as fp32 NumPy arrays, each None unless asked for.
         dvox_on_device: dL/dvoxels stays a CUDA tensor (for ShapeDecoderGradients.backward)."""
         if want_weight_grads:
-            raise NotImplementedError("TextureInputGradients differentiates the inputs only: no weight gradients for the "
-                                      "Texture+Normal network")
+            raise NotImplementedError("TextureInputGradients differentiates the inputs only: the weight gradients of the "
+                                      "Texture+Normal network come from training.TextureTrainer")
         if self.tape is None:
             raise RuntimeError("call forward() first")
         dev = self.store.device

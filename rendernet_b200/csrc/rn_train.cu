@@ -17,6 +17,7 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <initializer_list>
 
 #include "../../include/rendernet_b200.h"
 #include "rn_dropout_hash.h"
@@ -192,6 +193,114 @@ __global__ void __launch_bounds__(256) prelu_alpha_grad_kernel(const void* __res
     if (acc[c] != 0.f) atomicAdd(&dalpha[c], acc[c] * scale);
 }
 
+// Parameter gradient of the texture decoder's FC + PReLU (e_tex_fc1, RenderNet_Texture_Face_Normal.py:37-38) in one pass over
+// gy and z.  A thread owns four adjacent columns: gz = gy * (z > 0 ? 1 : alpha) of all BT (>= B, zero padded) rows stays in
+// registers, and dW[k][n..n+3] = sum_b x[b][k] gz[b][n..n+3] is one float4 store per k, x read as a broadcast from shared
+// memory.  blockIdx.x splits K (the CTAs of one column block run side by side and share gy / z in L2); only the K part 0
+// writes gz, db and dalpha.  Every sum runs over b in a fixed order: the result is reproducible bit for bit.
+template <int BT>
+__global__ void __launch_bounds__(128) fc_param_grad_kernel(const float* __restrict__ x, const float* __restrict__ gy,
+                                                            const float* __restrict__ z, const float* __restrict__ alpha,
+                                                            float* __restrict__ gz, float* __restrict__ dw, float* __restrict__ db,
+                                                            float* __restrict__ dalpha, int B, int K, int N, int kchunk) {
+  extern __shared__ float sx[];                     // [BT][kchunk], rows b >= B zero
+  const int k0 = blockIdx.x * kchunk;
+  const int kn = min(kchunk, K - k0);
+  for (int i = threadIdx.x; i < BT * kchunk; i += blockDim.x) {
+    const int b = i / kchunk, k = i % kchunk;
+    sx[i] = (b < B && k < kn) ? x[static_cast<long long>(b) * K + k0 + k] : 0.f;
+  }
+  __syncthreads();
+  const long long n = (static_cast<long long>(blockIdx.y) * blockDim.x + threadIdx.x) * 4;
+  if (n >= N) return;
+  const float4 a = *reinterpret_cast<const float4*>(alpha + n);
+  const bool first = blockIdx.x == 0;
+  float4 g[BT];
+  float4 sb = make_float4(0.f, 0.f, 0.f, 0.f), sa = sb;
+#pragma unroll
+  for (int b = 0; b < BT; ++b) {
+    g[b] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (b < B) {
+      const long long o = static_cast<long long>(b) * N + n;
+      const float4 gv = *reinterpret_cast<const float4*>(gy + o), zv = *reinterpret_cast<const float4*>(z + o);
+      g[b] = make_float4(zv.x > 0.f ? gv.x : gv.x * a.x, zv.y > 0.f ? gv.y : gv.y * a.y, zv.z > 0.f ? gv.z : gv.z * a.z,
+                         zv.w > 0.f ? gv.w : gv.w * a.w);
+      if (first) {
+        sb.x += g[b].x; sb.y += g[b].y; sb.z += g[b].z; sb.w += g[b].w;
+        if (zv.x < 0.f) sa.x = fmaf(gv.x, zv.x, sa.x);
+        if (zv.y < 0.f) sa.y = fmaf(gv.y, zv.y, sa.y);
+        if (zv.z < 0.f) sa.z = fmaf(gv.z, zv.z, sa.z);
+        if (zv.w < 0.f) sa.w = fmaf(gv.w, zv.w, sa.w);
+        if (gz) *reinterpret_cast<float4*>(gz + o) = g[b];
+      }
+    }
+  }
+  if (first) {
+    *reinterpret_cast<float4*>(db + n) = sb;
+    *reinterpret_cast<float4*>(dalpha + n) = sa;
+  }
+  for (int k = 0; k < kn; ++k) {
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int b = 0; b < BT; ++b) {
+      const float xv = sx[b * kchunk + k];
+      acc.x = fmaf(xv, g[b].x, acc.x); acc.y = fmaf(xv, g[b].y, acc.y);
+      acc.z = fmaf(xv, g[b].z, acc.z); acc.w = fmaf(xv, g[b].w, acc.w);
+    }
+    __stcs(reinterpret_cast<float4*>(dw + static_cast<long long>(k0 + k) * N + n), acc);     // streamed: dW is not re-read here
+  }
+}
+
+// fp32 PReLU derivative with the bias and slope gradients of a thin decoder conv (C = 4 or 8 channels, 16-byte aligned):
+// gz = gy * (z > 0 ? 1 : alpha[c]), db[c] += sum gz, dalpha[c] += sum_{z<0} gy * z.  A thread walks whole voxels and keeps the
+// 2C partial sums in registers; warp shuffles and shared memory reduce them, then one atomic per CTA and channel.
+template <int C>
+__global__ void __launch_bounds__(256) prelu_grad_f32_kernel(const float* __restrict__ gy, const float* __restrict__ z,
+                                                             const float* __restrict__ alpha, float* __restrict__ gz,
+                                                             float* __restrict__ db, float* __restrict__ dalpha, long long nvox) {
+  constexpr int Q = C / 4;
+  __shared__ float red[8][2 * C];
+  float a[C], sb[C], sa[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) { a[c] = alpha[c]; sb[c] = 0.f; sa[c] = 0.f; }
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long v = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; v < nvox; v += stride) {
+#pragma unroll
+    for (int q = 0; q < Q; ++q) {
+      const long long o = v * C + 4 * q;
+      const float4 gv = *reinterpret_cast<const float4*>(gy + o), zv = *reinterpret_cast<const float4*>(z + o);
+      const float gs[4] = {gv.x, gv.y, gv.z, gv.w}, zs[4] = {zv.x, zv.y, zv.z, zv.w};
+      float os[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int c = 4 * q + j;
+        os[j] = zs[j] > 0.f ? gs[j] : gs[j] * a[c];
+        sb[c] += os[j];
+        if (zs[j] < 0.f) sa[c] = fmaf(gs[j], zs[j], sa[c]);
+      }
+      *reinterpret_cast<float4*>(gz + o) = make_float4(os[0], os[1], os[2], os[3]);
+    }
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int c = 0; c < C; ++c) {
+    float u = sb[c], w = sa[c];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      u += __shfl_xor_sync(0xffffffffu, u, o);
+      w += __shfl_xor_sync(0xffffffffu, w, o);
+    }
+    if (lane == 0) { red[warp][c] = u; red[warp][C + c] = w; }
+  }
+  __syncthreads();
+  if (threadIdx.x < 2 * C) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s += red[w][threadIdx.x];
+    atomicAdd(threadIdx.x < C ? &db[threadIdx.x] : &dalpha[threadIdx.x - C], s);
+  }
+}
+
 __global__ void __launch_bounds__(256) dropout_kernel(const void* x, void* out, long long n, float keep,
                                                       unsigned long long threshold, uint32_t seed, uint32_t salt, int fmt) {
   const float inv = 1.0f / keep;
@@ -273,14 +382,21 @@ extern "C" int rn_conv_weight_grad_direct(const void* P, const void* Q, float* d
   p.a_tiles = (Ca + kTile - 1) / kTile;
   p.b_tiles = (Cb + kTile - 1) / kTile;
   p.scale = scale;
-  if ((Ca == 8 && Cb == 1) || (Ca == 16 && Cb == 3)) {               // thin layers: per-thread channel blocks, positions across threads
+  // thin layers: per-thread channel blocks, positions across threads.  Shader: e_conv1 (8,1), e_conv11 (16,3); Texture+Normal:
+  // e_tex_conv0 (4,4), e_tex_conv1 / e_tex_conv2 (4,8), e_conv1 (8,5)
+  const bool thin = (Ca == 8 && Cb == 1) || (Ca == 16 && Cb == 3) || (Ca == 4 && Cb == 4) || (Ca == 4 && Cb == 8) ||
+                    (Ca == 8 && Cb == 5);
+  if (thin) {
     long long nsplit = (132LL * 8 + taps - 1) / taps;
     const long long maxsplit = (p.npos + 255) / 256;
     if (nsplit > maxsplit) nsplit = maxsplit;
     if (nsplit < 1) nsplit = 1;
     dim3 grid(static_cast<unsigned>(nsplit), static_cast<unsigned>(taps));
-    if (Ca == 8) wgrad_thin_kernel<8, 1><<<grid, 256, 0, st>>>(p);
-    else wgrad_thin_kernel<16, 3><<<grid, 256, 0, st>>>(p);
+    if (Ca == 8 && Cb == 1) wgrad_thin_kernel<8, 1><<<grid, 256, 0, st>>>(p);
+    else if (Ca == 16) wgrad_thin_kernel<16, 3><<<grid, 256, 0, st>>>(p);
+    else if (Ca == 4 && Cb == 4) wgrad_thin_kernel<4, 4><<<grid, 256, 0, st>>>(p);
+    else if (Ca == 4) wgrad_thin_kernel<4, 8><<<grid, 256, 0, st>>>(p);
+    else wgrad_thin_kernel<8, 5><<<grid, 256, 0, st>>>(p);
     RN_COUNT_LAUNCH();
     return static_cast<int>(cudaGetLastError());
   }
@@ -303,6 +419,52 @@ extern "C" int rn_prelu_alpha_grad(const void* g, const void* z, float* dalpha, 
   cudaError_t e = cudaMemsetAsync(dalpha, 0, static_cast<size_t>(C) * sizeof(float), st);
   if (e != cudaSuccess) return static_cast<int>(e);
   prelu_alpha_grad_kernel<<<grid_for(n, 256 * 16), 256, static_cast<size_t>(C) * sizeof(float), st>>>(g, z, dalpha, n, C, fmt, scale);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int rn_fully_connected_param_grad(const float* x, const float* gy, const float* z, const float* alpha, float* gz,
+                                             float* dw, float* db, float* dalpha, int B, int K, int N, void* stream) {
+  if (!x || !gy || !z || !alpha || !dw || !db || !dalpha || B < 1 || K < 1 || N < 1) return -1;
+  if (B > 32) return -2;
+  if (N % 4 != 0) return -3;
+  for (const void* q : {static_cast<const void*>(gy), static_cast<const void*>(z), static_cast<const void*>(alpha),
+                        static_cast<const void*>(gz), static_cast<const void*>(dw), static_cast<const void*>(db),
+                        static_cast<const void*>(dalpha)})
+    if ((reinterpret_cast<uintptr_t>(q) & 15) != 0) return -3;                   // float4 rows
+  const int kparts = (K + 63) / 64;
+  const int kchunk = (K + kparts - 1) / kparts;
+  const int BT = B <= 4 ? 4 : B <= 8 ? 8 : B <= 16 ? 16 : B <= 24 ? 24 : 32;
+  const size_t smem = static_cast<size_t>(BT) * kchunk * sizeof(float);           // <= 8 KB
+  const dim3 grid(static_cast<unsigned>(kparts), static_cast<unsigned>((N / 4 + 127) / 128));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+#define RN_FCPG(T) fc_param_grad_kernel<T><<<grid, 128, smem, st>>>(x, gy, z, alpha, gz, dw, db, dalpha, B, K, N, kchunk)
+  switch (BT) {
+    case 4: RN_FCPG(4); break;
+    case 8: RN_FCPG(8); break;
+    case 16: RN_FCPG(16); break;
+    case 24: RN_FCPG(24); break;
+    default: RN_FCPG(32); break;
+  }
+#undef RN_FCPG
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int rn_prelu_grad_f32(const float* gy, const float* z, const float* alpha, float* gz, float* db, float* dalpha,
+                                 long long n, int C, void* stream) {
+  if (!gy || !z || !alpha || !gz || !db || !dalpha || n < 1 || n % C != 0) return -1;
+  if (C != 4 && C != 8) return -2;
+  for (const float* q : {gy, z, static_cast<const float*>(gz)})
+    if ((reinterpret_cast<uintptr_t>(q) & 15) != 0) return -3;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaMemsetAsync(db, 0, static_cast<size_t>(C) * sizeof(float), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(dalpha, 0, static_cast<size_t>(C) * sizeof(float), st);
+  if (e != cudaSuccess) return static_cast<int>(e);
+  const long long nvox = n / C;
+  const int grid = grid_for(nvox, 256 * 8, 132 * 8);
+  if (C == 4) prelu_grad_f32_kernel<4><<<grid, 256, 0, st>>>(gy, z, alpha, gz, db, dalpha, nvox);
+  else prelu_grad_f32_kernel<8><<<grid, 256, 0, st>>>(gy, z, alpha, gz, db, dalpha, nvox);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }

@@ -83,6 +83,18 @@ def _alpha_arg(alpha, cout_pad):
     return _dev_vec(alpha, cout_pad)
 
 
+def _keeps_preact(act, alpha) -> bool:
+    """Training step: a PReLU layer keeps its pre-activation on the tape (slope gradient, derivative) instead of fusing it away."""
+    st = _store()
+    return act == "prelu" and st.tape is not None and st.keep_preact and not isinstance(alpha, str)
+
+
+def _prelu_f32(z, alpha):
+    """PReLU of an fp32 pre-activation: z * (z > 0 ? 1 : alpha) is rn_prelu_backward_f32 with g = z; the same value as the fused
+    epilogue max(z, 0) + alpha * min(z, 0) of the decoder kernels."""
+    return ops.prelu_backward_f32(z, z, _dev_vec(alpha))
+
+
 def _record(**rec):
     """Append a layer record to the store's tape (backward.py differentiates the recorded forward pass)."""
     tape = _store().tape
@@ -301,10 +313,15 @@ def fully_connected(input_, output_size, reuse=False, scope='fully_connected', i
     def run(act, alpha, residual, want32):
         xt = xin.to(device=_store().device, dtype=torch.float32).contiguous()
         wd = _dev_f32(matrix)
-        y = ops.fully_connected(xt, wd, _dev_vec(b) if b is not None else None,
-                                _alpha_arg(alpha, None) if act == "prelu" else None, want32=True)
         if act not in (None, "prelu") or residual is not None:
             raise NotImplementedError("fully_connected: only a fused PReLU epilogue is supported")
+        if _keeps_preact(act, alpha):
+            z = ops.fully_connected(xt, wd, _dev_vec(b) if b is not None else None, None, want32=True)
+            y = _prelu_f32(z, alpha)
+            _record(op="fc", x=xt, w=matrix, b=b, act=act, alpha=alpha, y=y, rerun=lambda: z)
+            return y
+        y = ops.fully_connected(xt, wd, _dev_vec(b) if b is not None else None,
+                                _alpha_arg(alpha, None) if act == "prelu" else None, want32=True)
         _record(op="fc", x=xt, w=matrix, b=b, act=act, alpha=alpha, y=y,
                 rerun=lambda: ops.fully_connected(xt, wd, _dev_vec(b) if b is not None else None, None, want32=True))
         return y
@@ -462,10 +479,16 @@ def _deferred_small3d(x, w, b, stride, transposed):
         if not xt.is_cuda:
             xt = xt.to(_store().device)
         xt = xt.contiguous()
-        y = ops.conv3d_small(xt, _dev_f32(w), _dev_vec(b) if b is not None else None,
-                             _alpha_arg(alpha, cout) if act == "prelu" else None, stride, transposed, want32=True)
         if act not in (None, "prelu") or residual is not None:
             raise NotImplementedError("thin conv3d: only a fused PReLU epilogue is supported")
+        if _keeps_preact(act, alpha):
+            z = ops.conv3d_small(xt, _dev_f32(w), _dev_vec(b) if b is not None else None, None, stride, transposed, want32=True)
+            y = _prelu_f32(z, alpha)
+            _record(op="conv_small", transposed=transposed, stride=stride, x=xt, w=w, b=b, act=act, alpha=alpha, y=y,
+                    rerun=lambda: z)
+            return y
+        y = ops.conv3d_small(xt, _dev_f32(w), _dev_vec(b) if b is not None else None,
+                             _alpha_arg(alpha, cout) if act == "prelu" else None, stride, transposed, want32=True)
         _record(op="conv_small", transposed=transposed, stride=stride, x=xt, w=w, b=b, act=act, alpha=alpha, y=y,
                 rerun=lambda: ops.conv3d_small(xt, _dev_f32(w), _dev_vec(b) if b is not None else None, None, stride,
                                                transposed, want32=True))     # the pre-activation z

@@ -992,6 +992,43 @@ def prelu_alpha_grad(g, z, scale: float = 1.0) -> torch.Tensor:
     return da
 
 
+def fully_connected_param_grad(x: torch.Tensor, gy: torch.Tensor, z: torch.Tensor, alpha: torch.Tensor, want_gz: bool = False):
+    """Parameter gradient of y = prelu(x @ w + b; alpha) (rn_fully_connected_param_grad): x fp32 [B,K], gy = dL/dy and the
+    pre-activation z fp32 [B,N], alpha fp32 [N] -> (gz = dL/dz [B,N] or None, dW [K,N], db [N], dalpha [N]), fp32, reproducible
+    bit for bit.  B <= 32, N % 4 == 0."""
+    x, gy, z, alpha = (_cuda(t, torch.float32) for t in (x, gy, z, alpha))
+    B, K = (int(v) for v in x.shape)
+    N = int(gy.shape[1])
+    if tuple(gy.shape) != (B, N) or tuple(z.shape) != (B, N) or alpha.numel() != N:
+        raise ValueError(f"fully_connected_param_grad: x {tuple(x.shape)}, gy {tuple(gy.shape)}, z {tuple(z.shape)}, "
+                         f"alpha {tuple(alpha.shape)} do not match")
+    gz = torch.empty_like(gy) if want_gz else None
+    dw = torch.empty((K, N), device=x.device, dtype=torch.float32)
+    db = torch.empty(N, device=x.device, dtype=torch.float32)
+    da = torch.empty(N, device=x.device, dtype=torch.float32)
+    check(lib.rn_fully_connected_param_grad(x.data_ptr(), gy.data_ptr(), z.data_ptr(), alpha.data_ptr(), _ptr(gz), dw.data_ptr(),
+                                            db.data_ptr(), da.data_ptr(), B, K, N, _stream()), "rn_fully_connected_param_grad")
+    return gz, dw, db, da
+
+
+def prelu_grad_f32(gy: torch.Tensor, z: torch.Tensor, alpha: torch.Tensor):
+    """(gz = gy * (z > 0 ? 1 : alpha[c]), db[c] = sum gz, dalpha[c] = sum_{z<0} gy * z) of an fp32 channel-last layer with C = 4
+    or 8 channels (rn_prelu_grad_f32); z is the pre-activation."""
+    gy, z = _cuda(gy, torch.float32), _cuda(z, torch.float32)
+    if tuple(gy.shape) != tuple(z.shape):
+        raise ValueError(f"prelu_grad_f32: gy {tuple(gy.shape)} and z {tuple(z.shape)} differ")
+    Cc = int(gy.shape[-1])
+    alpha = _cuda(alpha.to(device=gy.device, dtype=torch.float32))
+    if alpha.numel() != Cc:
+        raise ValueError(f"prelu_grad_f32: {alpha.numel()} slopes for {Cc} channels")
+    gz = torch.empty_like(gy)
+    db = torch.empty(Cc, device=gy.device, dtype=torch.float32)
+    da = torch.empty(Cc, device=gy.device, dtype=torch.float32)
+    check(lib.rn_prelu_grad_f32(gy.data_ptr(), z.data_ptr(), alpha.data_ptr(), gz.data_ptr(), db.data_ptr(), da.data_ptr(),
+                                gy.numel(), Cc, _stream()), "rn_prelu_grad_f32")
+    return gz, db, da
+
+
 def dropout(x, keep: float, seed: int, salt: int):
     """tf.nn.dropout on a 16-bit activation (rn_dropout_16): x / keep where kept, 0 elsewhere; the mask is a pure function of
     (seed, salt, element index), so calling this on the gradient with the same (seed, salt) is the backward pass."""
