@@ -54,6 +54,12 @@ long long rn_launch_count(void);
  * Corner clamp / weight rule of :410-485: points with any source coordinate outside [0,size-1) give 0. */
 int rn_resample_f32(const float* vox, const float* minv, float* out, int B, int C, int size, int new_size,
                     int transform, void* stream);
+/* A patch window of rn_resample_f32(transform=1) (random-patch training, tools/model_util.py:77-161): rows p in [y0, y0+ph),
+ * columns q in [x0, x0+pw), every depth r.  out [B,ph,pw,new_size,C] fp32 = out_full[:, y0:y0+ph, x0:x0+pw], bit for bit.
+ * C = 1 or 4; ph, pw multiples of 16, 0 <= y0 <= new_size-ph, 0 <= x0 <= new_size-pw (else -2).  The same window rule holds
+ * for every *_window entry point below. */
+int rn_resample_window_f32(const float* vox, const float* minv, float* out, int B, int C, int size, int new_size, int y0, int x0,
+                           int ph, int pw, void* stream);
 
 /* tf_interpolate (tools/resampling_voxel_grid.py:381-486) at caller-supplied coordinates: x, y, z [B*n_per_item] fp32
  * (sampler x addresses the LAST spatial axis of vox, z the first: flat = b*S^3 + z*S^2 + y*S + x, :427-449),
@@ -227,6 +233,13 @@ int rn_conv3d_direct(const void* x, int x_is_f32, const float* w, const float* b
  * new_size % 16 == 0. */
 int rn_resample_conv1_fused(const float* vox, const float* minv, const float* w, const float* bias,
                             const float* alpha, void* out16, int B, int size, int new_size, int fmt, void* stream);
+/* rn_resample_conv1_fused on the window (y0, x0, ph, pw) of the transformed grid (rn_resample_window_f32's rule): e_conv1's SAME
+ * padding applies at the window's borders (points outside the window are zero, as when the grid is sliced before the conv).
+ * out16 [B,ph/2,pw/2,new_size/2,8]; bit-identical to rn_resample_window_f32 (C = 1) -> rn_conv3d_direct on [B,ph,pw,new,1].
+ * The full window (0, 0, new_size, new_size) is rn_resample_conv1_fused. */
+int rn_resample_conv1_fused_window(const float* vox, const float* minv, const float* w, const float* bias, const float* alpha,
+                                   void* out16, int B, int size, int new_size, int y0, int x0, int ph, int pw, int fmt,
+                                   void* stream);
 
 /* The same fusion for the Texture/Normal network's input (BASELINE config 4; RenderNet_Texture_Face_Normal.py:155-179):
  * tf_rotation_resampling of the geometry grid (vox fp32 [B,size^3], C = 1) AND of the decoded texture volume (tex fp32
@@ -235,6 +248,11 @@ int rn_resample_conv1_fused(const float* vox, const float* minv, const float* w,
  * rn_conv3d_direct. */
 int rn_resample5_conv1_fused(const float* vox, const float* tex, const float* minv, const float* w, const float* bias,
                              const float* alpha, void* out16, int B, int size, int new_size, int fmt, void* stream);
+/* rn_resample5_conv1_fused on a window (y0, x0, ph, pw), as rn_resample_conv1_fused_window: out16 [B,ph/2,pw/2,new_size/2,8],
+ * bit-identical to rn_resample_window_f32 (C = 1 and C = 4) -> rn_concat_channels_f32 -> rn_conv3d_direct. */
+int rn_resample5_conv1_fused_window(const float* vox, const float* tex, const float* minv, const float* w, const float* bias,
+                                    const float* alpha, void* out16, int B, int size, int new_size, int y0, int x0, int ph, int pw,
+                                    int fmt, void* stream);
 
 /* ---- binvox run-length decode on the device (tools/binvox_rw.py:84-93; SURVEY 8 f-2) ----------------------
  * pairs: the raw (value, count) byte pairs of n_items files back to back; run_start[r] = number of voxels before run r
@@ -294,6 +312,11 @@ int rn_resample_backward_f32(const float* vox, const float* minv, const float* g
  * decisions are the forward kernel's. */
 int rn_resample5_backward_f32(const float* vox, const float* tex, const float* minv, const float* gout, float* dvox, float* dtex,
                               float* dminv, int B, int size, int new_size, void* stream);
+/* rn_resample5_backward_f32 for a window (y0, x0, ph, pw; rn_resample_window_f32's rule): gout = dL/d(cropped concat)
+ * [B,ph,pw,new_size,5]; only the window's points scatter.  dvox, dtex, dminv as above (accumulated, each may be NULL). */
+int rn_resample5_backward_window_f32(const float* vox, const float* tex, const float* minv, const float* gout, float* dvox,
+                                     float* dtex, float* dminv, int B, int size, int new_size, int y0, int x0, int ph, int pw,
+                                     void* stream);
 /* fp32 PReLU derivative (texture decoder, tools/layer_util.py:27-45): out[i] = g[i] * (z[i] > 0 ? 1 : alpha[i % C]) with z the
  * PRE-activation (slopes may be negative). */
 int rn_prelu_backward_f32(const float* g, const float* z, const float* alpha, float* out, long long n, int C, void* stream);

@@ -53,6 +53,7 @@ SIGNATURES = {
     "rn_error_string": (C.c_char_p, [_i]),
     "rn_launch_count": (_ll, []),
     "rn_resample_f32": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "rn_resample_window_f32": (_i, [_vp, _vp, _vp] + [_i] * 8 + [_vp]),
     "rn_interpolate_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _ll, _vp]),
     "rn_pack_conv_weights": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     "rn_cast_f32_to_16": (_i, [_vp, _vp, _ll, _ll, _i, _vp]),
@@ -76,6 +77,8 @@ SIGNATURES = {
     "rn_conv3d_direct": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "rn_resample_conv1_fused": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "rn_resample5_conv1_fused": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "rn_resample_conv1_fused_window": (_i, [_vp] * 6 + [_i] * 8 + [_vp]),
+    "rn_resample5_conv1_fused_window": (_i, [_vp] * 7 + [_i] * 8 + [_vp]),
     "rn_binvox_decode": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "rn_fully_connected": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "rn_conv3d_small": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
@@ -85,6 +88,7 @@ SIGNATURES = {
     "rn_conv3d_backward_data_direct": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp]),
     "rn_resample_backward_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "rn_resample5_backward_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "rn_resample5_backward_window_f32": (_i, [_vp] * 7 + [_i] * 7 + [_vp]),
     "rn_prelu_backward_f32": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _vp]),
     "rn_fully_connected_backward_workspace": (_ll, [_i, _i, _i]),
     "rn_fully_connected_backward_data": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),

@@ -51,7 +51,7 @@ from . import ops
 from . import tfcompat as tf
 from .RenderNet_Shader import RenderNet
 from .engine import pose_to_matrix
-from .resampling_voxel_grid import ConcatResampledGrid, ResampledGrid
+from .resampling_voxel_grid import ConcatResampledGrid, CroppedGrid, ResampledGrid
 
 
 def _key(t) -> int:
@@ -427,15 +427,17 @@ class _InputGradients:
         if rec["op"] in ("resample_conv1", "resample5_conv1"):
             # e_conv1 read the resampled grid straight out of the fused kernel: materialise it once for the correlation (the
             # standalone resampler is bit-identical to the fused one); Texture+Normal: geometry and decoded texture, concatenated
+            # (a patch record: the same grid's window alone, SAME-padded at the patch's borders)
             grid = rec["grid"]
+            win = {} if rec.get("window") is None else dict(window=rec["window"])
             if rec["op"] == "resample_conv1":
-                q = ops.resample(grid.voxel, grid.minv, self.new_size, True)
+                q = ops.resample(grid.voxel, grid.minv, self.new_size, True, **win)
             else:
-                q = ops.concat_channels(ops.resample(grid.geom.voxel, grid.minv, self.new_size, True),
-                                        ops.resample(grid.tex.voxel, grid.minv, self.new_size, True))
+                q = ops.concat_channels(ops.resample(grid.geom.voxel, grid.minv, self.new_size, True, **win),
+                                        ops.resample(grid.tex.voxel, grid.minv, self.new_size, True, **win))
             st = tuple(int(v) for v in rec["stride"])
             ks = tuple(int(v) for v in w.shape[:3])
-            pad = tuple(ops.same_pad_before(self.new_size, ks[i], st[i]) for i in range(3))
+            pad = tuple(ops.same_pad_before(int(q.shape[1 + i]), ks[i], st[i]) for i in range(3))
             d = ops.conv_weight_grad_direct(g, q, ks, st, pad, Ca=cout, Cb=int(w.shape[3]), scale=inv)      # [k,k,k,co,ci]
             wg[w._rn_name] = d.permute(0, 1, 2, 4, 3).contiguous()
             return
@@ -556,6 +558,8 @@ class ShaderInputGradients(_InputGradients):
         if rec["op"] != "resample_conv1":
             raise RuntimeError(f"a Shader tape cannot hold a {rec['op']} record")
         if self._need_inputs:
+            if rec.get("window") is not None:
+                raise NotImplementedError("input gradients (dL/dvoxels, dL/dpose) of a patch forward: render whole frames")
             N = self.new_size
             w32 = rec["w"].to(self.store.device).float().contiguous()
             self._dgrid = ops.conv3d_backward_data_direct(g, w32, (self.B, N, N, N, 1), rec["stride"], want32=True,
@@ -609,8 +613,9 @@ class TextureInputGradients(_InputGradients):
         self.tex_in = torch.as_tensor(np.asarray(texture, np.float32)).reshape(self.B, -1).to(dev).contiguous()
         self.minv = torch.from_numpy(pose_to_matrix(self.view_params, self.size, self.new_size)).to(dev)
 
-    def _record_network(self, is_training: bool, prob: float):
-        """Decoder -> two deferred resamplings -> RenderNet under the current store and tape (is_training / prob: dropout)."""
+    def _record_network(self, is_training: bool, prob: float, window=None):
+        """Decoder -> two deferred resamplings -> RenderNet under the current store and tape (is_training / prob: dropout).
+        window = (y0, x0, ph, pw): the network runs on that patch of the concatenated grid (CroppedGrid)."""
         from .RenderNet_Texture_Face_Normal import RenderNet as RenderNetTexture, decoder_texture
         from .Reconstruct_RenderNet_Face import RenderNet_pretrained, texture_decoder_pretrained
         if self.model == "texture":
@@ -621,6 +626,8 @@ class TextureInputGradients(_InputGradients):
         # record holds the very tensors (geometry, decoded texture) the backward scatters into
         grid = ConcatResampledGrid(ResampledGrid(self.vox, self.minv, self.new_size, transform=True),
                                    ResampledGrid(self.tex3d, self.minv, self.new_size, transform=True))
+        if window is not None:
+            grid = CroppedGrid(grid, *window)
         if self.model == "texture":
             self.albedo, self.normal = RenderNetTexture(grid, prob=prob, is_training=is_training)
         else:
@@ -688,13 +695,14 @@ class TextureInputGradients(_InputGradients):
         if rec["op"] != "resample5_conv1":
             raise RuntimeError(f"a Texture tape cannot hold a {rec['op']} record")
         want_dvox, want_dtex, want_dpose = self._want
-        grid = rec["grid"]
+        grid, win = rec["grid"], rec.get("window")
         N = self.new_size
-        dgrid = ops.conv3d_backward_data_direct(g, self._w32(rec["w"]), (self.B, N, N, N, 5), rec["stride"], want32=True,
+        ph, pw = (N, N) if win is None else win[2:]      # a patch record: dL/d(the concat's window), scattered from it alone
+        dgrid = ops.conv3d_backward_data_direct(g, self._w32(rec["w"]), (self.B, ph, pw, N, 5), rec["stride"], want32=True,
                                                 out_scale=1.0 / self.last_loss_scale)
         self.last_dgrid = dgrid
         self._dvox, dtex, self._dminv = ops.resample5_backward(grid.geom.voxel, grid.tex.voxel, grid.minv, dgrid, want_dvox,
-                                                               want_dtex, want_dpose)
+                                                               want_dtex, want_dpose, window=win)
         if dtex is not None:
             grads[_key(grid.tex.voxel)] = dtex
             self._dtex_reached = True

@@ -248,22 +248,25 @@ __global__ void __launch_bounds__(256) resample_backward_kernel(const float* __r
 // points and concatenated, G = dL/d(concat) [B,N,N,N,5].  Each sample coordinate is computed once, with the forward kernel's
 // sample_coord arithmetic and in/out test; channel 0 scatters into dvox, channels 1..4 into dtex (float4 corner gathers), and
 // dM^-1 collects all five channels.  Per corner the five channels are first contracted to s_k = G0 V_k + G1..4 . T_k, so
-// d/dx = sum_k (dw_k/dx) s_k.  Same warp-per-row layout and block reduction as resample_backward_kernel.
+// d/dx = sum_k (dw_k/dx) s_k.  Same warp-per-row layout and block reduction as resample_backward_kernel.  G covers the window
+// of rows [wy0, wy0+wh) x columns [wx0, wx0+ww) (all depths; the whole grid: 0, 0, nsz, nsz), [B,wh,ww,nsz,5]: only the
+// points of that window scatter.
 __global__ void __launch_bounds__(256) resample5_backward_kernel(const float* __restrict__ vox, const float* __restrict__ tex,
                                                                  const float* __restrict__ minv, const float* __restrict__ gout,
                                                                  float* __restrict__ dvox, float* __restrict__ dtex,
-                                                                 float* __restrict__ dminv, int B, int size, int nsz) {
+                                                                 float* __restrict__ dminv, int B, int size, int nsz, int wy0,
+                                                                 int wx0, int wh, int ww) {
   __shared__ float red[8][12];
   const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int rows = B * nsz * nsz;
+  const int rows = B * wh * ww;
   float dm[12];
 #pragma unroll
   for (int i = 0; i < 12; ++i) dm[i] = 0.f;
   if (warp_global < rows) {
-    const int b = warp_global / (nsz * nsz);
-    const int o1 = (warp_global / nsz) % nsz;
-    const int o2 = warp_global % nsz;
+    const int b = warp_global / (wh * ww);
+    const int o1 = wy0 + (warp_global / ww) % wh;
+    const int o2 = wx0 + warp_global % ww;
     const float* M = minv + b * 12;
     const float m00 = __ldg(M + 0), m01 = __ldg(M + 1), m02 = __ldg(M + 2), m03 = __ldg(M + 3);
     const float m10 = __ldg(M + 4), m11 = __ldg(M + 5), m12 = __ldg(M + 6), m13 = __ldg(M + 7);
@@ -329,7 +332,7 @@ __global__ void __launch_bounds__(256) resample5_backward_kernel(const float* __
     float v = 0.f;
     for (int wv = 0; wv < 8; ++wv) v += red[wv][threadIdx.x];
     const int first_row = (blockIdx.x * blockDim.x) >> 5;
-    if (first_row < rows && v != 0.f) atomicAdd(dminv + (first_row / (nsz * nsz)) * 12 + threadIdx.x, v);
+    if (first_row < rows && v != 0.f) atomicAdd(dminv + (first_row / (wh * ww)) * 12 + threadIdx.x, v);
   }
 }
 
@@ -573,16 +576,32 @@ extern "C" int rn_resample_backward_f32(const float* vox, const float* minv, con
   return static_cast<int>(cudaGetLastError());
 }
 
+static int resample5_backward_launch(const float* vox, const float* tex, const float* minv, const float* gout, float* dvox,
+                                     float* dtex, float* dminv, int B, int size, int new_size, int y0, int x0, int ph, int pw,
+                                     void* stream) {
+  if ((reinterpret_cast<uintptr_t>(tex) & 15) != 0 || (reinterpret_cast<uintptr_t>(dtex) & 15) != 0) return -3;
+  const long long rows = static_cast<long long>(B) * ph * pw;
+  resample5_backward_kernel<<<static_cast<int>((rows * 32 + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      vox, tex, minv, gout, dvox, dtex, dminv, B, size, new_size, y0, x0, ph, pw);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
 extern "C" int rn_resample5_backward_f32(const float* vox, const float* tex, const float* minv, const float* gout, float* dvox,
                                          float* dtex, float* dminv, int B, int size, int new_size, void* stream) {
   if (!vox || !tex || !minv || !gout || (!dvox && !dtex && !dminv) || B < 1 || size < 2 || new_size < 1) return -1;
   if ((new_size * new_size) % 8 != 0) return -2;      // a block's 8 rows must belong to one batch item
-  if ((reinterpret_cast<uintptr_t>(tex) & 15) != 0 || (reinterpret_cast<uintptr_t>(dtex) & 15) != 0) return -3;
-  const long long rows = static_cast<long long>(B) * new_size * new_size;
-  resample5_backward_kernel<<<static_cast<int>((rows * 32 + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      vox, tex, minv, gout, dvox, dtex, dminv, B, size, new_size);
-  RN_COUNT_LAUNCH();
-  return static_cast<int>(cudaGetLastError());
+  return resample5_backward_launch(vox, tex, minv, gout, dvox, dtex, dminv, B, size, new_size, 0, 0, new_size, new_size, stream);
+}
+
+extern "C" int rn_resample5_backward_window_f32(const float* vox, const float* tex, const float* minv, const float* gout,
+                                                float* dvox, float* dtex, float* dminv, int B, int size, int new_size, int y0,
+                                                int x0, int ph, int pw, void* stream) {
+  if (!vox || !tex || !minv || !gout || (!dvox && !dtex && !dminv) || B < 1 || size < 2 || new_size < 16) return -1;
+  // same window rule as rn_ops.cu's window_ok; ph * pw % 8 == 0 keeps a block's 8 rows in one batch item
+  if (ph < 16 || pw < 16 || ph % 16 != 0 || pw % 16 != 0 || y0 < 0 || x0 < 0 || y0 > new_size - ph || x0 > new_size - pw)
+    return -2;
+  return resample5_backward_launch(vox, tex, minv, gout, dvox, dtex, dminv, B, size, new_size, y0, x0, ph, pw, stream);
 }
 
 extern "C" int rn_prelu_backward_f32(const float* g, const float* z, const float* alpha, float* out, long long n, int C,

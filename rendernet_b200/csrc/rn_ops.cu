@@ -71,18 +71,20 @@ __device__ __forceinline__ float sample_coord(float m0, float m1, float m2, floa
 }
 
 // One warp per output row (innermost output axis); each lane owns 4 consecutive points per iteration so
-// C=1 rows are written with one 16-byte store per lane (512 B per warp instruction).
+// C=1 rows are written with one 16-byte store per lane (512 B per warp instruction).  The rows are those of the window
+// o1 in [wy0, wy0+wh), o2 in [wx0, wx0+ww) of the nsz^2 output rows per item (the whole grid: 0, 0, nsz, nsz), written
+// densely: out is [B,wh,ww,nsz,C].
 template <int C>
 __global__ void __launch_bounds__(256) resample_kernel(const float* __restrict__ vox, const float* __restrict__ minv,
                                                        float* __restrict__ out, int B, int size, int nsz,
-                                                       int transform) {
+                                                       int transform, int wy0, int wx0, int wh, int ww) {
   const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  const int rows = B * nsz * nsz;
+  const int rows = B * wh * ww;
   if (warp_global >= rows) return;
-  const int b = warp_global / (nsz * nsz);
-  const int o1 = (warp_global / nsz) % nsz;
-  const int o2 = warp_global % nsz;
+  const int b = warp_global / (wh * ww);
+  const int o1 = wy0 + (warp_global / ww) % wh;
+  const int o2 = wx0 + warp_global % ww;
   const float* M = minv + b * 12;
   const float m00 = __ldg(M + 0), m01 = __ldg(M + 1), m02 = __ldg(M + 2), m03 = __ldg(M + 3);
   const float m10 = __ldg(M + 4), m11 = __ldg(M + 5), m12 = __ldg(M + 6), m13 = __ldg(M + 7);
@@ -398,7 +400,9 @@ __global__ void __launch_bounds__(256) conv3d_direct_kernel(const void* __restri
 // points it needs into shared memory (same arithmetic, operation for operation, as resample_kernel), and if every one
 // of them is exactly 0 -- outside the rotated cube or empty space, ~85-90 % of all tiles -- the outputs are
 // PReLU(bias) and the 5^3 convolution is skipped.  Accumulation order per output = conv3d_direct_kernel's
-// (ky, kx, kz), so results are bit-identical to the unfused pair.
+// (ky, kx, kz), so results are bit-identical to the unfused pair.  The CTAs cover a window of rows [wy0, wy0+wh) x columns
+// [wx0, wx0+ww) of the transformed grid (all depths; the whole grid: 0, 0, nsz, nsz): points outside it are SAME padding,
+// as when the grid is sliced before the convolution (training on patches, RenderNet_Shader.py:150-156).
 constexpr int RC_T = 8;                 // outputs per tile edge
 constexpr int RC_IN = 2 * RC_T + 3;     // 19 input points per edge
 constexpr int RC_ZP = 20;               // padded z row: even z at [0,10), odd z at [10,19) -> conflict-free stride-2 reads
@@ -407,17 +411,18 @@ __global__ void __launch_bounds__(256) resample_conv1_kernel(const float* __rest
                                                              const float* __restrict__ minv,
                                                              const float* __restrict__ w, const float* __restrict__ bias,
                                                              const float* __restrict__ alpha, uint16_t* __restrict__ out,
-                                                             int B, int size, int nsz, int fmt) {
+                                                             int B, int size, int nsz, int fmt, int wy0, int wx0, int wh,
+                                                             int ww) {
   __shared__ float tile[RC_IN * RC_IN * RC_ZP];
   __shared__ __align__(16) float ws[125 * 8];
   const int tid = threadIdx.x;
-  const int No = nsz >> 1;                // output edge
-  const int tpe = No / RC_T;              // tiles per edge
+  const int Ho = wh >> 1, Wo = ww >> 1, Do = nsz >> 1;      // output extents of the window
+  const int tpy = Ho / RC_T, tpx = Wo / RC_T, tpz = Do / RC_T;
   int bid = blockIdx.x;
-  const int tz = bid % tpe; bid /= tpe;
-  const int tx = bid % tpe; bid /= tpe;
-  const int ty = bid % tpe;
-  const int b = bid / tpe;
+  const int tz = bid % tpz; bid /= tpz;
+  const int tx = bid % tpx; bid /= tpx;
+  const int ty = bid % tpy;
+  const int b = bid / tpy;
   for (int i = tid; i < 125 * 8; i += 256) ws[i] = __ldg(w + i);
 
   const float* M = minv + b * 12;
@@ -427,7 +432,7 @@ __global__ void __launch_bounds__(256) resample_conv1_kernel(const float* __rest
   const float lim = static_cast<float>(size - 1);
   const float* vb = vox + static_cast<size_t>(b) * size * size * size;
   const size_t sy = static_cast<size_t>(size), sz = static_cast<size_t>(size) * size;
-  const int p0 = 2 * ty * RC_T - 1, q0 = 2 * tx * RC_T - 1, r0 = 2 * tz * RC_T - 1;
+  const int p0 = wy0 + 2 * ty * RC_T - 1, q0 = wx0 + 2 * tx * RC_T - 1, r0 = 2 * tz * RC_T - 1;
 
   // Tile-level rejection: the source coordinate is affine in (p,q,r), so over the tile's input box each of x,y,z is
   // bounded by its values at the box's 8 corners.  If one axis lies entirely outside [0, size-1) (with a margin far
@@ -436,8 +441,8 @@ __global__ void __launch_bounds__(256) resample_conv1_kernel(const float* __rest
   int nonzero = 0;
   bool maybe_inside = true;
   {
-    const float pl = static_cast<float>(max(p0, 0)), ph = static_cast<float>(min(p0 + RC_IN - 1, nsz - 1));
-    const float ql = static_cast<float>(max(q0, 0)), qh = static_cast<float>(min(q0 + RC_IN - 1, nsz - 1));
+    const float pl = static_cast<float>(max(p0, wy0)), ph = static_cast<float>(min(p0 + RC_IN - 1, wy0 + wh - 1));
+    const float ql = static_cast<float>(max(q0, wx0)), qh = static_cast<float>(min(q0 + RC_IN - 1, wx0 + ww - 1));
     const float rl = static_cast<float>(max(r0, 0)), rh = static_cast<float>(min(r0 + RC_IN - 1, nsz - 1));
     const float gyl = static_cast<float>(nsz - 1) - ph, gyh = static_cast<float>(nsz - 1) - pl;   // gy = nsz-1-p
     const float mrow[3][4] = {{m00, m01, m02, m03}, {m10, m11, m12, m13}, {m20, m21, m22, m23}};
@@ -458,7 +463,7 @@ __global__ void __launch_bounds__(256) resample_conv1_kernel(const float* __rest
       const int iy = row / RC_IN, ix = row - iy * RC_IN;
       const int p = p0 + iy, q = q0 + ix, r = r0 + iz;
       float v = 0.f;
-      if (p >= 0 && p < nsz && q >= 0 && q < nsz && r >= 0 && r < nsz) {
+      if (p >= wy0 && p < wy0 + wh && q >= wx0 && q < wx0 + ww && r >= 0 && r < nsz) {   // SAME zeros at the window border
         // N[b,p,q,r] = T[b,q,nsz-1-p,r]; grid point (gx,gy,gz) = (r, nsz-1-p, q)
         const float gx = static_cast<float>(r), gy = static_cast<float>(nsz - 1 - p), gz = static_cast<float>(q);
         const float x = sample_coord(m00, m01, m02, m03, gx, gy, gz);
@@ -538,12 +543,12 @@ __global__ void __launch_bounds__(256) resample_conv1_kernel(const float* __rest
     pack16x2(u0, u1, fmt, &pk0[c / 2], &pl0[c / 2]);
     pack16x2(v0, v1, fmt, &pk1[c / 2], &pl1[c / 2]);
   }
-  const size_t o0 = (((static_cast<size_t>(b) * No + (ty * RC_T + oy)) * No + (tx * RC_T + ox)) * No + (tz * RC_T + oz)) * 8;
-  const size_t o1 = o0 + static_cast<size_t>(4) * No * No * 8;
+  const size_t o0 = (((static_cast<size_t>(b) * Ho + (ty * RC_T + oy)) * Wo + (tx * RC_T + ox)) * Do + (tz * RC_T + oz)) * 8;
+  const size_t o1 = o0 + static_cast<size_t>(4) * Wo * Do * 8;
   *reinterpret_cast<uint4*>(out + o0) = make_uint4(pk0[0], pk0[1], pk0[2], pk0[3]);
   *reinterpret_cast<uint4*>(out + o1) = make_uint4(pk1[0], pk1[1], pk1[2], pk1[3]);
   if (fmt == 2) {    // LO plane of the fp16 hi/lo pair
-    const size_t plane = static_cast<size_t>(B) * No * No * No * 8;
+    const size_t plane = static_cast<size_t>(B) * Ho * Wo * Do * 8;
     *reinterpret_cast<uint4*>(out + plane + o0) = make_uint4(pl0[0], pl0[1], pl0[2], pl0[3]);
     *reinterpret_cast<uint4*>(out + plane + o1) = make_uint4(pl1[0], pl1[1], pl1[2], pl1[3]);
   }
@@ -564,18 +569,19 @@ constexpr int RC5_TILE = RC_IN * RC_IN * RC_ZP;          // floats per channel p
 __global__ void __launch_bounds__(256) resample5_conv1_kernel(const float* __restrict__ vox, const float* __restrict__ tex,
                                                               const float* __restrict__ minv, const float* __restrict__ w,
                                                               const float* __restrict__ bias, const float* __restrict__ alpha,
-                                                              uint16_t* __restrict__ out, int B, int size, int nsz, int fmt) {
+                                                              uint16_t* __restrict__ out, int B, int size, int nsz, int fmt,
+                                                              int wy0, int wx0, int wh, int ww) {
   extern __shared__ __align__(16) float smem5[];
   float* tile = smem5;                                   // [5][19*19*20]
   float* ws = smem5 + RC5_C * RC5_TILE;                  // [125][5][8]
   const int tid = threadIdx.x;
-  const int No = nsz >> 1;
-  const int tpe = No / RC_T;
+  const int Ho = wh >> 1, Wo = ww >> 1, Do = nsz >> 1;
+  const int tpy = Ho / RC_T, tpx = Wo / RC_T, tpz = Do / RC_T;
   int bid = blockIdx.x;
-  const int tz = bid % tpe; bid /= tpe;
-  const int tx = bid % tpe; bid /= tpe;
-  const int ty = bid % tpe;
-  const int b = bid / tpe;
+  const int tz = bid % tpz; bid /= tpz;
+  const int tx = bid % tpx; bid /= tpx;
+  const int ty = bid % tpy;
+  const int b = bid / tpy;
   for (int i = tid; i < 125 * RC5_C * 8; i += 256) ws[i] = __ldg(w + i);
 
   const float* M = minv + b * 12;
@@ -587,13 +593,13 @@ __global__ void __launch_bounds__(256) resample5_conv1_kernel(const float* __res
   const float* vb = vox + static_cast<size_t>(b) * vol;
   const float* tb = tex + static_cast<size_t>(b) * vol * 4;
   const size_t sy = static_cast<size_t>(size), sz = static_cast<size_t>(size) * size;
-  const int p0 = 2 * ty * RC_T - 1, q0 = 2 * tx * RC_T - 1, r0 = 2 * tz * RC_T - 1;
+  const int p0 = wy0 + 2 * ty * RC_T - 1, q0 = wx0 + 2 * tx * RC_T - 1, r0 = 2 * tz * RC_T - 1;
 
   int nonzero = 0;
   bool maybe_inside = true;
   {
-    const float pl = static_cast<float>(max(p0, 0)), ph = static_cast<float>(min(p0 + RC_IN - 1, nsz - 1));
-    const float ql = static_cast<float>(max(q0, 0)), qh = static_cast<float>(min(q0 + RC_IN - 1, nsz - 1));
+    const float pl = static_cast<float>(max(p0, wy0)), ph = static_cast<float>(min(p0 + RC_IN - 1, wy0 + wh - 1));
+    const float ql = static_cast<float>(max(q0, wx0)), qh = static_cast<float>(min(q0 + RC_IN - 1, wx0 + ww - 1));
     const float rl = static_cast<float>(max(r0, 0)), rh = static_cast<float>(min(r0 + RC_IN - 1, nsz - 1));
     const float gyl = static_cast<float>(nsz - 1) - ph, gyh = static_cast<float>(nsz - 1) - pl;
     const float mrow[3][4] = {{m00, m01, m02, m03}, {m10, m11, m12, m13}, {m20, m21, m22, m23}};
@@ -612,7 +618,7 @@ __global__ void __launch_bounds__(256) resample5_conv1_kernel(const float* __res
       const int iy = row / RC_IN, ix = row - iy * RC_IN;
       const int p = p0 + iy, q = q0 + ix, r = r0 + iz;
       float v[RC5_C] = {0.f, 0.f, 0.f, 0.f, 0.f};
-      if (p >= 0 && p < nsz && q >= 0 && q < nsz && r >= 0 && r < nsz) {
+      if (p >= wy0 && p < wy0 + wh && q >= wx0 && q < wx0 + ww && r >= 0 && r < nsz) {   // SAME zeros at the window border
         const float gx = static_cast<float>(r), gy = static_cast<float>(nsz - 1 - p), gz = static_cast<float>(q);
         const float x = sample_coord(m00, m01, m02, m03, gx, gy, gz);
         const float y = sample_coord(m10, m11, m12, m13, gx, gy, gz);
@@ -705,12 +711,12 @@ __global__ void __launch_bounds__(256) resample5_conv1_kernel(const float* __res
     pack16x2(u0, u1, fmt, &pk0[c / 2], &pl0[c / 2]);
     pack16x2(v0, v1, fmt, &pk1[c / 2], &pl1[c / 2]);
   }
-  const size_t o0 = (((static_cast<size_t>(b) * No + (ty * RC_T + oy)) * No + (tx * RC_T + ox)) * No + (tz * RC_T + oz)) * 8;
-  const size_t o1 = o0 + static_cast<size_t>(4) * No * No * 8;
+  const size_t o0 = (((static_cast<size_t>(b) * Ho + (ty * RC_T + oy)) * Wo + (tx * RC_T + ox)) * Do + (tz * RC_T + oz)) * 8;
+  const size_t o1 = o0 + static_cast<size_t>(4) * Wo * Do * 8;
   *reinterpret_cast<uint4*>(out + o0) = make_uint4(pk0[0], pk0[1], pk0[2], pk0[3]);
   *reinterpret_cast<uint4*>(out + o1) = make_uint4(pk1[0], pk1[1], pk1[2], pk1[3]);
   if (fmt == 2) {
-    const size_t plane = static_cast<size_t>(B) * No * No * No * 8;
+    const size_t plane = static_cast<size_t>(B) * Ho * Wo * Do * 8;
     *reinterpret_cast<uint4*>(out + plane + o0) = make_uint4(pl0[0], pl0[1], pl0[2], pl0[3]);
     *reinterpret_cast<uint4*>(out + plane + o1) = make_uint4(pl1[0], pl1[1], pl1[2], pl1[3]);
   }
@@ -1018,22 +1024,42 @@ extern "C" const char* rn_error_string(int code) {
   return cudaGetErrorString(static_cast<cudaError_t>(code));
 }
 
-extern "C" int rn_resample_f32(const float* vox, const float* minv, float* out, int B, int C, int size, int new_size,
-                               int transform, void* stream) {
-  if (!vox || !minv || !out || B < 1 || size < 2 || new_size < 1) return -1;
+// the rows [y0, y0+ph) x columns [x0, x0+pw) of the new_size^2 rows per item
+static int resample_launch(const float* vox, const float* minv, float* out, int B, int C, int size, int new_size, int transform,
+                           int y0, int x0, int ph, int pw, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const long long rows = static_cast<long long>(B) * new_size * new_size;
+  const long long rows = static_cast<long long>(B) * ph * pw;
   const int block = 256;
   const int grid = static_cast<int>((rows * 32 + block - 1) / block);
   switch (C) {
-    case 1: resample_kernel<1><<<grid, block, 0, st>>>(vox, minv, out, B, size, new_size, transform); break;
-    case 2: resample_kernel<2><<<grid, block, 0, st>>>(vox, minv, out, B, size, new_size, transform); break;
-    case 3: resample_kernel<3><<<grid, block, 0, st>>>(vox, minv, out, B, size, new_size, transform); break;
-    case 4: resample_kernel<4><<<grid, block, 0, st>>>(vox, minv, out, B, size, new_size, transform); break;
+    case 1: resample_kernel<1><<<grid, block, 0, st>>>(vox, minv, out, B, size, new_size, transform, y0, x0, ph, pw); break;
+    case 2: resample_kernel<2><<<grid, block, 0, st>>>(vox, minv, out, B, size, new_size, transform, y0, x0, ph, pw); break;
+    case 3: resample_kernel<3><<<grid, block, 0, st>>>(vox, minv, out, B, size, new_size, transform, y0, x0, ph, pw); break;
+    case 4: resample_kernel<4><<<grid, block, 0, st>>>(vox, minv, out, B, size, new_size, transform, y0, x0, ph, pw); break;
     default: return -2;
   }
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
+}
+
+// A patch window of the axis-transformed grid: ph, pw multiples of 16 (8^3-output tiles of the stride-2 e_conv1) inside
+// [0, new_size).  Shared by every *_window entry point.
+static bool window_ok(int new_size, int y0, int x0, int ph, int pw) {
+  return ph >= 16 && pw >= 16 && ph % 16 == 0 && pw % 16 == 0 && y0 >= 0 && x0 >= 0 && y0 <= new_size - ph &&
+         x0 <= new_size - pw;
+}
+
+extern "C" int rn_resample_f32(const float* vox, const float* minv, float* out, int B, int C, int size, int new_size,
+                               int transform, void* stream) {
+  if (!vox || !minv || !out || B < 1 || size < 2 || new_size < 1) return -1;
+  return resample_launch(vox, minv, out, B, C, size, new_size, transform, 0, 0, new_size, new_size, stream);
+}
+
+extern "C" int rn_resample_window_f32(const float* vox, const float* minv, float* out, int B, int C, int size, int new_size,
+                                      int y0, int x0, int ph, int pw, void* stream) {
+  if (!vox || !minv || !out || B < 1 || size < 2 || new_size < 16) return -1;
+  if ((C != 1 && C != 4) || !window_ok(new_size, y0, x0, ph, pw)) return -2;
+  return resample_launch(vox, minv, out, B, C, size, new_size, 1, y0, x0, ph, pw, stream);
 }
 
 // plane: element offset of the LO plane for fmt 2 (0 = right after this call's own output)
@@ -1519,28 +1545,33 @@ extern "C" int rn_conv3d_direct(const void* x, int x_is_f32, const float* w, con
   return static_cast<int>(cudaGetLastError());
 }
 
-extern "C" int rn_resample_conv1_fused(const float* vox, const float* minv, const float* w, const float* bias,
-                                       const float* alpha, void* out16, int B, int size, int new_size, int fmt,
-                                       void* stream) {
+extern "C" int rn_resample_conv1_fused_window(const float* vox, const float* minv, const float* w, const float* bias,
+                                              const float* alpha, void* out16, int B, int size, int new_size, int y0, int x0,
+                                              int ph, int pw, int fmt, void* stream) {
   if (!vox || !minv || !w || !bias || !out16 || B < 1 || size < 2) return -1;
-  if (new_size < 16 || new_size % 16 != 0) return -2;   // 8^3-output tiles
-  const int tpe = new_size / 2 / RC_T;
-  const long long blocks = static_cast<long long>(B) * tpe * tpe * tpe;
+  if (new_size < 16 || new_size % 16 != 0 || !window_ok(new_size, y0, x0, ph, pw)) return -2;   // 8^3-output tiles
+  const long long blocks = static_cast<long long>(B) * (ph / 16) * (pw / 16) * (new_size / 16);
   if (blocks > 0x7fffffffLL) return -3;
   resample_conv1_kernel<<<static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      vox, minv, w, bias, alpha, static_cast<uint16_t*>(out16), B, size, new_size, fmt);
+      vox, minv, w, bias, alpha, static_cast<uint16_t*>(out16), B, size, new_size, fmt, y0, x0, ph, pw);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }
 
-extern "C" int rn_resample5_conv1_fused(const float* vox, const float* tex, const float* minv, const float* w,
-                                        const float* bias, const float* alpha, void* out16, int B, int size, int new_size,
-                                        int fmt, void* stream) {
+extern "C" int rn_resample_conv1_fused(const float* vox, const float* minv, const float* w, const float* bias,
+                                       const float* alpha, void* out16, int B, int size, int new_size, int fmt,
+                                       void* stream) {
+  return rn_resample_conv1_fused_window(vox, minv, w, bias, alpha, out16, B, size, new_size, 0, 0, new_size, new_size, fmt,
+                                        stream);
+}
+
+extern "C" int rn_resample5_conv1_fused_window(const float* vox, const float* tex, const float* minv, const float* w,
+                                               const float* bias, const float* alpha, void* out16, int B, int size,
+                                               int new_size, int y0, int x0, int ph, int pw, int fmt, void* stream) {
   if (!vox || !tex || !minv || !w || !bias || !out16 || B < 1 || size < 2 || fmt < 0 || fmt > 2) return -1;
-  if (new_size < 16 || new_size % 16 != 0) return -2;
+  if (new_size < 16 || new_size % 16 != 0 || !window_ok(new_size, y0, x0, ph, pw)) return -2;
   if ((reinterpret_cast<uintptr_t>(tex) & 15) != 0) return -4;      // float4 gathers of the 4-channel texture volume
-  const int tpe = new_size / 2 / RC_T;
-  const long long blocks = static_cast<long long>(B) * tpe * tpe * tpe;
+  const long long blocks = static_cast<long long>(B) * (ph / 16) * (pw / 16) * (new_size / 16);
   if (blocks > 0x7fffffffLL) return -3;
   const size_t smem = (static_cast<size_t>(RC5_C) * RC5_TILE + 125 * RC5_C * 8) * sizeof(float);
   static std::atomic<bool> attr_set[64];
@@ -1553,9 +1584,16 @@ extern "C" int rn_resample5_conv1_fused(const float* vox, const float* tex, cons
     attr_set[dev].store(true, std::memory_order_release);
   }
   resample5_conv1_kernel<<<static_cast<int>(blocks), 256, smem, static_cast<cudaStream_t>(stream)>>>(
-      vox, tex, minv, w, bias, alpha, static_cast<uint16_t*>(out16), B, size, new_size, fmt);
+      vox, tex, minv, w, bias, alpha, static_cast<uint16_t*>(out16), B, size, new_size, fmt, y0, x0, ph, pw);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int rn_resample5_conv1_fused(const float* vox, const float* tex, const float* minv, const float* w,
+                                        const float* bias, const float* alpha, void* out16, int B, int size, int new_size,
+                                        int fmt, void* stream) {
+  return rn_resample5_conv1_fused_window(vox, tex, minv, w, bias, alpha, out16, B, size, new_size, 0, 0, new_size, new_size,
+                                         fmt, stream);
 }
 
 extern "C" int rn_binvox_decode(const uint8_t* pairs, const int* run_start, const int* item_first_run, float* out,

@@ -16,7 +16,7 @@ import torch
 
 from . import ops
 from . import tfcompat as tf
-from .resampling_voxel_grid import ConcatResampledGrid, ResampledGrid
+from .resampling_voxel_grid import ConcatResampledGrid, CroppedGrid, ResampledGrid
 from .tfcompat import Deferred, realize
 
 USE_MERGED_TCONV = True    # one launch (N = 4*Cout, 9 taps) instead of 4 phase launches for k=4 stride-2 transposed convs
@@ -544,40 +544,48 @@ def _deferred_direct3d(x, w, b, stride):
         if wd is None:
             wd = w.to(_store().device).contiguous()
             _store().packed[("w32", w._rn_name)] = wd
-        if (USE_FUSED_RESAMPLE_CONV1 and isinstance(xin, ResampledGrid) and xin.transform and xin._value is None
-                and key == (1, 8, 5) and list(stride) == [2, 2, 2] and xin.new_size % 16 == 0
+        # a CroppedGrid (training on patches) runs the same fused kernels on its window; the record keeps the whole grid and
+        # the window, so one tape format serves both
+        grid, window = (xin.grid, xin.window) if isinstance(xin, CroppedGrid) else (xin, None)
+        if (USE_FUSED_RESAMPLE_CONV1 and isinstance(grid, ResampledGrid) and grid.transform and xin._value is None
+                and key == (1, 8, 5) and list(stride) == [2, 2, 2] and grid.new_size % 16 == 0
                 and act in (None, "prelu") and residual is None and not want32):
             # resample + axis transform + e_conv1 + bias + PReLU in one kernel; the 128^3 grid is never written
             bd = _dev_vec(b) if b is not None else torch.zeros(cout, device=wd.device, dtype=torch.float32)
             ad = _alpha_arg(alpha, cout) if act == "prelu" else None
             if act == "prelu" and _store().tape is not None and _store().keep_preact and not isinstance(alpha, str):
-                z = ops.resample_conv1(xin.voxel, xin.minv, xin.new_size, wd, bd, None, tf.COMPUTE_DTYPE, fmt=_store().fmt)
+                z = ops.resample_conv1(grid.voxel, grid.minv, grid.new_size, wd, bd, None, tf.COMPUTE_DTYPE, fmt=_store().fmt,
+                                       window=window)
                 y = ops.bias_act(z, None, _dev_vec(alpha), "prelu")         # training step: keep z (see _deferred_conv.run)
-                _record(op="resample_conv1", grid=xin, w=w, b=b, act=act, alpha=alpha, stride=list(stride), y=y, rerun=lambda: z)
+                _record(op="resample_conv1", grid=grid, window=window, w=w, b=b, act=act, alpha=alpha, stride=list(stride), y=y,
+                        rerun=lambda: z)
                 return y
-            y = ops.resample_conv1(xin.voxel, xin.minv, xin.new_size, wd, bd, ad, tf.COMPUTE_DTYPE, fmt=_store().fmt)
-            _record(op="resample_conv1", grid=xin, w=w, b=b, act=act, alpha=alpha, stride=list(stride), y=y,
-                    rerun=lambda: ops.resample_conv1(xin.voxel, xin.minv, xin.new_size, wd, bd, None, tf.COMPUTE_DTYPE,
-                                                     fmt=_store().fmt))
+            y = ops.resample_conv1(grid.voxel, grid.minv, grid.new_size, wd, bd, ad, tf.COMPUTE_DTYPE, fmt=_store().fmt,
+                                   window=window)
+            _record(op="resample_conv1", grid=grid, window=window, w=w, b=b, act=act, alpha=alpha, stride=list(stride), y=y,
+                    rerun=lambda: ops.resample_conv1(grid.voxel, grid.minv, grid.new_size, wd, bd, None, tf.COMPUTE_DTYPE,
+                                                     fmt=_store().fmt, window=window))
             return y
-        if (USE_FUSED_RESAMPLE_CONV1 and isinstance(xin, ConcatResampledGrid) and xin.transform and xin._value is None
-                and key == (5, 8, 5) and list(stride) == [2, 2, 2] and xin.new_size % 16 == 0
+        if (USE_FUSED_RESAMPLE_CONV1 and isinstance(grid, ConcatResampledGrid) and grid.transform and xin._value is None
+                and key == (5, 8, 5) and list(stride) == [2, 2, 2] and grid.new_size % 16 == 0
                 and act in (None, "prelu") and residual is None and not want32):
             # Texture net: resample (C=1) + resample (C=4) + concat + e_conv1 + bias + PReLU in one kernel
             bd = _dev_vec(b) if b is not None else torch.zeros(cout, device=wd.device, dtype=torch.float32)
             ad = _alpha_arg(alpha, cout) if act == "prelu" else None
 
             def z5():
-                return ops.resample5_conv1(xin.geom.voxel, xin.tex.voxel, xin.minv, xin.new_size, wd, bd, None, tf.COMPUTE_DTYPE,
-                                           fmt=_store().fmt)
+                return ops.resample5_conv1(grid.geom.voxel, grid.tex.voxel, grid.minv, grid.new_size, wd, bd, None,
+                                           tf.COMPUTE_DTYPE, fmt=_store().fmt, window=window)
             if act == "prelu" and _store().tape is not None and _store().keep_preact and not isinstance(alpha, str):
                 z = z5()
                 y = ops.bias_act(z, None, _dev_vec(alpha), "prelu")         # training step: keep z (see _deferred_conv.run)
-                _record(op="resample5_conv1", grid=xin, w=w, b=b, act=act, alpha=alpha, stride=list(stride), y=y, rerun=lambda: z)
+                _record(op="resample5_conv1", grid=grid, window=window, w=w, b=b, act=act, alpha=alpha, stride=list(stride),
+                        y=y, rerun=lambda: z)
                 return y
-            y = ops.resample5_conv1(xin.geom.voxel, xin.tex.voxel, xin.minv, xin.new_size, wd, bd, ad, tf.COMPUTE_DTYPE,
-                                    fmt=_store().fmt)
-            _record(op="resample5_conv1", grid=xin, w=w, b=b, act=act, alpha=alpha, stride=list(stride), y=y, rerun=z5)
+            y = ops.resample5_conv1(grid.geom.voxel, grid.tex.voxel, grid.minv, grid.new_size, wd, bd, ad, tf.COMPUTE_DTYPE,
+                                    fmt=_store().fmt, window=window)
+            _record(op="resample5_conv1", grid=grid, window=window, w=w, b=b, act=act, alpha=alpha, stride=list(stride), y=y,
+                    rerun=z5)
             return y
         xt = realize(xin)
         if not xt.is_cuda:

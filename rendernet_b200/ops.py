@@ -136,14 +136,38 @@ def round_up(v: int, m: int) -> int:
 
 
 # --------------------------------------------------------------------------------------- resampler
-def resample(vox: torch.Tensor, minv: torch.Tensor, new_size: int, transform: bool) -> torch.Tensor:
-    """vox [B,S,S,S,C] fp32, minv [B,3,4] fp32 -> [B,N,N,N,C] fp32 (rn_resample_f32)."""
+def check_window(window, new_size: int):
+    """A patch window (y0, x0, ph, pw) of the axis-transformed new_size^3 grid -- rows [y0, y0+ph), columns [x0, x0+pw), every
+    depth -- as ints; ValueError unless ph and pw are multiples of 16 (the fused e_conv1's 8^3 output tiles at stride 2) and the
+    window lies inside the grid.  Checked before anything is launched."""
+    y0, x0, ph, pw = (int(v) for v in window)
+    if ph < 16 or pw < 16 or ph % 16 or pw % 16:
+        raise ValueError(f"patch window {ph}x{pw}: the extents must be positive multiples of 16")
+    if not (0 <= y0 <= new_size - ph and 0 <= x0 <= new_size - pw):
+        raise ValueError(f"patch window origin ({y0}, {x0}) with extent {ph}x{pw} leaves the {new_size}^3 grid")
+    return y0, x0, ph, pw
+
+
+def resample(vox: torch.Tensor, minv: torch.Tensor, new_size: int, transform: bool, window=None) -> torch.Tensor:
+    """vox [B,S,S,S,C] fp32, minv [B,3,4] fp32 -> [B,N,N,N,C] fp32 (rn_resample_f32).  window = (y0, x0, ph, pw) (check_window;
+    transform only, C = 1 or 4): the patch out[:, y0:y0+ph, x0:x0+pw] alone, [B,ph,pw,N,C], bit for bit (rn_resample_window_f32)."""
+    if window is not None:
+        y0, x0, ph, pw = check_window(window, new_size)
+        if not transform:
+            raise ValueError("resample: a patch window is taken from the axis-transformed grid (transform=True)")
     vox = _cuda(vox, torch.float32)
     minv = _cuda(minv, torch.float32)
     B, S, _, _, Cc = vox.shape
-    out = torch.empty((B, new_size, new_size, new_size, Cc), device=vox.device, dtype=torch.float32)
-    check(lib.rn_resample_f32(vox.data_ptr(), minv.data_ptr(), out.data_ptr(), B, Cc, S, new_size,
-                              1 if transform else 0, _stream()), "rn_resample_f32")
+    if window is None:
+        out = torch.empty((B, new_size, new_size, new_size, Cc), device=vox.device, dtype=torch.float32)
+        check(lib.rn_resample_f32(vox.data_ptr(), minv.data_ptr(), out.data_ptr(), B, Cc, S, new_size,
+                                  1 if transform else 0, _stream()), "rn_resample_f32")
+        return out
+    if Cc not in (1, 4) or tuple(minv.shape) != (B, 3, 4):
+        raise ValueError(f"resample: a windowed resample takes C = 1 or 4 channels, got {tuple(vox.shape)}")
+    out = torch.empty((B, ph, pw, new_size, Cc), device=vox.device, dtype=torch.float32)
+    check(lib.rn_resample_window_f32(vox.data_ptr(), minv.data_ptr(), out.data_ptr(), B, Cc, S, new_size, y0, x0, ph, pw,
+                                     _stream()), "rn_resample_window_f32")
     return out
 
 
@@ -534,9 +558,12 @@ def conv3d_direct(x: torch.Tensor, w_tf: torch.Tensor, bias: torch.Tensor, alpha
 
 
 def resample_conv1(vox: torch.Tensor, minv: torch.Tensor, new_size: int, w_tf: torch.Tensor, bias: torch.Tensor,
-                   alpha: Optional[torch.Tensor], dtype: torch.dtype = torch.float16, fmt: Optional[int] = None):
+                   alpha: Optional[torch.Tensor], dtype: torch.dtype = torch.float16, fmt: Optional[int] = None, window=None):
     """Fused resampler + axis transform + e_conv1 (5^3 s2, 1->8) + bias + PReLU; empty tiles skip the conv.
-    vox fp32 [B,S,S,S,1], minv fp32 [B,3,4], w_tf fp32 [5,5,5,1,8] -> 16-bit [B,new/2,new/2,new/2,8]."""
+    vox fp32 [B,S,S,S,1], minv fp32 [B,3,4], w_tf fp32 [5,5,5,1,8] -> 16-bit [B,new/2,new/2,new/2,8].  window = (y0, x0, ph, pw)
+    (check_window): e_conv1 on that patch of the grid, SAME-padded at the patch's borders -> [B,ph/2,pw/2,new/2,8]
+    (rn_resample_conv1_fused_window)."""
+    y0, x0, ph, pw = (0, 0, new_size, new_size) if window is None else check_window(window, new_size)
     vox = _cuda(vox, torch.float32)
     minv = _cuda(minv, torch.float32)
     w_tf = _cuda(w_tf, torch.float32)
@@ -544,32 +571,42 @@ def resample_conv1(vox: torch.Tensor, minv: torch.Tensor, new_size: int, w_tf: t
     B, S = vox.shape[0], vox.shape[1]
     if tuple(vox.shape) != (B, S, S, S, 1) or tuple(w_tf.shape) != (5, 5, 5, 1, 8) or tuple(minv.shape) != (B, 3, 4):
         raise ValueError(f"resample_conv1: unsupported shapes {tuple(vox.shape)}, {tuple(w_tf.shape)}")
-    No = new_size // 2
     fmt = fmt_of(dtype) if fmt is None else int(fmt)
-    out = _alloc16((B, No, No, No, 8), fmt, dtype, vox.device)
-    check(lib.rn_resample_conv1_fused(vox.data_ptr(), minv.data_ptr(), w_tf.data_ptr(), bias.data_ptr(), _ptr(alpha),
-                                      out.data_ptr(), B, S, new_size, fmt, _stream()),
-          "rn_resample_conv1_fused")
+    out = _alloc16((B, ph // 2, pw // 2, new_size // 2, 8), fmt, dtype, vox.device)
+    if window is None:
+        check(lib.rn_resample_conv1_fused(vox.data_ptr(), minv.data_ptr(), w_tf.data_ptr(), bias.data_ptr(), _ptr(alpha),
+                                          out.data_ptr(), B, S, new_size, fmt, _stream()),
+              "rn_resample_conv1_fused")
+    else:
+        check(lib.rn_resample_conv1_fused_window(vox.data_ptr(), minv.data_ptr(), w_tf.data_ptr(), bias.data_ptr(), _ptr(alpha),
+                                                 out.data_ptr(), B, S, new_size, y0, x0, ph, pw, fmt, _stream()),
+              "rn_resample_conv1_fused_window")
     return _wrap16(out, fmt)
 
 
 def resample5_conv1(vox: torch.Tensor, tex: torch.Tensor, minv: torch.Tensor, new_size: int, w_tf: torch.Tensor,
                     bias: torch.Tensor, alpha: Optional[torch.Tensor], dtype: torch.dtype = torch.float16,
-                    fmt: Optional[int] = None):
+                    fmt: Optional[int] = None, window=None):
     """Texture net input chain in one kernel (rn_resample5_conv1_fused): resample geometry (C = 1) and texture volume (C = 4)
     with one pose + axis transform + concat + e_conv1 (5^3 s2, 5 -> 8) + bias + PReLU.
-    vox fp32 [B,S,S,S,1], tex fp32 [B,S,S,S,4], minv fp32 [B,3,4], w_tf fp32 [5,5,5,5,8] -> 16-bit [B,new/2,new/2,new/2,8]."""
+    vox fp32 [B,S,S,S,1], tex fp32 [B,S,S,S,4], minv fp32 [B,3,4], w_tf fp32 [5,5,5,5,8] -> 16-bit [B,new/2,new/2,new/2,8].
+    window = (y0, x0, ph, pw): on that patch, as resample_conv1 -> [B,ph/2,pw/2,new/2,8] (rn_resample5_conv1_fused_window)."""
+    y0, x0, ph, pw = (0, 0, new_size, new_size) if window is None else check_window(window, new_size)
     vox, tex, minv = _cuda(vox, torch.float32), _cuda(tex, torch.float32), _cuda(minv, torch.float32)
     w_tf, bias = _cuda(w_tf, torch.float32), _cuda(bias, torch.float32)
     B, S = vox.shape[0], vox.shape[1]
     if (tuple(vox.shape) != (B, S, S, S, 1) or tuple(tex.shape) != (B, S, S, S, 4) or tuple(w_tf.shape) != (5, 5, 5, 5, 8)
             or tuple(minv.shape) != (B, 3, 4)):
         raise ValueError(f"resample5_conv1: unsupported shapes {tuple(vox.shape)}, {tuple(tex.shape)}, {tuple(w_tf.shape)}")
-    No = new_size // 2
     fmt = fmt_of(dtype) if fmt is None else int(fmt)
-    out = _alloc16((B, No, No, No, 8), fmt, dtype, vox.device)
-    check(lib.rn_resample5_conv1_fused(vox.data_ptr(), tex.data_ptr(), minv.data_ptr(), w_tf.data_ptr(), bias.data_ptr(),
-                                       _ptr(alpha), out.data_ptr(), B, S, new_size, fmt, _stream()), "rn_resample5_conv1_fused")
+    out = _alloc16((B, ph // 2, pw // 2, new_size // 2, 8), fmt, dtype, vox.device)
+    if window is None:
+        check(lib.rn_resample5_conv1_fused(vox.data_ptr(), tex.data_ptr(), minv.data_ptr(), w_tf.data_ptr(), bias.data_ptr(),
+                                           _ptr(alpha), out.data_ptr(), B, S, new_size, fmt, _stream()), "rn_resample5_conv1_fused")
+    else:
+        check(lib.rn_resample5_conv1_fused_window(vox.data_ptr(), tex.data_ptr(), minv.data_ptr(), w_tf.data_ptr(),
+                                                  bias.data_ptr(), _ptr(alpha), out.data_ptr(), B, S, new_size, y0, x0, ph, pw,
+                                                  fmt, _stream()), "rn_resample5_conv1_fused_window")
     return _wrap16(out, fmt)
 
 
@@ -848,20 +885,32 @@ def resample_backward(vox: torch.Tensor, minv: torch.Tensor, gout: torch.Tensor,
 
 
 def resample5_backward(vox: torch.Tensor, tex: torch.Tensor, minv: torch.Tensor, gout: torch.Tensor, want_dvox: bool = True,
-                       want_dtex: bool = True, want_dminv: bool = True):
+                       want_dtex: bool = True, want_dminv: bool = True, window=None):
     """Backward of `resample5_conv1`'s input chain (rn_resample5_backward_f32): gout = dL/d(concat) fp32 [B,N,N,N,5] ->
-    (dvox [B,S,S,S,1], dtex [B,S,S,S,4], dminv [B,3,4]), fp32, each None unless asked for."""
+    (dvox [B,S,S,S,1], dtex [B,S,S,S,4], dminv [B,3,4]), fp32, each None unless asked for.  window = (y0, x0, ph, pw)
+    (check_window): gout = dL/d(the concat's patch) [B,ph,pw,N,5]; only the patch's points scatter
+    (rn_resample5_backward_window_f32)."""
+    if window is not None:
+        N = int(gout.shape[3])
+        y0, x0, ph, pw = check_window(window, N)
     vox, tex, minv, gout = (_cuda(t, torch.float32) for t in (vox, tex, minv, gout))
     B, S = vox.shape[0], vox.shape[1]
-    N = gout.shape[1]
+    if window is None:
+        N = gout.shape[1]
+        ph = pw = N
     if (tuple(vox.shape) != (B, S, S, S, 1) or tuple(tex.shape) != (B, S, S, S, 4) or tuple(minv.shape) != (B, 3, 4)
-            or tuple(gout.shape) != (B, N, N, N, 5)):
+            or tuple(gout.shape) != (B, ph, pw, N, 5)):
         raise ValueError(f"resample5_backward: unsupported shapes {tuple(vox.shape)}, {tuple(tex.shape)}, {tuple(gout.shape)}")
     dvox = torch.zeros_like(vox) if want_dvox else None
     dtex = torch.zeros_like(tex) if want_dtex else None
     dminv = torch.zeros_like(minv) if want_dminv else None
-    check(lib.rn_resample5_backward_f32(vox.data_ptr(), tex.data_ptr(), minv.data_ptr(), gout.data_ptr(), _ptr(dvox), _ptr(dtex),
-                                        _ptr(dminv), B, S, N, _stream()), "rn_resample5_backward_f32")
+    if window is None:
+        check(lib.rn_resample5_backward_f32(vox.data_ptr(), tex.data_ptr(), minv.data_ptr(), gout.data_ptr(), _ptr(dvox),
+                                            _ptr(dtex), _ptr(dminv), B, S, N, _stream()), "rn_resample5_backward_f32")
+    else:
+        check(lib.rn_resample5_backward_window_f32(vox.data_ptr(), tex.data_ptr(), minv.data_ptr(), gout.data_ptr(), _ptr(dvox),
+                                                   _ptr(dtex), _ptr(dminv), B, S, N, y0, x0, ph, pw, _stream()),
+              "rn_resample5_backward_window_f32")
     return dvox, dtex, dminv
 
 

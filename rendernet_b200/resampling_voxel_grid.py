@@ -122,11 +122,51 @@ class ConcatResampledGrid:
         return list(self.shape)
 
 
+class CroppedGrid:
+    """A deferred patch of an axis-transformed ResampledGrid (C = 1 or 4) or ConcatResampledGrid: rows [y0, y0+ph), columns
+    [x0, x0+pw), every depth -- what tools/model_util.py:77-161 slice out of the rotated grid for training on random patches.
+    When the consumer is e_conv1 the fused kernels run on the window alone (rn_resample*_conv1_fused_window; SAME padding at
+    the patch's borders, as after a slice), so neither the grid nor the patch is written.  ph and pw are multiples of 16."""
+
+    def __init__(self, grid, y0: int, x0: int, ph: int, pw: int):
+        if not isinstance(grid, (ResampledGrid, ConcatResampledGrid)) or not grid.transform or grid._value is not None:
+            raise ValueError("CroppedGrid: crops a deferred, axis-transformed resampled grid")
+        if isinstance(grid, ResampledGrid) and grid.shape[-1] not in (1, 4):
+            raise ValueError("CroppedGrid: a resampled grid of 1 or 4 channels")
+        self.window = ops.check_window((y0, x0, ph, pw), grid.new_size)
+        self.grid = grid
+        self.minv, self.new_size, self.transform = grid.minv, grid.new_size, True
+        B, N, C = grid.shape[0], grid.new_size, grid.shape[-1]
+        self.shape = (B, int(ph), int(pw), N, C)
+        self.dtype = torch.float32
+        self._value = None
+
+    def realize(self) -> torch.Tensor:
+        if self._value is None:
+            g, w = self.grid, self.window
+            if isinstance(g, ConcatResampledGrid):
+                self._value = ops.concat_channels(ops.resample(g.geom.voxel, g.minv, g.new_size, True, window=w),
+                                                  ops.resample(g.tex.voxel, g.minv, g.new_size, True, window=w))
+            else:
+                self._value = ops.resample(g.voxel, g.minv, g.new_size, True, window=w)
+        return self._value
+
+    def get_shape(self):
+        return list(self.shape)
+
+
 def concat_resampled(a, b):
-    """tf.concat([a, b], 4): stays deferred for (geometry, texture) pairs of resampled grids, plain concat otherwise."""
+    """tf.concat([a, b], 4): stays deferred for (geometry, texture) pairs of resampled grids, and for pairs of patches of them
+    cropped at one window, plain concat otherwise."""
     if isinstance(a, ResampledGrid) and isinstance(b, ResampledGrid) and a._value is None and b._value is None:
         try:
             return ConcatResampledGrid(a, b)
+        except ValueError:
+            pass
+    if (isinstance(a, CroppedGrid) and isinstance(b, CroppedGrid) and a.window == b.window and a._value is None
+            and b._value is None and isinstance(a.grid, ResampledGrid) and isinstance(b.grid, ResampledGrid)):
+        try:
+            return CroppedGrid(ConcatResampledGrid(a.grid, b.grid), *a.window)
         except ValueError:
             pass
     return ops.concat_channels(a.realize() if hasattr(a, "realize") else a, b.realize() if hasattr(b, "realize") else b)

@@ -13,8 +13,15 @@ PReLU-slope reductions) -> rn_adam_step on every variable -> the kernel-ready pa
 re-packed from the updated fp32 masters at the next forward.
 
 Scope notes.  The variables live on the device as fp32 masters (exactly what TF keeps); arithmetic inside the convolutions is the
-store's precision mode ("exact": fp16 hi/lo operand pairs, fp32-equivalent; "fast": fp16 operands, gradients loss-scaled).  The
-reference's random patch crop (:152-155, a memory workaround of 2018 GPUs) is not reproduced: a step trains on whole frames.
+store's precision mode ("exact": fp16 hi/lo operand pairs, fp32-equivalent; "fast": fp16 operands, gradients loss-scaled).
+
+Patches.  The reference trains on random patches (:150-156, tools/model_util.py:77-161): one P x P window of the rotated,
+axis-transformed 128^3 grid (all 128 depths, one origin per batch), the network's SAME padding at the window's borders, and the
+target cropped at 4x the origin with a 4P edge; P = 32 for the first epochs, then 64 (patch_size_for_epoch).  `step(...,
+patch_size=P)` does the same: the origin comes from crop_origin (deterministic in (seed, step, rank)), the fused resample + e_conv1
+kernels run on the window alone (resampling_voxel_grid.CroppedGrid), the loss is the reference's over the patch, and the backward
+walk (e_conv1's filter gradient, the texture decoder's gradients) sees the window only.  patch_size None or new_size trains on
+whole frames; validation (training=False) always renders whole frames, as the reference's tf.cond does.
 Data loading, the Supervisor / checkpoint loop and sample dumps (:170-306) stay out of scope (SURVEY §2)."""
 from __future__ import annotations
 
@@ -30,15 +37,42 @@ from . import tfcompat as tf
 from .RenderNet_Shader import RenderNet
 from .backward import ShaderInputGradients, TextureInputGradients, _key
 from .engine import pose_to_matrix
-from .resampling_voxel_grid import ResampledGrid
+from .resampling_voxel_grid import CroppedGrid, ResampledGrid
 
 # every path of a backward walk reaches e_conv1's filter gradient: an fp16 overflow anywhere makes it non-finite
 E_CONV1_WEIGHTS = "encoder/e_conv1/e_conv1/weights"
+_M64 = (1 << 64) - 1
 
 
 def _as_device_f32(t, like: torch.Tensor) -> torch.Tensor:
     t = torch.as_tensor(np.asarray(t, np.float32) if not isinstance(t, torch.Tensor) else t)
     return t.to(device=like.device, dtype=torch.float32).reshape(tuple(like.shape)).contiguous()
+
+
+def _splitmix64(x: int) -> int:
+    z = (x + 0x9E3779B97F4A7C15) & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def patch_size_for_epoch(epoch: int, network: str = "shader", new_size: int = 128) -> int:
+    """The reference's patch schedule: new_size // 4 for the first 5 epochs of the Shader (RenderNet_Shader.py:204-207) or the
+    first 4 of the Texture+Normal network (RenderNet_Texture_Face_Normal.py:225-228), new_size // 2 after."""
+    first = {"shader": 5, "texture": 4}.get(network)
+    if first is None:
+        raise ValueError(f"network must be 'shader' or 'texture', not {network!r}")
+    return new_size // 4 if epoch < first else new_size // 2
+
+
+def _crop_image(t, y0: int, x0: int, patch: int, new_size: int):
+    """The target patch of a voxel window (tools/model_util.py:94-99): rows / columns from f x the origin, edge f x patch, with
+    f = image_dim // new_size.  NumPy targets are cropped on the host, before the copy to the device."""
+    if not isinstance(t, torch.Tensor):
+        t = np.asarray(t, np.float32)
+    f = int(t.shape[1]) // new_size
+    c = t[:, y0 * f:(y0 + patch) * f, x0 * f:(x0 + patch) * f]
+    return c.contiguous() if isinstance(c, torch.Tensor) else np.ascontiguousarray(c)
 
 
 class _Trainer:
@@ -66,6 +100,7 @@ class _Trainer:
         self.m: Dict[str, torch.Tensor] = {}
         self.v: Dict[str, torch.Tensor] = {}
         self.last_loss: Optional[float] = None
+        self.last_crop = None            # ((y0, x0), P) of the last training forward on a patch, None after a whole frame
 
     # ------------------------------------------------------------------------------------------- pieces of a step
     def learning_rate(self, step: Optional[int] = None) -> float:
@@ -73,12 +108,33 @@ class _Trainer:
         step = self.global_step if step is None else step
         return self.e_eta * self.decay_rate ** (step // self.decay_steps)
 
+    def _rank(self) -> int:
+        if self.data_parallel and torch.distributed.is_available() and torch.distributed.is_initialized():
+            return torch.distributed.get_rank()
+        return 0
+
     def dropout_seed(self, step: int) -> int:
         """Seed of the dropout masks of optimiser step `step` (mixes the trainer's seed and the step; 32 bits)."""
-        rank = 0
-        if self.data_parallel and torch.distributed.is_available() and torch.distributed.is_initialized():
-            rank = torch.distributed.get_rank()           # data-parallel ranks draw different masks from the same trainer seed
+        rank = self._rank()                               # data-parallel ranks draw different masks from the same trainer seed
         return (self.seed * 0x9E3779B1 + step * 0x85EBCA6B + rank * 0xC2B2AE35 + 0x1234567) & 0xFFFFFFFF
+
+    def crop_origin(self, step: int, patch_size: int):
+        """(y0, x0) of optimiser step `step`'s patch, each uniform on [0, new_size - patch_size]: one origin per batch, as the
+        reference's tf.random_uniform([2]) (tools/model_util.py:93), drawn by SplitMix64 from (seed, step, rank) -- the rank only
+        with data_parallel, as in dropout_seed.  Deterministic, so an overflow retry of a step trains on the same patch."""
+        n = self.new_size - int(patch_size) + 1
+        if n < 1:
+            raise ValueError(f"patch_size {patch_size} exceeds the {self.new_size}-grid")
+        key = _splitmix64((self.seed & _M64) ^ _splitmix64(step * 0xC2B2AE3D27D4EB4F + self._rank() * 0x165667B19E3779F9))
+        return _splitmix64(key) % n, _splitmix64(key ^ 0xA0761D6478BD642F) % n
+
+    def _window(self, training: bool, patch_size, origin):
+        """(y0, x0, P, P) of a training step on patches, or None (whole frames: validation, patch_size None or new_size)."""
+        if not training or patch_size is None or int(patch_size) == self.new_size:
+            return None
+        P = int(patch_size)
+        y0, x0 = self.crop_origin(self.global_step, P) if origin is None else (int(origin[0]), int(origin[1]))
+        return ops.check_window((y0, x0, P, P), self.new_size)
 
     @contextlib.contextmanager
     def _training_tape(self, training: bool):
@@ -130,13 +186,13 @@ class _Trainer:
             raise RuntimeError(f"{len(missing)} variables received no gradient, e.g. {missing[:3]}")
 
     # ------------------------------------------------------------------------------------------- the step
-    def _step(self, *inputs) -> float:
+    def _step(self, *inputs, patch_size=None, origin=None) -> float:
         """One optimiser step on `inputs` (loss_and_gradients' arguments); returns the loss BEFORE the update."""
         dp = self.data_parallel and torch.distributed.is_available() and torch.distributed.is_initialized()
         for _ in range(12):
             overflow = False
             try:
-                loss, grads = self.loss_and_gradients(*inputs, training=True)
+                loss, grads = self.loss_and_gradients(*inputs, training=True, patch_size=patch_size, origin=origin)
             except FloatingPointError:                 # dynamic loss scaling: halve and redo the step (same dropout masks)
                 overflow = True
             if dp:                                     # every rank must take the same branch
@@ -199,20 +255,29 @@ class ShaderTrainer(_Trainer, ShaderInputGradients):
         self._init_training(keep_prob, learning_rate, decay_steps, decay_rate, beta1, beta2, epsilon, seed, data_parallel)
         self.loss_kind = loss or ("bce" if is_greyscale else "mse")        # RenderNet_Shader.py:158-163
 
-    def forward(self, voxels, view_params, training: bool = True) -> torch.Tensor:
-        """The training-mode forward pass (dropout masks drawn from (seed, global_step, call index, element)); tape recorded."""
+    def forward(self, voxels, view_params, training: bool = True, window=None) -> torch.Tensor:
+        """The training-mode forward pass (dropout masks drawn from (seed, global_step, call index, element)); tape recorded.
+        window = (y0, x0, ph, pw): the network runs on that patch of the rotated grid -> image [B,4ph,4pw,C]."""
         dev = self.store.device
         self.view_params = np.asarray(view_params, np.float32)
         self.vox = torch.as_tensor(np.asarray(voxels, np.float32)).reshape(self.B, self.size, self.size, self.size, 1).to(dev)
         self.minv = torch.from_numpy(pose_to_matrix(self.view_params, self.size, self.new_size)).to(dev)
         with self._training_tape(training):
             grid = ResampledGrid(self.vox, self.minv, self.new_size, transform=True)
+            if window is not None:
+                grid = CroppedGrid(grid, *window)
             self.img = RenderNet(grid, is_training=training, prob=self.keep_prob, is_greyscale=self.is_greyscale)
         return self.img
 
-    def loss_and_gradients(self, voxels, view_params, target, training: bool = True):
-        """-> (loss (Python float), {variable name: dL/dvariable fp32 device tensor}); no update."""
-        img = self.forward(voxels, view_params, training=training)
+    def loss_and_gradients(self, voxels, view_params, target, training: bool = True, patch_size=None, origin=None):
+        """-> (loss (Python float), {variable name: dL/dvariable fp32 device tensor}); no update.  target: the whole frame
+        [B,512,512,C].  patch_size (training only): the forward, the loss and the gradients cover one patch_size^2 window of the
+        grid at `origin` (default crop_origin(global_step, patch_size)) and the matching target patch."""
+        window = self._window(training, patch_size, origin)
+        self.last_crop = None if window is None else (window[:2], window[2])
+        if window is not None:
+            target = _crop_image(target, window[0], window[1], window[2], self.new_size)
+        img = self.forward(voxels, view_params, training=training, window=window)
         tgt = _as_device_f32(target, img)
         with torch.cuda.device(self.device):
             loss, dimg = ops.image_loss_grad(img.contiguous(), tgt, self.loss_kind)
@@ -222,9 +287,10 @@ class ShaderTrainer(_Trainer, ShaderInputGradients):
         self.last_loss = float(loss.item())
         return self.last_loss, self.weight_grads
 
-    def step(self, voxels, view_params, target) -> float:
-        """One optimiser step (RenderNet_Shader.py:156-167); returns the loss BEFORE the update."""
-        return self._step(voxels, view_params, target)
+    def step(self, voxels, view_params, target, patch_size=None, origin=None) -> float:
+        """One optimiser step (RenderNet_Shader.py:156-167); returns the loss BEFORE the update.  patch_size / origin: train on a
+        patch (loss_and_gradients)."""
+        return self._step(voxels, view_params, target, patch_size=patch_size, origin=origin)
 
 
 class TextureTrainer(_Trainer, TextureInputGradients):
@@ -250,16 +316,24 @@ class TextureTrainer(_Trainer, TextureInputGradients):
                          loss_scale=loss_scale, seed=seed, device=device)
         self._init_training(keep_prob, learning_rate, decay_steps, decay_rate, beta1, beta2, epsilon, seed, data_parallel)
 
-    def forward(self, voxels, texture, view_params, training: bool = True):
-        """The training-mode forward pass -> (image, normal map), fp32 [B,512,512,3] each on the device; tape recorded."""
+    def forward(self, voxels, texture, view_params, training: bool = True, window=None):
+        """The training-mode forward pass -> (image, normal map), fp32 [B,512,512,3] each on the device; tape recorded.
+        window = (y0, x0, ph, pw): the network runs on that patch of the concatenated grid -> [B,4ph,4pw,3] each."""
         self._set_inputs(voxels, texture, view_params)
         with self._training_tape(training):
-            self._record_network(is_training=training, prob=self.keep_prob)
+            self._record_network(is_training=training, prob=self.keep_prob, window=window)
         return self.albedo, self.normal
 
-    def loss_and_gradients(self, voxels, texture, view_params, image_target, normal_target, training: bool = True):
-        """-> (loss (Python float), {variable name: dL/dvariable fp32 device tensor}); no update."""
-        img, nrm = self.forward(voxels, texture, view_params, training=training)
+    def loss_and_gradients(self, voxels, texture, view_params, image_target, normal_target, training: bool = True,
+                           patch_size=None, origin=None):
+        """-> (loss (Python float), {variable name: dL/dvariable fp32 device tensor}); no update.  Targets: whole frames;
+        patch_size / origin as in ShaderTrainer.loss_and_gradients (both targets cropped at the same window)."""
+        window = self._window(training, patch_size, origin)
+        self.last_crop = None if window is None else (window[:2], window[2])
+        if window is not None:
+            image_target = _crop_image(image_target, window[0], window[1], window[2], self.new_size)
+            normal_target = _crop_image(normal_target, window[0], window[1], window[2], self.new_size)
+        img, nrm = self.forward(voxels, texture, view_params, training=training, window=window)
         with torch.cuda.device(self.device):
             l_img, d_img = ops.image_loss_grad(img.contiguous(), _as_device_f32(image_target, img), "mse")
             l_nrm, d_nrm = ops.image_loss_grad(nrm.contiguous(), _as_device_f32(normal_target, nrm), "mse")
@@ -281,6 +355,7 @@ class TextureTrainer(_Trainer, TextureInputGradients):
         self.last_loss = float((l_img + l_nrm).item())
         return self.last_loss, self.weight_grads
 
-    def step(self, voxels, texture, view_params, image_target, normal_target) -> float:
-        """One optimiser step (RenderNet_Texture_Face_Normal.py:176-187); returns the loss BEFORE the update."""
-        return self._step(voxels, texture, view_params, image_target, normal_target)
+    def step(self, voxels, texture, view_params, image_target, normal_target, patch_size=None, origin=None) -> float:
+        """One optimiser step (RenderNet_Texture_Face_Normal.py:176-187); returns the loss BEFORE the update.  patch_size /
+        origin: train on a patch (loss_and_gradients)."""
+        return self._step(voxels, texture, view_params, image_target, normal_target, patch_size=patch_size, origin=origin)
