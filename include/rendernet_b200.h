@@ -281,6 +281,18 @@ int rn_concat_channels_f32(const float* a, const float* b, float* out, long long
 int rn_phong_composite(const float* img, const float* light_dir, const float* light_col, float ambient,
                        float k_diffuse, int background_white, int with_mask, float* out_f32, uint8_t* out_u8,
                        int B, int H, int W, void* stream);
+/* Shaded image of a normal map and an albedo: shade = Phong composite of `normal` [B,H,W,3] fp32, compos = albedo * shade (fp32,
+ * one multiply; albedo NULL: compos = shade).  composite = RN_PHONG_NUMPY: rn_phong_composite's arithmetic (tools/Phong_shading.py:
+ * 138-228); RN_PHONG_TF: TensorFlow's tf_phong_composite (:24-113), bit-identical to the shading rn_phong_recon_loss_grad
+ * measures (white mask sigmoid(255 (sqrt 3 - |n|) - 80), black sigmoid(255 |n| - 80), evaluated in double).  light_dir,
+ * light_col [B,3]; background_white selects the mask (and the colour the background is composited to).  Outputs, each NULL or
+ * [B,H,W,3]: shade_f32, compos_f32, compos_u8 = clip(255 compos, 0, 255) truncated to uint8 (RenderNet_demo.py:58).  At least
+ * one must be given.  rn_phong_composite is this entry with RN_PHONG_NUMPY, no albedo and compos as its output. */
+#define RN_PHONG_NUMPY 0
+#define RN_PHONG_TF 1
+int rn_phong_shade(const float* normal, const float* albedo, const float* light_dir, const float* light_col, float ambient,
+                   float k_diffuse, int composite, int background_white, int with_mask, float* shade_f32, float* compos_f32,
+                   uint8_t* compos_u8, int B, int H, int W, void* stream);
 
 /* ---- backward pass: input gradients of the forward path (SURVEY 8 f-4) --------------------------------------------
  * What inverse rendering differentiates through the frozen network (Reconstruct_RenderNet_Face.py:383-412).  The data

@@ -19,7 +19,8 @@ gradient.  `FaceReconstruction` puts them together into the reference's optimisa
 (:402-412, plain gradient descent on the latent, pose, texture and light azimuth), `run` the outer loop over pose hypotheses
 (`reconstruction_loop`, :455-537, with `create_param_center`, :304-318).  Deliberate differences: the first epoch's texture
 vectors come from a seeded generator (the reference calls the unseeded np.random.randn), and the reference's PNG / binvox / npz
-dumps (:497-519, :535) are replaced by a callback that receives the state after every step.
+dumps (:497-519, :535) are replaced by a callback that receives the state after every step; `FaceReconstruction.render(state)`
+produces the images those dumps show (shading, normal map, shaded prediction, voxels), also from other views and lights.
 """
 from __future__ import annotations
 
@@ -380,6 +381,26 @@ class FaceReconstruction:
             loss = ops.phong_recon_loss_grad(albedo, normal, self._target_dev(target), ldir, lcol, 0., 1.,
                                              black_background=False, with_mask=True)[0]
         return loss.cpu().numpy()
+
+    def render(self, state, view_params=None, light_azimuth=None) -> Dict[str, np.ndarray]:
+        """The images of a state (what :497-508 fetches every 100 steps): the shape decoder, the Texture+Normal network and the
+        shading of :372-378 (rn_phong_shade, TensorFlow's composite, white background, mask, ambient 0, k_d 1, light colour 1),
+        i.e. the very image the loss measures.  view_params [B,3] / light_azimuth [B,1] (radians) render the state's face from
+        another pose or under another light; None keeps the state's own.  Returns NumPy albedo, normal, shading, compos
+        (float32 [B,512,512,3]), compos_u8 (clip(255 compos) as uint8) and voxels ([B,64,64,64] float32)."""
+        B = self.B
+        pose = state["pose"] if view_params is None else view_params
+        az = state["light"] if light_azimuth is None else light_azimuth
+        pose = np.asarray(pose, np.float32).reshape(B, 3)
+        az = np.asarray(az, np.float64).reshape(B, 1)
+        vox = self.sdg.forward(state["latent"])
+        albedo, normal = self.tig.forward(vox, state["texture"], pose)
+        with torch.cuda.device(self.device):
+            ldir = torch.from_numpy(light_pos(az, self.elevation)).to(self.device)
+            shade, compos, u8 = ops.phong_shade(normal, ldir, (1.0, 1.0, 1.0), 0., 1., albedo=albedo, composite="tf",
+                                                background_white=True, with_mask=True)
+        out = dict(albedo=albedo, normal=normal, shading=shade, compos=compos, compos_u8=u8, voxels=vox[..., 0])
+        return {k: v.cpu().numpy() for k, v in out.items()}
 
     def run(self, target, callback: Optional[Callable] = None) -> Dict[str, object]:
         """The whole reconstruction (:455-537) from a shaded target [B,512,512,3]: reconstruction_loop with this object's step and

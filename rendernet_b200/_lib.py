@@ -107,7 +107,9 @@ SIGNATURES = {
     "rn_image_loss_grad": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
     "rn_adam_step": (_i, [_vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _vp]),
     "rn_phong_composite": (_i, [_vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _i, _i, _i, _vp]),
+    "rn_phong_shade": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
 }
+RN_PHONG_NUMPY, RN_PHONG_TF = 0, 1
 
 
 def _load():

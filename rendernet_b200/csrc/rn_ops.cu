@@ -981,21 +981,36 @@ __global__ void binvox_decode_kernel(const uint8_t* __restrict__ pairs, const in
 }
 
 // ------------------------------------------------------------------------------------------ Phong
-__global__ void phong_kernel(const float* __restrict__ img, const float* __restrict__ light_dir,
-                             const float* __restrict__ light_col, float ambient, float k_diffuse, int white,
-                             int with_mask, float* __restrict__ out_f32, uint8_t* __restrict__ out_u8, int B,
-                             long long npix) {
-  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (i >= static_cast<long long>(B) * npix) return;
-  const int b = static_cast<int>(i / npix);
-  const float r = img[3 * i], g = img[3 * i + 1], bl = img[3 * i + 2];
-  float v[3];
-  phong_pixel(r, g, bl, light_dir[3 * b], light_dir[3 * b + 1], light_dir[3 * b + 2], light_col + 3 * b, ambient, k_diffuse, white,
-              with_mask, v);
+// The one Phong pass (rn_phong_shade; rn_phong_composite is its NumPy-composite, no-albedo case).  One thread per pixel,
+// blockIdx.y = batch item.  shade = phong_pixel (TF = false) or tf_phong_pixel (TF = true); compos = albedo * shade, or shade
+// itself without an albedo; each of shade_f32, compos_f32 and compos_u8 (= clip(255 compos) truncated) may be NULL.
+template <bool TF>
+__global__ void __launch_bounds__(256) phong_shade_kernel(const float* __restrict__ normal, const float* __restrict__ albedo,
+                                                          const float* __restrict__ light_dir, const float* __restrict__ light_col,
+                                                          float ambient, float k_diffuse, int white, int with_mask,
+                                                          float* __restrict__ shade_f32, float* __restrict__ compos_f32,
+                                                          uint8_t* __restrict__ compos_u8, int HW) {
+  const int b = blockIdx.y;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= HW) return;
+  const size_t o = (static_cast<size_t>(b) * HW + p) * 3;
+  const float l0 = __ldg(light_dir + 3 * b), l1 = __ldg(light_dir + 3 * b + 1), l2 = __ldg(light_dir + 3 * b + 2);
+  const float col[3] = {__ldg(light_col + 3 * b), __ldg(light_col + 3 * b + 1), __ldg(light_col + 3 * b + 2)};
+  const float n0 = normal[o], n1 = normal[o + 1], n2 = normal[o + 2];
+  float s[3];
+  if constexpr (TF) {
+    const float lnorm = sqrtf(l0 * l0 + l1 * l1 + l2 * l2);                // as phong_recon_loss_grad_kernel normalises it
+    const float L[3] = {l0 / lnorm, l1 / lnorm, l2 / lnorm};
+    tf_phong_pixel(n0, n1, n2, L, col, ambient, k_diffuse, !white, with_mask, s);
+  } else {
+    phong_pixel(n0, n1, n2, l0, l1, l2, col, ambient, k_diffuse, white, with_mask, s);
+  }
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    if (out_f32 != nullptr) out_f32[3 * i + c] = v[c];
-    if (out_u8 != nullptr) out_u8[3 * i + c] = phong_u8(v[c]);
+    const float v = albedo != nullptr ? albedo[o + c] * s[c] : s[c];
+    if (shade_f32 != nullptr) shade_f32[o + c] = s[c];
+    if (compos_f32 != nullptr) compos_f32[o + c] = v;
+    if (compos_u8 != nullptr) compos_u8[o + c] = phong_u8(v);
   }
 }
 
@@ -1611,11 +1626,25 @@ extern "C" int rn_phong_composite(const float* img, const float* light_dir, cons
                                   float k_diffuse, int background_white, int with_mask, float* out_f32,
                                   uint8_t* out_u8, int B, int H, int W, void* stream) {
   if (!img || !light_dir || !light_col || (!out_f32 && !out_u8)) return -1;
-  const long long npix = static_cast<long long>(H) * W;
-  const long long total = npix * B;
-  const int block = 256;
-  phong_kernel<<<static_cast<int>((total + block - 1) / block), block, 0, static_cast<cudaStream_t>(stream)>>>(
-      img, light_dir, light_col, ambient, k_diffuse, background_white, with_mask, out_f32, out_u8, B, npix);
+  return rn_phong_shade(img, nullptr, light_dir, light_col, ambient, k_diffuse, RN_PHONG_NUMPY, background_white, with_mask,
+                        nullptr, out_f32, out_u8, B, H, W, stream);
+}
+
+extern "C" int rn_phong_shade(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
+                              float ambient, float k_diffuse, int composite, int background_white, int with_mask, float* shade_f32,
+                              float* compos_f32, uint8_t* compos_u8, int B, int H, int W, void* stream) {
+  if (!normal || !light_dir || !light_col || (!shade_f32 && !compos_f32 && !compos_u8) || B < 1 || H < 1 || W < 1) return -1;
+  if (composite != RN_PHONG_NUMPY && composite != RN_PHONG_TF) return -1;
+  if (B > 65535 || static_cast<long long>(H) * W > 0x7fffffffLL - 255) return -2;
+  const int HW = H * W;
+  const dim3 grid((HW + 255) / 256, B);
+  const int white = background_white != 0, mask = with_mask != 0;
+  if (composite == RN_PHONG_TF)
+    phong_shade_kernel<true><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, shade_f32, compos_f32, compos_u8, HW);
+  else
+    phong_shade_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, shade_f32, compos_f32, compos_u8, HW);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }

@@ -1,6 +1,7 @@
 // rn_phong.cuh -- one pixel of the demo's Phong composite (tools/Phong_shading.py:138-228 np_mask / np_phong_shading /
 // np_phong_composite, RenderNet_demo.py:54-58), shared by the stand-alone kernel (rn_ops.cu) and the fused epilogue of the
-// last up-conv (rn_igemm_kernel.cuh) so that both produce the same bits.
+// last up-conv (rn_igemm_kernel.cuh) so that both produce the same bits; and one pixel of TensorFlow's composite
+// (tf_phong_pixel), which the stand-alone kernel renders for face reconstruction.
 #pragma once
 #include <cstdint>
 
@@ -29,5 +30,33 @@ __device__ __forceinline__ void phong_pixel(float r, float g, float bl, float lx
   }
 }
 __device__ __forceinline__ uint8_t phong_u8(float v) { return static_cast<uint8_t>(fminf(fmaxf(255.f * v, 0.f), 255.f)); }
+
+// TensorFlow's composite (tools/Phong_shading.py:24-113 tf_mask / tf_mask_white / tf_phong_shading / tf_phong_composite), the
+// shading Reconstruct_RenderNet_Face.py:372-378 multiplies the albedo by.  (n0,n1,n2) = normal map in [0,1]; L = the light
+// direction ALREADY normalised as l / |l| (division, not a reciprocal); col = light colour.  The operation order, the fp32
+// rounding points and the mask in double are those of the forward half of phong_recon_loss_grad_kernel (rn_backward.cu), so the
+// image this returns is the one the reconstruction loss measures, bit for bit.  Unlike phong_pixel: the normal is not clamped
+// away from |n - 0.5| = 0, the white mask is sigmoid(255 (sqrt 3 - |n|) - 80) and the black one sigmoid(255 |n| - 80).
+__device__ __forceinline__ void tf_phong_pixel(float n0, float n1, float n2, const float* L, const float* col, float ambient,
+                                               float k_diffuse, int black, int with_mask, float* out) {
+  const float v[3] = {n0 - 0.5f, n1 - 0.5f, n2 - 0.5f};
+  const float vn = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+  const float u[3] = {v[0] / vn, v[1] / vn, v[2] / vn};
+  const float d = u[0] * L[0] + u[1] * L[1] + u[2] * L[2];
+  const float dmax = fmaxf(d, 0.f);
+  float m = 1.f;
+  if (with_mask) {
+    const double nnd = sqrt(static_cast<double>(n0) * n0 + static_cast<double>(n1) * n1 + static_cast<double>(n2) * n2);
+    const double s = black ? 255.0 * nnd - 80.0 : 255.0 * (1.7320508075688772 - nnd) - 80.0;
+    m = static_cast<float>(1.0 / (1.0 + exp(-s)));
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float pre = k_diffuse * dmax * col[c];
+    const float dif = fminf(fmaxf(pre, 0.f), 1.f);
+    const float x = with_mask ? m * (ambient + dif) + (1.f - m) : ambient + dif;
+    out[c] = fminf(fmaxf(x, 0.f), 1.f);
+  }
+}
 
 }  // namespace rn

@@ -286,59 +286,127 @@ class RenderEngine(_EngineBase):
         return got[0] if self.phong is None else (got[0], got[1])
 
 
+TEXTURE_PHONG_DEFAULTS = dict(light_col=(1.0, 1.0, 1.0), ambient=0.0, k_diffuse=1.0, composite="tf", background_white=True,
+                              with_mask=True)     # the reconstruction's shading (Reconstruct_RenderNet_Face.py:326-328, :377)
+
+
 class TextureRenderEngine(_EngineBase):
     """BASELINE config 4: voxels + 199-d texture vector + pose -> (albedo image, normal map), as one CUDA graph
     (texture decoder -> two resamplings (C=1, C=4) -> concat -> Texture/Normal RenderNet;
-    RenderNet_Texture_Face_Normal.py:155-179)."""
+    RenderNet_Texture_Face_Normal.py:155-179).
+
+    model="texture": RenderNet_Texture_Face_Normal's decoder_texture + RenderNet on `weights` {tf variable name: array} (None:
+    the seeded initialisers).  model="pretrained": Reconstruct_RenderNet_Face's texture_decoder_pretrained + RenderNet_pretrained
+    on the npz-keyed dictionary FaceReconstruction holds (ReLU residual blocks), as backward.TextureInputGradients does.
+
+    phong=dict(light_dir [1|B,3], light_col=(1,1,1), ambient=0., k_diffuse=1., composite="tf", background_white=True,
+    with_mask=True) adds the shaded image to the step: compos = albedo * Phong(normal, light) (composite "tf": the reconstruction's
+    tf_phong_composite, "numpy": the demo's np_phong_composite) and its uint8 form, in one more kernel inside the same graph.
+    The outputs are then (albedo, normal, compos, compos_u8).  The light direction is a device input like the voxels: `upload`,
+    `submit` and `render` take light_dir=[1|B,3] (None: the light given here), so relighting needs no re-capture."""
 
     def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, size: int = 64, new_size: int = 128,
                  use_graph: bool = True, seed: int = 0, device: str = "cuda", precision: str = "fast", strict: bool = True,
-                 fuse_input: bool = True):
-        super().__init__(weights, precision, seed, device, use_graph, strict)
+                 fuse_input: bool = True, model: str = "texture", phong: Optional[dict] = None):
+        if model not in ("texture", "pretrained"):
+            raise ValueError(f"model must be 'texture' or 'pretrained', not {model!r}")
+        if model == "pretrained" and weights is None:
+            raise ValueError("model='pretrained' builds its variables from the npz-keyed weight dictionary: pass one")
+        if phong is not None:
+            unknown = set(phong) - set(TEXTURE_PHONG_DEFAULTS) - {"light_dir"}
+            if unknown or "light_dir" not in phong:
+                raise ValueError(f"phong needs light_dir and takes {sorted(TEXTURE_PHONG_DEFAULTS)}; got {sorted(phong)}")
+            phong = {**TEXTURE_PHONG_DEFAULTS, **phong}
+            if phong["composite"] not in ops.PHONG_COMPOSITES:
+                raise ValueError(f"phong composite must be one of {sorted(ops.PHONG_COMPOSITES)}, not {phong['composite']!r}")
+            self._light_default = self._light_rows(phong["light_dir"], batch, "light_dir")
+            light_col = self._light_rows(phong["light_col"], batch, "light_col")
+        super().__init__(weights if model == "texture" else None, precision, seed, device, use_graph, strict)
         self.B, self.size, self.new_size = batch, size, new_size
+        self.model = model
+        self.weight_dict = weights if model == "pretrained" else None
+        self.phong = phong
         self.fuse_input = fuse_input      # False: two stand-alone resamplings + concat + CUDA-core e_conv1 (the r01 path; A/B, tests)
         dev = self.device
         self.vox = torch.zeros((batch, size, size, size, 1), device=dev, dtype=torch.float32)
         self.tex = torch.zeros((batch, 199), device=dev, dtype=torch.float32)
         self.minv = torch.zeros((batch, 3, 4), device=dev, dtype=torch.float32)
         self.inputs = [self.vox, self.tex, self.minv]
+        if phong is not None:
+            self.light_dir = self._light_default.to(dev)          # the graph reads this buffer: a step's light is uploaded into it
+            self.light_col = light_col.to(dev)
+            self.inputs.append(self.light_dir)
         self.out = None
         self._finish_init()
-        self.vox_host, self.tex_host, self.minv_host = self.inputs_host
+        self.vox_host, self.tex_host, self.minv_host = self.inputs_host[:3]
         self.out_host = tuple(self.outputs_host)
+
+    @staticmethod
+    def _light_rows(t, B, what) -> torch.Tensor:
+        t = torch.as_tensor(np.asarray(t.cpu() if isinstance(t, torch.Tensor) else t, np.float32))
+        if t.dim() == 1 and t.numel() == 3:
+            t = t.reshape(1, 3)
+        if t.dim() != 2 or t.shape[1] != 3 or t.shape[0] not in (1, B):
+            raise ValueError(f"{what} must have shape [1,3] or [{B},3], not {tuple(t.shape)}")
+        return t.expand(B, 3).contiguous()
 
     def _forward(self):
         from .RenderNet_Texture_Face_Normal import RenderNet as RenderNetTexture, decoder_texture
+        from .Reconstruct_RenderNet_Face import RenderNet_pretrained, texture_decoder_pretrained
         # both resamplings stay deferred: resample x2 + axis transform + concat + e_conv1 run as one kernel
-        tex3d = tf.realize(decoder_texture(self.tex))
+        if self.model == "texture":
+            tex3d = tf.realize(decoder_texture(self.tex))
+        else:
+            tex3d = tf.realize(texture_decoder_pretrained(self.tex, self.weight_dict))
         if not self.fuse_input:
             x5 = ops.concat_channels(ops.resample(self.vox, self.minv, self.new_size, True),
                                      ops.resample(tex3d, self.minv, self.new_size, True))
         else:
             x5 = ConcatResampledGrid(ResampledGrid(self.vox, self.minv, self.new_size, transform=True),
                                      ResampledGrid(tex3d, self.minv, self.new_size, transform=True))
-        self.out = RenderNetTexture(x5, is_training=False)
+        if self.model == "texture":
+            self.out = RenderNetTexture(x5, is_training=False)
+        else:
+            self.out = RenderNet_pretrained(x5, self.weight_dict)
+        if self.phong is not None:
+            albedo, normal = self.out
+            p = self.phong
+            _, compos, u8 = ops.phong_shade(normal, self.light_dir, self.light_col, p["ambient"], p["k_diffuse"], albedo=albedo,
+                                            composite=p["composite"], background_white=p["background_white"],
+                                            with_mask=p["with_mask"], want_shade=False)
+            self.out = (albedo, normal, compos, u8)
         return list(self.out)
 
-    def _host_inputs(self, voxels, texture, view_params):
-        return [torch.as_tensor(np.asarray(voxels, np.float32)), torch.as_tensor(np.asarray(texture, np.float32)),
-                torch.from_numpy(pose_to_matrix(view_params, self.size, self.new_size))]
+    def _host_inputs(self, voxels, texture, view_params, light_dir=None):
+        got = [torch.as_tensor(np.asarray(voxels, np.float32)), torch.as_tensor(np.asarray(texture, np.float32)),
+               torch.from_numpy(pose_to_matrix(view_params, self.size, self.new_size))]
+        if self.phong is not None:
+            got.append(self._light_default if light_dir is None else self._light_rows(light_dir, self.B, "light_dir"))
+        elif light_dir is not None:
+            raise ValueError("light_dir needs an engine built with phong=")
+        return got
+
+    def _pipe_outputs(self):
+        return [0, 1] if self.phong is None else [3]          # (albedo, normal), or the uint8 shaded image
 
     def step_device(self):
         super().step_device()
         return self.out
 
-    def upload(self, voxels, texture, view_params):
-        self._upload(self._host_inputs(voxels, texture, view_params))
+    def upload(self, voxels, texture, view_params, light_dir=None):
+        self._upload(self._host_inputs(voxels, texture, view_params, light_dir))
 
-    def submit(self, voxels, texture, view_params) -> int:
-        """Pipelined step (see RenderEngine.submit); `result(ticket)` -> (albedo image, normal map) in pinned host memory."""
-        return self._submit(self._host_inputs(voxels, texture, view_params))
+    def submit(self, voxels, texture, view_params, light_dir=None) -> int:
+        """Pipelined step (see RenderEngine.submit); `result(ticket)` -> (albedo image, normal map) in pinned host memory, or
+        with phong the uint8 shaded image alone (what RenderEngine ships).  light_dir: this step's light (None: the engine's)."""
+        return self._submit(self._host_inputs(voxels, texture, view_params, light_dir))
 
     def result(self, ticket: int):
-        return tuple(self._result(ticket))
+        got = self._result(ticket)
+        return tuple(got) if self.phong is None else got[0]
 
-    def render(self, voxels, texture, view_params):
-        self.upload(voxels, texture, view_params)
+    def render(self, voxels, texture, view_params, light_dir=None):
+        """-> (albedo, normal) fp32 [B,512,512,3] on the host, or with phong (albedo, normal, compos fp32, compos uint8)."""
+        self.upload(voxels, texture, view_params, light_dir)
         self.step_device()
-        return tuple(self._download([0, 1]))
+        return tuple(self._download(range(len(self.outputs))))

@@ -672,6 +672,55 @@ def phong_composite(img: torch.Tensor, light_dir: torch.Tensor, light_col: torch
     return (out, u8) if want_u8 else out
 
 
+PHONG_COMPOSITES = {"numpy": 0, "tf": 1}      # RN_PHONG_NUMPY, RN_PHONG_TF
+
+
+def _light_rows(t, B: int, device, what: str) -> torch.Tensor:
+    """[1|B,3] light direction / colour (tensor, array or sequence) -> contiguous fp32 [B,3] on `device`.  A [B,3] fp32 CUDA
+    tensor on `device` is used as it is (no copy), so a buffer that a CUDA graph reads can be passed."""
+    import numpy as np
+    t = t if isinstance(t, torch.Tensor) else torch.as_tensor(np.asarray(t, np.float32))
+    if t.dim() == 1 and t.numel() == 3:
+        t = t.reshape(1, 3)
+    if t.dim() != 2 or t.shape[1] != 3 or t.shape[0] not in (1, B):
+        raise ValueError(f"{what} must have shape [1,3] or [{B},3], not {tuple(t.shape)}")
+    t = t.to(device=device, dtype=torch.float32)
+    return (t.expand(B, 3) if t.shape[0] != B else t).contiguous()
+
+
+def phong_shade(normal: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambient: float = 0.0, k_diffuse: float = 1.0,
+                albedo: Optional[torch.Tensor] = None, composite: str = "tf", background_white: bool = True,
+                with_mask: bool = True, want_shade: bool = True, want_compos: bool = True, want_u8: bool = True):
+    """Shaded image (rn_phong_shade): shade = Phong composite of the normal map, compos = albedo * shade.
+    normal, albedo: fp32 [B,H,W,3] CUDA tensors (albedo None: compos is shade).  light_dir, light_col: 1 or B rows of 3.
+    composite "tf": TensorFlow's tf_phong_composite, the image the reconstruction loss measures (rn_phong_recon_loss_grad);
+    "numpy": the demo's np_phong_composite (rn_phong_composite).  Returns (shade fp32, compos fp32, compos uint8 = clip(255 x)),
+    each None unless asked for; without an albedo, compos is the shade tensor itself."""
+    if composite not in PHONG_COMPOSITES:
+        raise ValueError(f"composite must be one of {sorted(PHONG_COMPOSITES)}, not {composite!r}")
+    if len(normal.shape) != 4 or normal.shape[3] != 3:
+        raise ValueError(f"phong_shade: normal map must be [B,H,W,3], not {tuple(normal.shape)}")
+    B, H, W, _ = normal.shape
+    if albedo is not None and tuple(albedo.shape) != tuple(normal.shape):
+        raise ValueError(f"phong_shade: albedo {tuple(albedo.shape)} and normal map {tuple(normal.shape)} differ in shape")
+    ld = _light_rows(light_dir, B, normal.device, "light_dir")
+    lc = _light_rows(light_col, B, normal.device, "light_col")
+    normal = _cuda(normal, torch.float32)
+    albedo = None if albedo is None else _cuda(albedo, torch.float32)
+    alias = albedo is None and want_compos
+    if alias:
+        want_shade, want_compos = True, False           # compos == shade: one buffer
+    if not (want_shade or want_compos or want_u8):
+        raise ValueError("phong_shade: ask for at least one output")
+    shade = torch.empty_like(normal) if want_shade else None
+    compos = torch.empty_like(normal) if want_compos else None
+    u8 = torch.empty(normal.shape, device=normal.device, dtype=torch.uint8) if want_u8 else None
+    check(lib.rn_phong_shade(normal.data_ptr(), _ptr(albedo), ld.data_ptr(), lc.data_ptr(), float(ambient), float(k_diffuse),
+                             PHONG_COMPOSITES[composite], 1 if background_white else 0, 1 if with_mask else 0, _ptr(shade),
+                             _ptr(compos), _ptr(u8), B, H, W, _stream()), "rn_phong_shade")
+    return shade, (shade if alias else compos), u8
+
+
 def bias_act(x, bias: Optional[torch.Tensor], alpha: Optional[torch.Tensor], act: Optional[str],
              residual=None, want32: bool = False, fmt: int = 0):
     """y = act(x + bias[c]) + residual on a 16-bit channel-last tensor (rn_bias_act_16).  An fp32 `x` is first cast to
