@@ -345,6 +345,20 @@ int rn_phong_recon_loss_grad(const float* albedo, const float* normal, const flo
                              const float* light_col, float ambient, float k_diffuse, int black_background, int with_mask,
                              double* loss, float* d_albedo, float* d_normal, float* d_light_dir, int B, int H, int W,
                              void* stream);
+/* Shader pose / light fit objective over the demo's NumPy composite (RenderNet_demo.py:54-58, tools/Phong_shading.py:138-228):
+ * out = rn_phong_composite(img, light_dir, light_col, ambient, k_diffuse, background_white, with_mask) -- the same device function
+ * (rn_phong.cuh phong_pixel), so the image the loss measures is the one rn_phong_composite and the fused epilogue render, bit for
+ * bit -- loss[b] += mean_{h,w,c} (target - out)^2 (double [B], ACCUMULATED into), and in the same pass d_img (fp32 [B,H,W,3],
+ * overwritten) and d_light_dir [B,3] (ACCUMULATED into: zero it first; may be NULL; the light direction need not be unit: the
+ * gradient runs through l / |l|).  img, target [B,H,W,3]; light_dir, light_col [B,3].  The gradient covers n = (img - 0.5) /
+ * |img - 0.5|, l / |l| and the soft mask (sigmoid(255 |img| - 150) black, sigmoid(255 |1 - img| - 80) white), whose derivative is
+ * evaluated in double from the fp32 pixel.  Conventions as rn_phong_recon_loss_grad: max(x, 0) passes where x >= 0, a clip where
+ * lo <= x <= hi.  At img = (0.5, 0.5, 0.5) the normal is 0/0: the forward shades the pixel as unlit (as rn_phong_composite does),
+ * and the gradient there is the mask term alone (nothing through the normal, nothing to d_light_dir); at |img| = 0 (black) or
+ * |1 - img| = 0 (white) the mask term is 0. */
+int rn_phong_composite_loss_grad(const float* img, const float* target, const float* light_dir, const float* light_col,
+                                 float ambient, float k_diffuse, int background_white, int with_mask, double* loss, float* d_img,
+                                 float* d_light_dir, int B, int H, int W, void* stream);
 long long rn_fully_connected_backward_workspace(int B, int K, int N);
 int rn_fully_connected_backward_data(const float* g, const float* w, float* work, float* dx, int B, int K, int N, void* stream);
 
@@ -419,6 +433,12 @@ int rn_dropout_mask_host(unsigned char* mask, long long n, float keep, unsigned 
  * img / target / dimg fp32 [n] (dimg may be NULL), *loss (device double) is overwritten. */
 int rn_image_loss_grad(const float* img, const float* target, float* dimg, double* loss, long long n, int batch, int kind,
                        void* stream);
+/* The same losses per item, for a search over several hypotheses (Reconstruct_RenderNet_Face.py:522-534): img / target / dimg fp32
+ * [batch, npix, C] (C = 1 or 3), loss double [batch] (overwritten).  kind 0: loss[b] = mean over the item's npix * C elements of
+ * (img - target)^2; kind 1: loss[b] = -sum over them of t log(1e-6 + p) + (1 - t) log(1e-6 + 1 - p).  dimg (may be NULL) =
+ * d sum_b loss[b] / dimg, overwritten: batch x rn_image_loss_grad's gradient. */
+int rn_image_loss_grad_items(const float* img, const float* target, float* dimg, double* loss, long long npix, int C, int batch,
+                             int kind, void* stream);
 /* One tf.train.AdamOptimizer update of a flat fp32 parameter (RenderNet_Shader.py:167, beta1 = 0.5): m += (g-m)(1-beta1),
  * v += (g^2-v)(1-beta2), param -= lr_t * m / (sqrt(v) + eps), with lr_t = lr * sqrt(1-beta2^t) / (1-beta1^t) passed by the caller. */
 int rn_adam_step(float* param, const float* grad, float* m, float* v, long long n, float lr_t, float beta1, float beta2, float eps,

@@ -105,6 +105,8 @@ SIGNATURES = {
     "rn_dropout_16": (_i, [_vp, _vp, _ll, _f, C.c_uint, C.c_uint, _i, _vp]),
     "rn_dropout_mask_host": (_i, [_vp, _ll, _f, C.c_uint, C.c_uint]),
     "rn_image_loss_grad": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
+    "rn_image_loss_grad_items": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _i, _vp]),
+    "rn_phong_composite_loss_grad": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "rn_adam_step": (_i, [_vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _vp]),
     "rn_phong_composite": (_i, [_vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _i, _i, _i, _vp]),
     "rn_phong_shade": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),

@@ -9,7 +9,9 @@
 //     respect to the voxel grid (scatter-add of the 8 corner weights) and to the 3x4 inverse sampling matrix (derivative of
 //     the corner weights w.r.t. the sample coordinates), from which the host derives d/d(azimuth, elevation, scale);
 //   * the Texture net's 5-channel version of it (geometry + decoded texture sampled at one set of points), and the texture
-//     decoder's fp32 PReLU and fully_connected data gradients (RenderNet_Texture_Face_Normal.py:34-46).
+//     decoder's fp32 PReLU and fully_connected data gradients (RenderNet_Texture_Face_Normal.py:34-46);
+//   * the image objectives of inverse rendering: face reconstruction over TensorFlow's Phong composite, and the Shader pose /
+//     light fit over the demo's NumPy composite (rendernet_b200/shader_fit.py).
 #include <cstdint>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -18,6 +20,7 @@
 #include <atomic>
 
 #include "../../include/rendernet_b200.h"
+#include "rn_phong.cuh"
 
 namespace rn {
 extern std::atomic<long long> g_launch_count;
@@ -511,6 +514,100 @@ __global__ void __launch_bounds__(256) phong_recon_loss_grad_kernel(const float*
   }
 }
 
+// ------------------------------------------------------------------------------------------ Shader pose / light fit objective
+// The demo's NumPy composite (RenderNet_demo.py:54-58, tools/Phong_shading.py:138-228) against a target image:
+//   out = phong_pixel(img, l, col, ambient, k_d, white, with_mask)     (rn_phong.cuh: the image rn_phong_composite renders)
+//   loss[b] += mean_{h,w,c} (target - out)^2                           (double)
+// and its gradients in the same pass, with the conventions of phong_recon_loss_grad_kernel: max(x, 0) passes where x >= 0, a
+// clip where lo <= x <= hi.  Three paths reach img: the normalisation d = (img - 0.5) . L / |img - 0.5| (dd/dv = (L - d u) / |v|,
+// u = v / |v|), and the soft mask m = sigmoid(255 |img| - 150) (black) / sigmoid(255 |1 - img| - 80) (white), whose derivative
+// m (1 - m) 255 (+-a / |a|) is evaluated in double from the fp32 pixel (the argument multiplies |a|'s rounding by 255).  dL/dL
+// = dd u is reduced over the block and mapped through the light's normalisation (I - L L^T) / |l|.  At img = (0.5, 0.5, 0.5)
+// d is 0 * inf = NaN; phong_pixel's fmaxf turns it into 0 (the pixel is shaded as if unlit) and the gradient passes nothing
+// through the normal there (only the mask term reaches d_img; nothing reaches d_light).  Where |a| = 0 the mask term is 0.
+__global__ void __launch_bounds__(256) phong_composite_loss_grad_kernel(const float* __restrict__ img, const float* __restrict__ target,
+                                                                        const float* __restrict__ light_dir,
+                                                                        const float* __restrict__ light_col, float ambient,
+                                                                        float k_diffuse, int white, int with_mask,
+                                                                        double* __restrict__ loss, float* __restrict__ d_img,
+                                                                        float* __restrict__ d_light, int HW) {
+  __shared__ double red_loss[8];
+  __shared__ float red[8][3];
+  const int b = blockIdx.y;
+  const float l0 = __ldg(light_dir + 3 * b), l1 = __ldg(light_dir + 3 * b + 1), l2 = __ldg(light_dir + 3 * b + 2);
+  const float col[3] = {__ldg(light_col + 3 * b), __ldg(light_col + 3 * b + 1), __ldg(light_col + 3 * b + 2)};
+  const float inv_n = 2.f / (3.f * static_cast<float>(HW));          // d mean / d out, times the 2 of the square
+  double lsum = 0.0;
+  float dl[3] = {0.f, 0.f, 0.f};                                      // dL/dL (the normalised light)
+  PhongTerms t;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;               // < HW for thread 0 of every block
+  if (p < HW) {
+    const size_t o = (static_cast<size_t>(b) * HW + p) * 3;
+    const float r = img[o], g = img[o + 1], bl = img[o + 2];
+    float out[3];
+    phong_pixel(r, g, bl, l0, l1, l2, col, ambient, k_diffuse, white, with_mask, out, &t);
+    float dndl = 0.f, dm = 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float res = out[c] - target[o + c];
+      lsum += static_cast<double>(res) * res;
+      const float dx = (t.x[c] >= 0.f && t.x[c] <= 1.f) ? inv_n * res : 0.f;      // clip(compos, 0, 1)
+      if (with_mask) dm += dx * (ambient + t.diff[c] - 1.f);
+      const float ddiff = with_mask ? dx * t.mask : dx;
+      const float dpre = (t.pre[c] >= 0.f && t.pre[c] <= 1.f) ? ddiff : 0.f;      // clip(diffuse, 0, 1)
+      dndl += dpre * k_diffuse * col[c];
+    }
+    const float dd = t.d >= 0.f ? dndl : 0.f;                        // max(d, 0); false for the NaN of img = 0.5
+    float di[3] = {0.f, 0.f, 0.f};
+    if (dd != 0.f) {
+      const float u[3] = {(r - 0.5f) * t.inv, (g - 0.5f) * t.inv, (bl - 0.5f) * t.inv};
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        di[i] = dd * (t.L[i] - t.d * u[i]) * t.inv;
+        dl[i] = dd * u[i];
+      }
+    }
+    if (with_mask && dm != 0.f) {
+      const double a[3] = {white ? 1.0 - r : static_cast<double>(r), white ? 1.0 - g : static_cast<double>(g),
+                           white ? 1.0 - bl : static_cast<double>(bl)};
+      const double nrm = sqrt(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]);
+      if (nrm > 0.0) {
+        const double md = 1.0 / (1.0 + exp(-(255.0 * nrm - (white ? 80.0 : 150.0))));
+        const double ds = static_cast<double>(dm) * md * (1.0 - md) * (white ? -255.0 : 255.0) / nrm;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) di[i] += static_cast<float>(ds * a[i]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) d_img[o + i] = di[i];
+  }
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, off);
+  if (lane == 0) red_loss[wib] = lsum;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    float v = dl[i];
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    if (lane == 0) red[wib][i] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    float v[3] = {0.f, 0.f, 0.f};
+    for (int w = 0; w < 8; ++w) {
+      s += red_loss[w];
+      for (int i = 0; i < 3; ++i) v[i] += red[w][i];
+    }
+    atomicAdd(loss + b, s / (3.0 * HW));
+    if (d_light != nullptr) {                                          // d (l/|l|) = (dL - L (L.dL)) / |l|
+      const float ldv = t.L[0] * v[0] + t.L[1] * v[1] + t.L[2] * v[2];
+      for (int i = 0; i < 3; ++i) atomicAdd(d_light + 3 * b + i, (v[i] - t.L[i] * ldv) * t.linv);
+    }
+  }
+}
+
 }  // namespace rn
 
 using namespace rn;
@@ -650,6 +747,19 @@ extern "C" int rn_phong_recon_loss_grad(const float* albedo, const float* normal
   phong_recon_loss_grad_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       albedo, normal, target, light_dir, light_col, ambient, k_diffuse, black_background, with_mask, loss, d_albedo, d_normal,
       d_light_dir, HW);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int rn_phong_composite_loss_grad(const float* img, const float* target, const float* light_dir, const float* light_col,
+                                            float ambient, float k_diffuse, int background_white, int with_mask, double* loss,
+                                            float* d_img, float* d_light_dir, int B, int H, int W, void* stream) {
+  if (!img || !target || !light_dir || !light_col || !loss || !d_img || B < 1 || H < 1 || W < 1) return -1;
+  if (static_cast<long long>(H) * W > 0x7fffffffLL - 256 || B > 65535) return -2;
+  const int HW = H * W;
+  const dim3 grid((HW + 255) / 256, B);
+  phong_composite_loss_grad_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      img, target, light_dir, light_col, ambient, k_diffuse, background_white, with_mask, loss, d_img, d_light_dir, HW);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }

@@ -1,31 +1,53 @@
 // rn_phong.cuh -- one pixel of the demo's Phong composite (tools/Phong_shading.py:138-228 np_mask / np_phong_shading /
-// np_phong_composite, RenderNet_demo.py:54-58), shared by the stand-alone kernel (rn_ops.cu) and the fused epilogue of the
-// last up-conv (rn_igemm_kernel.cuh) so that both produce the same bits; and one pixel of TensorFlow's composite
+// np_phong_composite, RenderNet_demo.py:54-58), shared by the stand-alone kernel (rn_ops.cu), the fused epilogue of the
+// last up-conv (rn_igemm_kernel.cuh) and the Shader fit's loss kernel (rn_backward.cu) so that all three produce the same bits;
+// and one pixel of TensorFlow's composite
 // (tf_phong_pixel), which the stand-alone kernel renders for face reconstruction.
 #pragma once
 #include <cstdint>
 
 namespace rn {
 
-// (r,g,b) = normal map in [0,1]; l = light direction (not normalised), col = light colour.  Returns the shaded colour.
+// The intermediate values of one phong_pixel call, for its backward (phong_composite_loss_grad_kernel, rn_backward.cu).
+struct PhongTerms {
+  float L[3];      // the normalised light l / |l|
+  float linv;      // 1 / |l|
+  float inv;       // 1 / |img - 0.5|
+  float d;         // (img - 0.5) . L / |img - 0.5|, before max(., 0)
+  float mask;      // the fp32 mask (1 without mask)
+  float pre[3];    // k_d max(d, 0) col_c, before the clip to [0, 1]
+  float diff[3];   // the clipped diffuse term
+  float x[3];      // the composite, before the clip to [0, 1]
+};
+
+// (r,g,b) = normal map in [0,1]; l = light direction (not normalised), col = light colour.  Returns the shaded colour and, if
+// `t` is not NULL, the intermediates the gradient needs (the same values: recorded, not recomputed).
 __device__ __forceinline__ void phong_pixel(float r, float g, float bl, float lx, float ly, float lz, const float* col,
-                                            float ambient, float k_diffuse, int white, int with_mask, float* out) {
+                                            float ambient, float k_diffuse, int white, int with_mask, float* out,
+                                            PhongTerms* t = nullptr) {
   // np_phong_shading (:162-200): n = (img-0.5)/|img-0.5| ; diffuse = k_d * max(n.l, 0) * light_col, clipped
   const float nx = r - 0.5f, ny = g - 0.5f, nz = bl - 0.5f;
   const float inv = 1.0f / sqrtf(nx * nx + ny * ny + nz * nz);
   const float linv = 1.0f / sqrtf(lx * lx + ly * ly + lz * lz);
   lx *= linv; ly *= linv; lz *= linv;
-  const float ndl = fmaxf((nx * lx + ny * ly + nz * lz) * inv, 0.f);
+  const float d = (nx * lx + ny * ly + nz * lz) * inv;
+  const float ndl = fmaxf(d, 0.f);
   float mask = 1.f;
   if (with_mask) {  // np_mask (:138-148) / np_mask_white (:150-160)
     const float nrm = white ? sqrtf((1.f - r) * (1.f - r) + (1.f - g) * (1.f - g) + (1.f - bl) * (1.f - bl))
                             : sqrtf(r * r + g * g + bl * bl);
     mask = 1.f / (1.f + expf(-(255.f * nrm - (white ? 80.f : 150.f))));
   }
+  if (t != nullptr) {
+    t->L[0] = lx; t->L[1] = ly; t->L[2] = lz;
+    t->linv = linv; t->inv = inv; t->d = d; t->mask = mask;
+  }
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float diff = fminf(fmaxf(k_diffuse * ndl * col[c], 0.f), 1.f);
+    const float pre = k_diffuse * ndl * col[c];
+    const float diff = fminf(fmaxf(pre, 0.f), 1.f);
     float v = with_mask ? mask * (ambient + diff) + (1.f - mask) : ambient + diff;
+    if (t != nullptr) { t->pre[c] = pre; t->diff[c] = diff; t->x[c] = v; }
     out[c] = fminf(fmaxf(v, 0.f), 1.f);
   }
 }

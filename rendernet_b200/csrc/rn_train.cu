@@ -341,6 +341,39 @@ __global__ void __launch_bounds__(256) image_loss_grad_kernel(const float* __res
   if (threadIdx.x == 0) atomicAdd(loss, red[0] * (kind == 0 ? 1.0 / static_cast<double>(n) : 1.0 / static_cast<double>(batch)));
 }
 
+// Per item (rn_image_loss_grad_items): blockIdx.y = item b of m elements.  kind 0: loss[b] = mean (p - t)^2, dL/dp = 2 (p - t) / m;
+// kind 1: loss[b] = -sum [t log(1e-6 + p) + (1 - t) log(1e-6 + 1 - p)], dL/dp = -(t / (1e-6 + p) - (1 - t) / (1e-6 + 1 - p)).
+// dimg is the gradient of sum_b loss[b].  One double atomic per block.
+__global__ void __launch_bounds__(256) image_loss_grad_items_kernel(const float* __restrict__ img, const float* __restrict__ target,
+                                                                    float* __restrict__ dimg, double* __restrict__ loss, long long m,
+                                                                    int kind) {
+  __shared__ double red[256];
+  const long long base = static_cast<long long>(blockIdx.y) * m;
+  double s = 0.0;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const float inv_m = 1.0f / static_cast<float>(m);
+  for (long long j = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; j < m; j += stride) {
+    const long long i = base + j;
+    const float p = img[i], t = target[i];
+    if (kind == 0) {
+      const float d = p - t;
+      s += static_cast<double>(d) * d;
+      if (dimg) dimg[i] = 2.0f * d * inv_m;
+    } else {
+      const float a = 1e-6f + p, b = 1e-6f + 1.0f - p;
+      s -= static_cast<double>(t * logf(a) + (1.0f - t) * logf(b));
+      if (dimg) dimg[i] = -(t / a - (1.0f - t) / b);
+    }
+  }
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) atomicAdd(loss + blockIdx.y, kind == 0 ? red[0] / static_cast<double>(m) : red[0]);
+}
+
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                    float* __restrict__ v, long long n, float lr_t, float beta1, float beta2, float eps) {
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
@@ -486,6 +519,21 @@ extern "C" int rn_image_loss_grad(const float* img, const float* target, float* 
   cudaError_t e = cudaMemsetAsync(loss, 0, sizeof(double), st);
   if (e != cudaSuccess) return static_cast<int>(e);
   image_loss_grad_kernel<<<grid_for(n, 256 * 8, 132 * 4), 256, 0, st>>>(img, target, dimg, loss, n, batch, kind);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int rn_image_loss_grad_items(const float* img, const float* target, float* dimg, double* loss, long long npix, int C,
+                                        int batch, int kind, void* stream) {
+  if (!img || !target || !loss || npix < 1 || (C != 1 && C != 3) || batch < 1 || batch > 65535 || (kind != 0 && kind != 1))
+    return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaMemsetAsync(loss, 0, static_cast<size_t>(batch) * sizeof(double), st);
+  if (e != cudaSuccess) return static_cast<int>(e);
+  const long long m = npix * C;
+  const int per_item = (132 * 4 + batch - 1) / batch;
+  const dim3 grid(static_cast<unsigned>(grid_for(m, 256 * 8, per_item)), static_cast<unsigned>(batch));
+  image_loss_grad_items_kernel<<<grid, 256, 0, st>>>(img, target, dimg, loss, m, kind);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }

@@ -1015,6 +1015,31 @@ def phong_recon_loss_grad(albedo: torch.Tensor, normal: torch.Tensor, target: to
     return loss, d_albedo, d_normal, d_light
 
 
+def phong_composite_loss_grad(img: torch.Tensor, target: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambient: float = 0.1,
+                              k_diffuse: float = 0.9, background_white: bool = False, with_mask: bool = True,
+                              want_light_grad: bool = True):
+    """The Shader fit's objective over the demo's composite (rn_phong_composite_loss_grad): loss[b] = mean (target -
+    np_phong_composite(img, light_dir, light_col, ambient, k_diffuse, background, with_mask))^2, the shading being
+    rn_phong_composite's bit for bit.  img, target fp32 [B,H,W,3] CUDA tensors; light_dir, light_col: 1 or B rows of 3 (the
+    direction need not be unit).  Defaults are the demo's (RenderNet_demo.py:18-20, black background, mask).  Returns
+    (loss fp64 [B], d_img fp32 [B,H,W,3], d_light_dir fp32 [B,3] or None)."""
+    if len(img.shape) != 4 or img.shape[3] != 3:
+        raise ValueError(f"phong_composite_loss_grad: img must be [B,H,W,3], not {tuple(img.shape)}")
+    if tuple(target.shape) != tuple(img.shape):
+        raise ValueError(f"phong_composite_loss_grad: target {tuple(target.shape)} and img {tuple(img.shape)} differ in shape")
+    B, H, W, _ = img.shape
+    ld = _light_rows(light_dir, B, img.device, "light_dir")
+    lc = _light_rows(light_col, B, img.device, "light_col")
+    img, target = _cuda(img, torch.float32), _cuda(target, torch.float32)
+    loss = torch.zeros(B, device=img.device, dtype=torch.float64)
+    d_img = torch.empty_like(img)
+    d_light = torch.zeros((B, 3), device=img.device, dtype=torch.float32) if want_light_grad else None
+    check(lib.rn_phong_composite_loss_grad(img.data_ptr(), target.data_ptr(), ld.data_ptr(), lc.data_ptr(), float(ambient),
+                                           float(k_diffuse), 1 if background_white else 0, 1 if with_mask else 0, loss.data_ptr(),
+                                           d_img.data_ptr(), _ptr(d_light), B, H, W, _stream()), "rn_phong_composite_loss_grad")
+    return loss, d_img, d_light
+
+
 def conv2d_weight_grad(x, g, kh: int, kw: int) -> torch.Tensor:
     """dW of a stride-1 SAME conv2d on the tensor cores (rn_conv2d_weight_grad): x 16-bit [B,H,W,Cin] (layer input), g 16-bit
     [B,H,W,Cout] (gradient of the conv output), same 16-bit format -> fp32 [kh,kw,Cin,Cout] (TF filter layout)."""
@@ -1156,6 +1181,28 @@ def image_loss_grad(img: torch.Tensor, target: torch.Tensor, kind: str = "mse", 
     dimg = torch.empty_like(img) if want_grad else None
     check(lib.rn_image_loss_grad(img.data_ptr(), target.data_ptr(), _ptr(dimg), loss.data_ptr(), img.numel(), int(img.shape[0]),
                                  {"mse": 0, "bce": 1}[kind], _stream()), "rn_image_loss_grad")
+    return loss, dimg
+
+
+IMAGE_LOSSES = {"mse": 0, "bce": 1}
+
+
+def image_loss_grad_items(img: torch.Tensor, target: torch.Tensor, kind: str = "mse", want_grad: bool = True):
+    """Per-item reconstruction loss (rn_image_loss_grad_items): img, target fp32 [B,H,W,C] CUDA tensors, C = 1 or 3.  "mse":
+    loss[b] = mean over the item of (img - target)^2; "bce": the reference's -sum over the item of t log(1e-6 + p) + (1 - t)
+    log(1e-6 + 1 - p).  Returns (loss fp64 [B], d sum_b loss[b] / dimg fp32 like img, or None)."""
+    if kind not in IMAGE_LOSSES:
+        raise ValueError(f"kind must be one of {sorted(IMAGE_LOSSES)}, not {kind!r}")
+    if len(img.shape) != 4 or img.shape[3] not in (1, 3):
+        raise ValueError(f"image_loss_grad_items: img must be [B,H,W,1|3], not {tuple(img.shape)}")
+    if tuple(target.shape) != tuple(img.shape):
+        raise ValueError(f"image_loss_grad_items: target {tuple(target.shape)} and img {tuple(img.shape)} differ in shape")
+    img, target = _cuda(img, torch.float32), _cuda(target, torch.float32)
+    B, H, W, C_ = img.shape
+    loss = torch.empty(B, device=img.device, dtype=torch.float64)
+    dimg = torch.empty_like(img) if want_grad else None
+    check(lib.rn_image_loss_grad_items(img.data_ptr(), target.data_ptr(), _ptr(dimg), loss.data_ptr(), H * W, C_, B,
+                                       IMAGE_LOSSES[kind], _stream()), "rn_image_loss_grad_items")
     return loss, dimg
 
 
