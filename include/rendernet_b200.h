@@ -443,6 +443,19 @@ int rn_image_loss_grad_items(const float* img, const float* target, float* dimg,
  * v += (g^2-v)(1-beta2), param -= lr_t * m / (sqrt(v) + eps), with lr_t = lr * sqrt(1-beta2^t) / (1-beta1^t) passed by the caller. */
 int rn_adam_step(float* param, const float* grad, float* m, float* v, long long n, float lr_t, float beta1, float beta2, float eps,
                  void* stream);
+/* Shape fit through the Shader network (rendernet_b200/shape_fit.py): the gradient of
+ *   L(occ) = sum_v loss_v + lambda_smooth R_s + lambda_bin R_b,
+ *   R_s = (1/N) sum over axis-neighbour pairs (i, j) inside the grid (no wrap-around) of (occ_i - occ_j)^2,
+ *   R_b = (1/N) sum_i occ_i (1 - occ_i),   N = S^3,
+ * w.r.t. one occupancy grid that every view renders.  dvox fp32 [V, S^3]: the per-view dL/dvoxels rn_resample_backward_f32
+ * writes; occ fp32 [S^3]; keep uint8 [S^3] or NULL (1 = voxel not carved away).  g fp32 [S^3], overwritten:
+ *   g[i] = keep[i] ? sum_v dvox[v][i] + lambda_smooth dR_s/docc_i + lambda_bin dR_b/docc_i : 0
+ * (the view sum in double, v = 0..V-1).  reg double [2] = (R_s, R_b), overwritten; both are taken over the whole grid, carved
+ * voxels included.  work: rn_voxel_fit_grad_workspace(S) doubles.  The reduction has a fixed order (block partials, then one
+ * block; the block count depends on S alone): two launches are bit-identical.  lambda_* >= 0 and finite, else rc -1. */
+long long rn_voxel_fit_grad_workspace(int S);
+int rn_voxel_fit_grad(const float* dvox, const float* occ, const unsigned char* keep, float* g, double* reg, double* work, int V,
+                      int S, float lambda_smooth, float lambda_bin, void* stream);
 
 #ifdef __cplusplus
 }

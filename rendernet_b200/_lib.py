@@ -108,6 +108,8 @@ SIGNATURES = {
     "rn_image_loss_grad_items": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _i, _vp]),
     "rn_phong_composite_loss_grad": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "rn_adam_step": (_i, [_vp, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _vp]),
+    "rn_voxel_fit_grad_workspace": (_ll, [_i]),
+    "rn_voxel_fit_grad": (_i, [_vp] * 6 + [_i, _i, _f, _f, _vp]),
     "rn_phong_composite": (_i, [_vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _i, _i, _i, _vp]),
     "rn_phong_shade": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
 }

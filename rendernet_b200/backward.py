@@ -495,9 +495,14 @@ class ShaderInputGradients(_InputGradients):
 
     # ------------------------------------------------------------------------------------------- forward
     def forward(self, voxels, view_params) -> torch.Tensor:
+        """voxels [B,64,64,64,1], view_params [B,3] -> image [B,512,512,3|1] fp32 on the device.  voxels may be a CUDA tensor
+        (e.g. a shape fit's occupancy, expanded over the views): it is used in place, without a host round trip."""
         dev = self.store.device
         self.view_params = np.asarray(view_params, np.float32)
-        self.vox = torch.as_tensor(np.asarray(voxels, np.float32)).reshape(self.B, self.size, self.size, self.size, 1).to(dev)
+        if isinstance(voxels, torch.Tensor) and voxels.is_cuda:
+            self.vox = voxels.to(device=dev, dtype=torch.float32).reshape(self.B, self.size, self.size, self.size, 1).contiguous()
+        else:
+            self.vox = torch.as_tensor(np.asarray(voxels, np.float32)).reshape(self.B, self.size, self.size, self.size, 1).to(dev)
         self.minv = torch.from_numpy(pose_to_matrix(self.view_params, self.size, self.new_size)).to(dev)
         self.tape = []
         self.store.tape = self.tape
@@ -511,8 +516,9 @@ class ShaderInputGradients(_InputGradients):
 
     # ------------------------------------------------------------------------------------------- backward
     def backward(self, dimg, want_dvox: bool = True, want_dpose: bool = True, want_weight_grads: bool = False,
-                 tensor_core_wgrad: bool = True):
+                 tensor_core_wgrad: bool = True, dvox_on_device: bool = False):
         """dimg: dL/dimg [B,512,512,3|1] (NumPy or tensor).  Returns (dL/dvoxels [B,S,S,S,1] or None, dL/dview_params [B,3] or None).
+        dvox_on_device: dL/dvoxels stays a CUDA tensor (for the shape fit's rn_voxel_fit_grad).
         want_weight_grads: also fills `self.weight_grads` {variable name: fp32 device tensor in the variable's TF layout} for EVERY
         variable the forward pass used -- filters (wgmma weight-gradient kernel for the wide stride-1 2-D layers and, depth-folded,
         the 3^3 layers; the strided-correlation kernel rn_conv_weight_grad_direct for the thin / strided / transposed ones), biases
@@ -551,7 +557,9 @@ class ShaderInputGradients(_InputGradients):
         dpose = None
         if want_dpose:
             dpose = pose_matrix_jacobian_vjp(self.view_params, dminv.cpu().numpy(), self.size, self.new_size)
-        return (dvox.cpu().numpy() if dvox is not None else None), dpose
+        if dvox is not None and not dvox_on_device:
+            dvox = dvox.cpu().numpy()
+        return dvox, dpose
 
     def _input_chain(self, rec, g, grads):
         """e_conv1 (5^3 s2, 1 -> 8) fused with the resampler: its data gradient dL/dgrid, fp32 and un-scaled."""

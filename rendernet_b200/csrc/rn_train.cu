@@ -11,6 +11,8 @@
 //     the same call applied to the gradient is its backward (the mask is recomputed, never stored).
 //   * rn_image_loss_grad         : reconstruction loss and its gradient w.r.t. the image (MSE :163, BCE :160-161).
 //   * rn_adam_step               : one Adam update of a flat fp32 parameter (TF formulation: lr_t folded by the caller).
+//   * rn_voxel_fit_grad          : the shape fit's gradient w.r.t. the shared occupancy grid (views summed, smoothness and
+//     binary regularisers, carve mask) and the two regularisers, with a fixed-order reduction.
 #include <cstdint>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -387,6 +389,89 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
   }
 }
 
+// Shape fit (rn_voxel_fit_grad): one thread per voxel i = (a*S + b)*S + c of the shared grid.  R_s takes the pairs (i, i+1) along
+// each axis once, from their lower voxel; dR_s/docc_i = (2/N) sum over i's in-grid axis neighbours j of (occ_i - occ_j).  The sum
+// over views runs v = 0..V-1 in double.  Each block writes its (R_s, R_b) partial sums; voxel_fit_reg_kernel adds them in order.
+__global__ void __launch_bounds__(256) voxel_fit_grad_kernel(const float* __restrict__ dvox, const float* __restrict__ occ,
+                                                             const unsigned char* __restrict__ keep, float* __restrict__ g,
+                                                             double* __restrict__ part, int V, int S, double ls, double lb) {
+  __shared__ double red[2][256];
+  const long long n = static_cast<long long>(S) * S * S, ss = static_cast<long long>(S) * S;
+  const double inv_n = 1.0 / static_cast<double>(n);
+  double rs = 0.0, rb = 0.0;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const unsigned iu = static_cast<unsigned>(i), su = static_cast<unsigned>(S);        // n <= 2^30
+    const int c = static_cast<int>(iu % su), b = static_cast<int>((iu / su) % su), a = static_cast<int>(iu / (su * su));
+    const double o = occ[i];
+    double ds = 0.0;
+    auto axis = [&](int p, long long step) {
+      if (p + 1 < S) {
+        const double d = o - static_cast<double>(occ[i + step]);
+        rs += d * d;
+        ds += d;
+      }
+      if (p > 0) ds += o - static_cast<double>(occ[i - step]);
+    };
+    axis(c, 1);
+    axis(b, S);
+    axis(a, ss);
+    rb += o * (1.0 - o);
+    if (keep && !keep[i]) {
+      g[i] = 0.0f;
+      continue;
+    }
+    double s = 0.0;
+    for (int v = 0; v < V; ++v) s += static_cast<double>(dvox[static_cast<long long>(v) * n + i]);
+    g[i] = static_cast<float>(s + (ls * 2.0 * ds + lb * (1.0 - 2.0 * o)) * inv_n);
+  }
+  red[0][threadIdx.x] = rs;
+  red[1][threadIdx.x] = rb;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (threadIdx.x < w) {
+      red[0][threadIdx.x] += red[0][threadIdx.x + w];
+      red[1][threadIdx.x] += red[1][threadIdx.x + w];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    part[2 * blockIdx.x] = red[0][0];
+    part[2 * blockIdx.x + 1] = red[1][0];
+  }
+}
+
+__global__ void __launch_bounds__(256) voxel_fit_reg_kernel(const double* __restrict__ part, int nblocks, double* __restrict__ reg,
+                                                            double inv_n) {
+  __shared__ double red[2][256];
+  double rs = 0.0, rb = 0.0;
+  for (int k = threadIdx.x; k < nblocks; k += blockDim.x) {
+    rs += part[2 * k];
+    rb += part[2 * k + 1];
+  }
+  red[0][threadIdx.x] = rs;
+  red[1][threadIdx.x] = rb;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (threadIdx.x < w) {
+      red[0][threadIdx.x] += red[0][threadIdx.x + w];
+      red[1][threadIdx.x] += red[1][threadIdx.x + w];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    reg[0] = red[0][0] * inv_n;
+    reg[1] = red[1][0] * inv_n;
+  }
+}
+
+// blocks of voxel_fit_grad_kernel: a function of S alone, so the partial sums (and the result) do not depend on the device
+inline int voxel_fit_blocks(int S) {
+  const long long n = static_cast<long long>(S) * S * S;
+  const long long b = (n + 1023) / 1024;
+  return static_cast<int>(b < 1 ? 1 : (b > 1024 ? 1024 : b));
+}
+
 inline int grid_for(long long n, int block, int cap = 132 * 16) {
   long long g = (n + block - 1) / block;
   return static_cast<int>(g < 1 ? 1 : (g > cap ? cap : g));
@@ -543,6 +628,24 @@ extern "C" int rn_adam_step(float* param, const float* grad, float* m, float* v,
   if (!param || !grad || !m || !v || n < 0) return -1;
   if (n == 0) return 0;
   adam_kernel<<<grid_for(n, 256 * 4), 256, 0, static_cast<cudaStream_t>(stream)>>>(param, grad, m, v, n, lr_t, beta1, beta2, eps);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" long long rn_voxel_fit_grad_workspace(int S) {
+  if (S < 1 || S > 1024) return -1;
+  return 2LL * voxel_fit_blocks(S);
+}
+
+extern "C" int rn_voxel_fit_grad(const float* dvox, const float* occ, const unsigned char* keep, float* g, double* reg, double* work,
+                                 int V, int S, float lambda_smooth, float lambda_bin, void* stream) {
+  if (!dvox || !occ || !g || !reg || !work || V < 1 || S < 1 || S > 1024) return -1;
+  if (!(lambda_smooth >= 0.f) || !(lambda_bin >= 0.f) || isinf(lambda_smooth) || isinf(lambda_bin)) return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int nb = voxel_fit_blocks(S);
+  voxel_fit_grad_kernel<<<nb, 256, 0, st>>>(dvox, occ, keep, g, work, V, S, lambda_smooth, lambda_bin);
+  RN_COUNT_LAUNCH();
+  voxel_fit_reg_kernel<<<1, 256, 0, st>>>(work, nb, reg, 1.0 / (static_cast<double>(S) * S * S));
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }

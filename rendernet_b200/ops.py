@@ -5,6 +5,7 @@ CPU path.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass
 from typing import Optional, Sequence
 
@@ -1214,3 +1215,40 @@ def adam_step(param: torch.Tensor, grad: torch.Tensor, m: torch.Tensor, v: torch
             raise TypeError("adam_step: contiguous fp32 CUDA tensors of one size expected")
     check(lib.rn_adam_step(param.data_ptr(), grad.data_ptr(), m.data_ptr(), v.data_ptr(), param.numel(), float(lr_t), float(beta1),
                            float(beta2), float(eps), _stream()), "rn_adam_step")
+
+
+def voxel_fit_grad(dvox: torch.Tensor, occ: torch.Tensor, keep: Optional[torch.Tensor] = None, lambda_smooth: float = 0.0,
+                   lambda_bin: float = 0.0):
+    """Gradient of the shape fit's objective w.r.t. one shared occupancy grid (rn_voxel_fit_grad).  occ: fp32 CUDA tensor of S^3
+    elements ([S,S,S], [S,S,S,1] or flat); dvox: fp32 [V, ...] with S^3 elements per view (the per-view dL/dvoxels); keep: uint8
+    of S^3 elements (1 = not carved) or None.  Returns (g fp32 shaped like occ, reg float64 [2] = (R_s, R_b)), both on the device:
+    g = keep * (sum_v dvox[v] + lambda_smooth dR_s/docc + lambda_bin dR_b/docc).  Malformed input raises ValueError."""
+    for name, t in (("dvox", dvox), ("occ", occ), ("keep", keep)):
+        if t is not None and not isinstance(t, torch.Tensor):
+            raise ValueError(f"voxel_fit_grad: {name} must be a tensor, not {type(t).__name__}")
+    if dvox.dtype != torch.float32 or occ.dtype != torch.float32:
+        raise ValueError(f"voxel_fit_grad: dvox and occ must be float32, not {dvox.dtype} / {occ.dtype}")
+    n = occ.numel()
+    S = round(n ** (1.0 / 3.0)) if n > 0 else 0
+    if S < 1 or S ** 3 != n or S > 1024:
+        raise ValueError(f"voxel_fit_grad: occ {tuple(occ.shape)} does not hold a cubic grid")
+    if dvox.dim() < 1 or dvox.shape[0] < 1 or dvox.numel() != int(dvox.shape[0]) * n:
+        raise ValueError(f"voxel_fit_grad: dvox {tuple(dvox.shape)} is not [V, ...] with {n} elements per view")
+    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != n):
+        raise ValueError(f"voxel_fit_grad: keep must be uint8 with {n} elements, not {keep.dtype} {tuple(keep.shape)}")
+    for name, lam in (("lambda_smooth", lambda_smooth), ("lambda_bin", lambda_bin)):
+        if not (math.isfinite(float(lam)) and float(lam) >= 0.0):
+            raise ValueError(f"voxel_fit_grad: {name} must be a finite number >= 0, not {lam}")
+    devs = {t.device for t in (dvox, occ, keep) if t is not None}
+    if any(d.type != "cuda" for d in devs):
+        raise ValueError("voxel_fit_grad: dvox, occ and keep must be CUDA tensors")
+    if len(devs) != 1:
+        raise ValueError(f"voxel_fit_grad: tensors on different devices {sorted(map(str, devs))}")
+    dvox, occ = dvox.contiguous(), occ.contiguous()
+    keep = keep.contiguous() if keep is not None else None
+    g = torch.empty_like(occ)
+    reg = torch.empty(2, device=occ.device, dtype=torch.float64)
+    work = torch.empty(int(lib.rn_voxel_fit_grad_workspace(S)), device=occ.device, dtype=torch.float64)
+    check(lib.rn_voxel_fit_grad(dvox.data_ptr(), occ.data_ptr(), _ptr(keep), g.data_ptr(), reg.data_ptr(), work.data_ptr(),
+                                int(dvox.shape[0]), S, float(lambda_smooth), float(lambda_bin), _stream()), "rn_voxel_fit_grad")
+    return g, reg

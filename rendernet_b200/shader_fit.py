@@ -15,7 +15,8 @@ Objectives (`shader_fit_gradients`):
   * "mse" / "bce": the raw network output (RGB or greyscale) against the target, per item (rn_image_loss_grad_items; "bce" is
     the loss the shipped greyscale Shader was trained with, RenderNet_Shader.py:158-163).
 The image gradient runs back through the network and the resampler (backward.ShaderInputGradients) to dL/d(view_params); the
-light map is differentiated on the host in float64.  The voxels are held fixed: the Shader has no shape prior.
+light map is differentiated on the host in float64.  The voxels are held fixed here: the Shader has no shape prior, so fitting
+the shape takes several views and a silhouette hull (shape_fit.py).
 
 Search (`pose_search`, the reference's loop with `create_param_center`): five pose hypotheses at the corners and the centre of a
 60 x 30 degree (azimuth x elevation) window around the initial guess, light azimuths linspace(230, 320) degrees unless given;
@@ -78,13 +79,15 @@ def _target_on(target, shape, device) -> torch.Tensor:
 def shader_fit_gradients(ig, voxels, view_params, target, objective: str, light=None, light_col=PHONG_DEFAULTS["light_col"],
                          ambient: float = PHONG_DEFAULTS["ambient"], k_diffuse: float = PHONG_DEFAULTS["k_diffuse"],
                          background_white: bool = PHONG_DEFAULTS["background_white"],
-                         with_mask: bool = PHONG_DEFAULTS["with_mask"], want_dvox: bool = False):
+                         with_mask: bool = PHONG_DEFAULTS["with_mask"], want_dvox: bool = False, want_dpose: bool = True,
+                         dvox_on_device: bool = False):
     """Loss [B] (float64) and the gradients of sum_b loss[b] at (voxels, view_params[, light]).
 
     ig: a backward.ShaderInputGradients of the batch size.  objective "phong" (RGB network only; light [B,2] = (azimuth,
     elevation) radians, required), "mse" or "bce" (raw output; light must be None).  target: [B,512,512,C] image (NumPy or
-    tensor).  Returns (loss, {"pose": dL/dview_params [B,3], "light": dL/d(azimuth, elevation) [B,2] or None, "voxels":
-    dL/dvoxels [B,64,64,64,1] if want_dvox else None}), NumPy float64 except dL/dvoxels (float32)."""
+    tensor).  Returns (loss, {"pose": dL/dview_params [B,3] if want_dpose else None, "light": dL/d(azimuth, elevation) [B,2] or
+    None, "voxels": dL/dvoxels [B,64,64,64,1] if want_dvox else None}), NumPy float64 except dL/dvoxels (float32; a CUDA tensor
+    if dvox_on_device)."""
     check_objective(objective, ig.is_greyscale)
     B = ig.B
     if objective == "phong":
@@ -107,8 +110,8 @@ def shader_fit_gradients(ig, voxels, view_params, target, objective: str, light=
             dlight = np.einsum("bi,bij->bj", dl.double().cpu().numpy(), light_dir_jacobian(light))
         else:
             loss, dimg = ops.image_loss_grad_items(img, tgt, objective)
-    dvox, dpose = ig.backward(dimg, want_dvox=want_dvox, want_dpose=True)
-    return loss.cpu().numpy(), dict(pose=np.asarray(dpose, np.float64), light=dlight, voxels=dvox)
+    dvox, dpose = ig.backward(dimg, want_dvox=want_dvox, want_dpose=want_dpose, dvox_on_device=dvox_on_device)
+    return loss.cpu().numpy(), dict(pose=np.asarray(dpose, np.float64) if want_dpose else None, light=dlight, voxels=dvox)
 
 
 def _deg(x):
