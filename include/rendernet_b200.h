@@ -187,6 +187,20 @@ int rn_conv3d_banded_same(const void* x, const void* w_banded, const float* bias
                           int act, const void* residual, int residual_is_f32, void* out16, float* out32, int B,
                           int H, int W, int D, int Cin, int Cout, int sz, int fmt, const rn_tuning* tune, void* stream);
 
+/* The same 3^3 SAME stride-1 conv3d for Cin = Cout = 32 (res1, res_block_3d at RenderNet_Shader.py:45-64; tools/layer_util.py:60-88)
+ * as a depth-sliced kernel (rn_conv3d_sliced.cu): tiles of 8 x 8 pixels x 8 output depths, each input depth issued as
+ * N = 96 MMAs into the three output depths it feeds (no band zeros), the whole filter resident in shared memory.
+ * w_sliced from rn_pack_conv3d_sliced: [9 = (ky,kx)][96 = (2 - kz)*32 + co][32 = ci] 16-bit (9*96*32 elements per plane;
+ * RN_FMT_F16X2: the LO plane follows).  x: [B,H,W,D,32], residual / out: [B,H,W,D,32] (16-bit, residual optionally fp32);
+ * bias_full / alpha_full [D*32] as for rn_conv3d_banded_same; act RN none or PReLU; any B, H, W; D a multiple of 8.
+ * rn_conv3d_sliced_plan reports {stages, dynamic shared memory bytes, grid, tiles, filter bytes, stage bytes, smem limit}
+ * without touching a device. */
+int rn_pack_conv3d_sliced(const float* w, void* packed, int fmt, void* stream);
+int rn_conv3d_sliced_same(const void* x, const void* w_sliced, const float* bias_full, const float* alpha_full, int act,
+                          const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W, int D,
+                          int Cin, int Cout, int fmt, void* stream);
+int rn_conv3d_sliced_plan(int B, int H, int W, int D, int fmt, int* out, int n_out);
+
 /* slim.conv2d_transpose / layer_util.conv2d_transpose (layer_util.py:186; RenderNet_Shader.py:106-129),
  * SAME, out = in*stride.  w_packed holds the stride^2 phase filters back to back, as produced by
  * rn_pack_conv2d_transpose_weights: [phase = ay*s+ax][taps_of_phase][cout_pad][Cin]. */

@@ -67,6 +67,9 @@ SIGNATURES = {
     "rn_pack_conv3d_banded": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "rn_expand_channels": (_i, [_vp, _vp, _i, _i, _vp]),
     "rn_conv3d_banded_same": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _tp, _vp]),
+    "rn_pack_conv3d_sliced": (_i, [_vp, _vp, _i, _vp]),
+    "rn_conv3d_sliced_same": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "rn_conv3d_sliced_plan": (_i, [_i, _i, _i, _i, _i, C.POINTER(C.c_int), _i]),
     "rn_pack_conv2d_transpose_weights": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "rn_conv2d_transpose_same": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _tp, _vp]),
     "rn_pack_conv2d_transpose_s2_merged": (_i, [_vp, _vp, _i, _i, _i, _vp]),

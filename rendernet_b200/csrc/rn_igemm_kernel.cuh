@@ -16,10 +16,10 @@
 //   * Persistent: grid = #SMs, static round-robin tile schedule with N fastest so concurrently running
 //     CTAs share the same activation rows in L2.  The producer runs ahead into the next tile while the consumers drain.
 //
-// This header holds the device code and the per-variant launcher template `launch_ms`.  It is included only by
-// rn_igemm_inst.cu, which the Makefile compiles once per <BN, CL, MS, SPLIT, HALF> variant (one object each, so that
-// `make -j` spreads them over the cores); rn_igemm.cu (host side: validation, tile/pipeline sizing, tensor maps) declares
-// the template and dispatches to the instantiated variants.
+// This header holds the device code and the per-variant launcher template `launch_ms`.  It is included by rn_igemm_inst.cu,
+// which the Makefile compiles once per <BN, CL, MS, SPLIT, HALF> variant (one object each, so that `make -j` spreads them
+// over the cores), and by rn_conv3d_sliced.cu, whose kernel shares `epilogue_chunk`; rn_igemm.cu (host side: validation,
+// tile/pipeline sizing, tensor maps) declares the template and dispatches to the instantiated variants.
 #pragma once
 #include <atomic>
 #include <cstdio>

@@ -270,6 +270,19 @@ __global__ void pack_banded_kernel(const float* __restrict__ w, uint16_t* __rest
   }
 }
 
+// ------------------------------------------------------------------------------------------ sliced conv3d filter
+// Ws[plane][tap=(ky,kx)][r = zs*32 + co][ci] = w[ky][kx][kz = 2 - zs][ci][co]: one K-major [96 x 32] tile per (ky, kx) whose
+// three 32-row slices are the kz = 2, 1, 0 filters: slice zs is what input depth j contributes to output depth j - 2 + zs
+// (rn_conv3d_sliced.cu).  Cin = Cout = 32; the LO plane (fmt 2) follows the HI plane.
+__global__ void pack_sliced_kernel(const float* __restrict__ w, uint16_t* __restrict__ packed, int fmt, long long plane) {
+  const int total = 9 * 96 * 32;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int ci = i % 32, r = (i / 32) % 96, tap = i / (32 * 96);
+    const int kz = 2 - r / 32, co = r % 32;
+    store16(packed, i, w[((tap * 3 + kz) * 32 + ci) * 32 + co], fmt, plane);
+  }
+}
+
 __global__ void expand_channels_kernel(const float* __restrict__ v, float* __restrict__ out, int C, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = v[i % C];
@@ -1311,6 +1324,14 @@ extern "C" int rn_pack_conv3d_banded(const float* w, void* packed, int Cin, int 
   const long long total = 9LL * L.kblocks * 128 * 64;
   pack_banded_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       w, static_cast<uint16_t*>(packed), Cin, Cout, L, sz, fmt, total);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int rn_pack_conv3d_sliced(const float* w, void* packed, int fmt, void* stream) {
+  if (!w || !packed || fmt < 0 || fmt > 2) return -1;
+  pack_sliced_kernel<<<grid_for(9 * 96 * 32, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      w, static_cast<uint16_t*>(packed), fmt, 9 * 96 * 32);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }

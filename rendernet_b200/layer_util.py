@@ -399,6 +399,9 @@ def _deferred_conv(kind, x, w, b, stride):
     def _run(xt, act, alpha, residual, want32):
         banded = (kind == "conv3d" and USE_BANDED_CONV3D and tuple(w.shape[:3]) == (3, 3, 3)
                   and ops.BandedConv3d.eligible(int(w.shape[3]), int(w.shape[4]), int(xt.shape[3]), stride))
+        # 3^3 32 -> 32 (res1): the depth-sliced kernel with the filter resident in shared memory; chosen by shape alone, so
+        # every caller (render, input gradients, training and its pre-activation reruns, patches) runs the same kernel
+        sliced = banded and ops.SlicedConv3d.eligible(int(w.shape[3]), int(w.shape[4]), int(xt.shape[3]), stride)
         if kind == "conv3d" and stride != 1 and not banded:
             raise NotImplementedError("z-strided conv3d needs the depth-folded path")
         xfold = 1
@@ -413,6 +416,13 @@ def _deferred_conv(kind, x, w, b, stride):
         if kind == "conv2d":
             return ops.conv2d(xt, L, act=act, residual=residual, want16=want16, want32=want32, alpha=a)
         if kind == "conv3d":
+            if sliced:
+                Ls = _store().packed.get(("sliced", w._rn_name, _store().fmt))
+                if Ls is None:
+                    Ls = ops.SlicedConv3d(w, b, dtype=tf.COMPUTE_DTYPE, device=_store().device, fmt=_store().fmt)
+                    _store().packed[("sliced", w._rn_name, _store().fmt)] = Ls
+                return ops.conv3d_sliced(xt, Ls, act=act, residual=residual, alpha=a,
+                                         alpha_tag=getattr(alpha, "_rn_name", None), want16=want16, want32=want32)
             if banded:
                 Lb = _store().packed.get(("banded", w._rn_name, stride, _store().fmt))
                 if Lb is None:

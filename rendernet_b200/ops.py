@@ -346,6 +346,20 @@ class BandedConv3d:
         return f
 
 
+def _expanded_bias_alpha(L, a: int, alpha, alpha_tag, Do: int, device):
+    """Per-depth expansion [Do*Cout] of a depth-folded conv3d's bias and PReLU slope (slope None unless act is PReLU)."""
+    bias_full = L.expanded(L.bias, Do, "bias")
+    alpha_full = None
+    if a == ACT_PRELU:
+        if alpha_tag is not None:
+            alpha_full = L.expanded(alpha[:L.cout], Do, ("alpha", alpha_tag))
+        else:                      # untagged alpha: never cached (a freed tensor's address can be reused)
+            v = _cuda(alpha[:L.cout].to(device=device, dtype=torch.float32))
+            alpha_full = torch.empty(Do * L.cout, device=device, dtype=torch.float32)
+            check(lib.rn_expand_channels(v.data_ptr(), alpha_full.data_ptr(), L.cout, Do, _stream()), "rn_expand_channels")
+    return bias_full, alpha_full
+
+
 def conv3d_banded(x: torch.Tensor, L: BandedConv3d, act: Optional[str] = None,
                   residual: Optional[torch.Tensor] = None, alpha: Optional[torch.Tensor] = None, alpha_tag=None,
                   want16: bool = True, want32: bool = False, out16=None, out32=None, tune=None):
@@ -357,18 +371,61 @@ def conv3d_banded(x: torch.Tensor, L: BandedConv3d, act: Optional[str] = None,
     out16, out32 = _out_buffers((B, H, W, Do, L.cout), L.dtype, x.device, want16, want32, out16, out32, L.fmt)
     residual, res_f32 = _residual(residual, L.fmt)
     a = _ACT[act]
-    bias_full = L.expanded(L.bias, Do, "bias")
-    alpha_full = None
-    if a == ACT_PRELU:
-        if alpha_tag is not None:
-            alpha_full = L.expanded(alpha[:L.cout], Do, ("alpha", alpha_tag))
-        else:                      # untagged alpha: never cached (a freed tensor's address can be reused)
-            v = _cuda(alpha[:L.cout].to(device=x.device, dtype=torch.float32))
-            alpha_full = torch.empty(Do * L.cout, device=x.device, dtype=torch.float32)
-            check(lib.rn_expand_channels(v.data_ptr(), alpha_full.data_ptr(), L.cout, Do, _stream()), "rn_expand_channels")
+    bias_full, alpha_full = _expanded_bias_alpha(L, a, alpha, alpha_tag, Do, x.device)
     check(lib.rn_conv3d_banded_same(x.data_ptr(), L.w.data_ptr(), bias_full.data_ptr(), _ptr(alpha_full), a,
                                     _ptr(residual), res_f32, _ptr(out16), _ptr(out32), B, H, W, D, Cin, L.cout, L.sz,
                                     L.fmt, _tune(tune), _stream()), "rn_conv3d_banded_same")
+    return _ret(out16, out32, want16, want32, L.fmt)
+
+
+class SlicedConv3d(BandedConv3d):
+    """3^3 SAME stride-1 conv3d with Cin = Cout = 32 (the Shader's res1) through rn_conv3d_sliced_same: the same
+    depth-folded operands as BandedConv3d, the filter packed as nine [96 x 32] tiles (kz = 2, 1, 0 slices of each
+    (ky, kx)) that the kernel keeps in shared memory."""
+
+    TAP_ELEMS = 9 * 96 * 32            # 16-bit elements per plane of the packed filter
+
+    def __init__(self, w_tf: torch.Tensor, bias: Optional[torch.Tensor], dtype=torch.float16, device="cuda",
+                 fmt: Optional[int] = None):
+        w_tf = torch.as_tensor(w_tf, dtype=torch.float32).to(device).contiguous()
+        if tuple(w_tf.shape) != (3, 3, 3, 32, 32):
+            raise ValueError("the sliced conv3d is built for 3^3 filters with 32 input and 32 output channels")
+        self.cin, self.cout, self.sz = 32, 32, 1
+        self.dtype = dtype
+        self.fmt = fmt_of(dtype) if fmt is None else int(fmt)
+        self.w = _alloc16((self.TAP_ELEMS,), self.fmt, dtype, device)
+        check(lib.rn_pack_conv3d_sliced(w_tf.data_ptr(), self.w.data_ptr(), self.fmt, _stream()), "rn_pack_conv3d_sliced")
+        self.bias = (bias if bias is not None else torch.zeros(self.cout)).to(device=device, dtype=torch.float32)
+        self._full = {}
+
+    @staticmethod
+    def eligible(cin: int, cout: int, D: int, sz: int = 1) -> bool:
+        return cin == 32 and cout == 32 and sz == 1 and D >= 8 and D % 8 == 0
+
+    @staticmethod
+    def plan(B: int, H: int, W: int, D: int, fmt: int) -> dict:
+        """Launch plan of one call, computed on the host (no device needed)."""
+        out = (C.c_int * 7)()
+        check(lib.rn_conv3d_sliced_plan(B, H, W, D, fmt, out, 7), "rn_conv3d_sliced_plan")
+        return dict(zip(("stages", "smem_bytes", "grid", "tiles", "filter_bytes", "stage_bytes", "smem_limit"), list(out)))
+
+
+def conv3d_sliced(x: torch.Tensor, L: SlicedConv3d, act: Optional[str] = None,
+                  residual: Optional[torch.Tensor] = None, alpha: Optional[torch.Tensor] = None, alpha_tag=None,
+                  want16: bool = True, want32: bool = False, out16=None, out32=None):
+    """x [B,H,W,D,32] 16-bit -> [B,H,W,D,32] (D a multiple of 8); the arguments mean what they mean for conv3d_banded."""
+    x = _act_in(x, L.fmt, L.dtype)
+    B, H, W, D, Cin = x.shape
+    assert Cin == L.cin
+    out16, out32 = _out_buffers((B, H, W, D, L.cout), L.dtype, x.device, want16, want32, out16, out32, L.fmt)
+    residual, res_f32 = _residual(residual, L.fmt)
+    a = _ACT[act]
+    if a not in (ACT_NONE, ACT_PRELU):
+        raise ValueError("the sliced conv3d fuses no activation or PReLU only")
+    bias_full, alpha_full = _expanded_bias_alpha(L, a, alpha, alpha_tag, D, x.device)
+    check(lib.rn_conv3d_sliced_same(x.data_ptr(), L.w.data_ptr(), bias_full.data_ptr(), _ptr(alpha_full), a,
+                                    _ptr(residual), res_f32, _ptr(out16), _ptr(out32), B, H, W, D, Cin, L.cout,
+                                    L.fmt, _stream()), "rn_conv3d_sliced_same")
     return _ret(out16, out32, want16, want32, L.fmt)
 
 
