@@ -373,6 +373,19 @@ int rn_phong_recon_loss_grad(const float* albedo, const float* normal, const flo
 int rn_phong_composite_loss_grad(const float* img, const float* target, const float* light_dir, const float* light_col,
                                  float ambient, float k_diffuse, int background_white, int with_mask, double* loss, float* d_img,
                                  float* d_light_dir, int B, int H, int W, void* stream);
+/* Backward of rn_phong_shade for any loss: g_compos = dL/d(compos) [B,H,W,3] fp32 -> d_normal [B,H,W,3] (overwritten), d_albedo
+ * [B,H,W,3] = g_compos * shade (overwritten; written only when albedo is given, and may be NULL) and d_light_dir [B,3]
+ * (ACCUMULATED into: zero it first; may be NULL).  The other arguments are rn_phong_shade's, and each composite is differentiated
+ * through its own forward device function, recomputed in the same thread: RN_PHONG_TF through tf_phong_pixel (the light
+ * normalised by a division by |l|), RN_PHONG_NUMPY through phong_pixel (a multiply by 1 / |l|).  Albedo NULL: compos = shade.
+ * Conventions of the fused objectives rn_phong_recon_loss_grad / rn_phong_composite_loss_grad: max(x, 0) passes where x >= 0, a
+ * clip where lo <= x <= hi, the mask's derivative in double from the fp32 pixel.  At normal = (0.5, 0.5, 0.5) the direction is
+ * 0/0: the forward shades the pixel as unlit, only the mask term reaches d_normal and nothing reaches d_light_dir (finite for
+ * both composites).  One thread per pixel, blockIdx.y = item; d_light_dir takes one atomic per block and component. */
+int rn_phong_shade_backward(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
+                            float ambient, float k_diffuse, int composite, int background_white, int with_mask,
+                            const float* g_compos, float* d_normal, float* d_albedo, float* d_light_dir, int B, int H, int W,
+                            void* stream);
 long long rn_fully_connected_backward_workspace(int B, int K, int N);
 int rn_fully_connected_backward_data(const float* g, const float* w, float* work, float* dx, int B, int K, int N, void* stream);
 

@@ -115,6 +115,7 @@ SIGNATURES = {
     "rn_voxel_fit_grad": (_i, [_vp] * 6 + [_i, _i, _f, _f, _vp]),
     "rn_phong_composite": (_i, [_vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _i, _i, _i, _vp]),
     "rn_phong_shade": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "rn_phong_shade_backward": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
 }
 RN_PHONG_NUMPY, RN_PHONG_TF = 0, 1
 

@@ -61,7 +61,13 @@ def _key(t) -> int:
 
 def pose_matrix_jacobian_vjp(view_params: np.ndarray, dminv: np.ndarray, size: int = 64, new_size: int = 128) -> np.ndarray:
     """dL/d(view_params) [B,3] from dL/d(Minv[:, :3, :]) [B,3,4]: differentiates M = T(+new/2).S.R.T(-size/2), R = RotZ(el).RotY(az-pi/2)
-    (tools/resampling_voxel_grid.py:515-602) and the matrix inverse, in float64 on the host (a 3 -> 12 map per item)."""
+    (tools/resampling_voxel_grid.py:515-602) and the matrix inverse, in float64 on the host (a 3 -> 12 map per item).  Runs
+    under torch.enable_grad(), so it also works inside a torch.autograd.Function's backward (rendernet_b200.nn)."""
+    with torch.enable_grad():
+        return _pose_matrix_jacobian_vjp(view_params, dminv, size, new_size)
+
+
+def _pose_matrix_jacobian_vjp(view_params, dminv, size, new_size):
     vp = torch.tensor(np.asarray(view_params, np.float64), requires_grad=True)
     B = vp.shape[0]
     az = vp[:, 0] - math.pi * 0.5
@@ -131,8 +137,11 @@ class _InputGradients:
     and the reverse walk over the tape (`_reverse_walk`).  A subclass records the tape in `forward` and differentiates, in
     `_input_chain`, the fused resample + e_conv1 record that starts its network."""
 
+    # the attributes a recording consists of (_snapshot / _restore)
+    _RECORDING = ("tape",)
+
     def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str, size: int, new_size: int,
-                 loss_scale, seed: int, device: str):
+                 loss_scale, seed: int, device: str, store: Optional[tf.VariableStore] = None):
         if not torch.cuda.is_available():
             raise RuntimeError(f"{type(self).__name__} needs a CUDA device (no CPU fallback)")
         self.B, self.size, self.new_size = batch, size, new_size
@@ -141,14 +150,30 @@ class _InputGradients:
         self.overflow_retries = OVERFLOW_RETRIES
         self.last_loss_scale = None                        # the scale the last walk used
         self.device = torch.device(device)
-        self.store = tf.VariableStore(precision=precision, device=str(self.device) if self.device.index is not None else "cuda",
-                                      seed=seed)
+        if store is not None:                              # shared with gradient objects of other batch sizes: weights and
+            if store.precision != precision:               # packed filters exist once
+                raise ValueError(f"the shared store computes in {store.precision!r}, not {precision!r}")
+            self.store = store
+        else:
+            self.store = tf.VariableStore(precision=precision, device=str(self.device) if self.device.index is not None else "cuda",
+                                          seed=seed)
         if weights is not None:
             with tf.use_store(self.store):
                 tf.load_weight_dict(weights)
         self._dgrad_cache: Dict[object, object] = {}
         self.tape = None
         self.last_dgrid = None
+        self._fc_dx = False          # weight-gradient walk: also carry dL/d(texture vector) through the decoder's FC
+
+    def _snapshot(self) -> Dict[str, object]:
+        """What `backward` reads from the object: the tape, the inputs and the outputs of the last forward.  Holding it keeps
+        that recording alive across later forwards (one recording per torch.autograd node, rendernet_b200.nn)."""
+        return {k: getattr(self, k, None) for k in self._RECORDING}
+
+    def _restore(self, rec: Dict[str, object]):
+        """Make a recording taken by _snapshot the object's current one again."""
+        for k, v in rec.items():
+            setattr(self, k, v)
 
     # ------------------------------------------------------------------------------------------- packed gradient filters
     def _zeros(self, n):
@@ -347,7 +372,7 @@ class _InputGradients:
         fp32, so no 1/scale is applied.  The FC's data gradient -- dL/d(texture vector), an input of the network -- is skipped."""
         act = rec["act"]
         if want_weight_grads:
-            self._decoder_weight_step(rec, g, grads)
+            self._decoder_weight_step(rec, g, grads, want_dx=self._fc_dx)
             return
         if act == "prelu":
             alpha = rec["alpha"]
@@ -369,7 +394,7 @@ class _InputGradients:
         k = _key(rec["x"])
         grads[k] = grads[k] + dx if k in grads else dx
 
-    def _decoder_weight_step(self, rec, g, grads):
+    def _decoder_weight_step(self, rec, g, grads, want_dx: bool = False):
         alpha, w, b, x = rec["alpha"], rec["w"], rec["b"], rec["x"]
         if rec["act"] != "prelu" or isinstance(alpha, str) or b is None or rec["op"] not in ("fc", "conv_small"):
             raise NotImplementedError(f"no weight gradients for a decoder {rec['op']} record with act {rec['act']!r}")
@@ -377,7 +402,12 @@ class _InputGradients:
         z = rec["rerun"]()
         a_dev = self._alpha(alpha, int(rec["y"].shape[-1]))
         if rec["op"] == "fc":
-            _, wg[w._rn_name], wg[b._rn_name], wg[alpha._rn_name] = ops.fully_connected_param_grad(x, g, z, a_dev)
+            gz, wg[w._rn_name], wg[b._rn_name], wg[alpha._rn_name] = ops.fully_connected_param_grad(x, g, z, a_dev,
+                                                                                                     want_gz=want_dx)
+            if want_dx:                        # dL/d(texture vector) as well (input and weight gradients in one walk)
+                dx = ops.fully_connected_backward_data(gz, self._w32(w))
+                k = _key(x)
+                grads[k] = grads[k] + dx if k in grads else dx
             return
         g, wg[b._rn_name], wg[alpha._rn_name] = ops.prelu_grad_f32(g, z, a_dev)
         s = int(rec["stride"])
@@ -487,9 +517,12 @@ class ShaderInputGradients(_InputGradients):
     call (choose_loss_scale; an overflow is retried at a lower scale); a number fixes it (an overflow raises
     FloatingPointError)."""
 
+    _RECORDING = ("tape", "vox", "minv", "view_params", "img")
+
     def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str = "exact", is_greyscale: bool = False,
-                 size: int = 64, new_size: int = 128, loss_scale=None, seed: int = 0, device: str = "cuda"):
-        super().__init__(weights, batch, precision, size, new_size, loss_scale, seed, device)
+                 size: int = 64, new_size: int = 128, loss_scale=None, seed: int = 0, device: str = "cuda",
+                 store: Optional[tf.VariableStore] = None):
+        super().__init__(weights, batch, precision, size, new_size, loss_scale, seed, device, store)
         self.is_greyscale = is_greyscale
         self.img = None
 
@@ -587,13 +620,17 @@ class TextureInputGradients(_InputGradients):
     (seeded initialisers).  model="pretrained": Reconstruct_RenderNet_Face's texture_decoder_pretrained + RenderNet_pretrained
     (ReLU residual blocks), `weights` the npz-keyed dictionary those functions read.  `loss_scale` as in ShaderInputGradients."""
 
+    _RECORDING = ("tape", "vox", "minv", "view_params", "albedo", "normal", "tex_in", "tex3d")
+
     def __init__(self, weights: Optional[Dict[str, np.ndarray]], batch: int, precision: str = "exact", model: str = "texture",
-                 size: int = 64, new_size: int = 128, loss_scale=None, seed: int = 0, device: str = "cuda"):
+                 size: int = 64, new_size: int = 128, loss_scale=None, seed: int = 0, device: str = "cuda",
+                 store: Optional[tf.VariableStore] = None):
         if model not in ("texture", "pretrained"):
             raise ValueError(f"model must be 'texture' or 'pretrained', not {model!r}")
         if model == "pretrained" and weights is None:
             raise ValueError("model='pretrained' builds its variables from the npz-keyed weight dictionary: pass one")
-        super().__init__(weights if model == "texture" else None, batch, precision, size, new_size, loss_scale, seed, device)
+        super().__init__(weights if model == "texture" else None, batch, precision, size, new_size, loss_scale, seed, device,
+                         store)
         self.model = model
         self.weight_dict = weights if model == "pretrained" else None
         self.albedo = self.normal = None
@@ -649,6 +686,14 @@ class TextureInputGradients(_InputGradients):
         if want_weight_grads:
             raise NotImplementedError("TextureInputGradients differentiates the inputs only: the weight gradients of the "
                                       "Texture+Normal network come from training.TextureTrainer")
+        return self._walk_outputs(d_albedo, d_normal, want_dvox, want_dtex, want_dpose, False, dvox_on_device)
+
+    def _walk_outputs(self, d_albedo, d_normal, want_dvox: bool, want_dtex: bool, want_dpose: bool, want_weight_grads: bool,
+                      dvox_on_device: bool):
+        """backward's walk.  want_weight_grads (rendernet_b200.nn.TextureRenderer): the walk TextureTrainer.loss_and_gradients
+        runs, filling `self.weight_grads` {variable name: fp32 device tensor}, dL/d(texture volume) carried through the decoder
+        with its weight gradients -- together with the input gradients asked for (the decoder's FC then also yields dL/d(texture
+        vector))."""
         if self.tape is None:
             raise RuntimeError("call forward() first")
         dev = self.store.device
@@ -660,15 +705,18 @@ class TextureInputGradients(_InputGradients):
             if tuple(d.shape) != tuple(out.shape):
                 raise ValueError(f"output gradient shape {tuple(d.shape)} != output shape {tuple(out.shape)}")
             grads[_key(out)] = d.contiguous()
-        self._want = (want_dvox, want_dtex, want_dpose)
+        self._want = (want_dvox, want_dtex or want_weight_grads, want_dpose)
+        self._fc_dx = want_weight_grads and want_dtex
         out = {}
 
         def walk(shrink):
             self._dvox = self._dminv = None
             self._dtex_reached = False
             self.last_dgrid = None
+            if want_weight_grads:
+                self.weight_grads = {}
             g = dict(grads)
-            self._reverse_walk(g, False, True, shrink)
+            self._reverse_walk(g, want_weight_grads, True, shrink)
             dtex = None
             if want_dtex:
                 dtex = g.pop(_key(self.tex_in), None)
@@ -676,13 +724,19 @@ class TextureInputGradients(_InputGradients):
                     raise RuntimeError("dL/d(texture volume) was computed but never reached the texture vector: the tape "
                                        "lost the link between the resampler and the texture decoder")
             out["dtex"] = dtex
-            return self._dvox, dtex, self._dminv
+            # with weight gradients every path of the walk reaches e_conv1's filter gradient
+            first = next((w for n, w in self.weight_grads.items() if n.endswith("e_conv1/e_conv1/weights")), None) \
+                if want_weight_grads else None
+            return self._dvox, dtex, self._dminv, first
 
         out["dtex"] = self._dvox = self._dminv = self.last_dgrid = None
-        with torch.cuda.device(self.device), tf.use_store(self.store):
-            if grads and (want_dvox or want_dtex or want_dpose):
-                self._walk_checked(walk)
-            torch.cuda.synchronize()
+        try:
+            with torch.cuda.device(self.device), tf.use_store(self.store):
+                if grads and (want_dvox or want_dtex or want_dpose or want_weight_grads):
+                    self._walk_checked(walk)
+                torch.cuda.synchronize()
+        finally:
+            self._fc_dx = False
         dtex = out["dtex"]
         B, S = self.B, self.size
         dvox = dpose = None
@@ -727,8 +781,11 @@ class ShapeDecoderGradients(_InputGradients):
     Every layer is fp32 on the CUDA cores (rn_fully_connected, rn_conv3d_f32), whatever the Texture+Normal network's precision,
     so the object has no precision of its own.  `weight_dict`: the decoder's npz-keyed arrays (g_zP_g_gc1_weights, ...)."""
 
-    def __init__(self, weight_dict: Dict[str, np.ndarray], batch: int, device: str = "cuda"):
-        super().__init__(None, batch, "exact", 64, 128, 1.0, 0, device)          # fp32 walk: the scale is never applied
+    _RECORDING = ("tape", "latent", "vox")
+
+    def __init__(self, weight_dict: Dict[str, np.ndarray], batch: int, device: str = "cuda",
+                 store: Optional[tf.VariableStore] = None):
+        super().__init__(None, batch, "exact", 64, 128, 1.0, 0, device, store)    # fp32 walk: the scale is never applied
         self.weight_dict = weight_dict
         self.vox = None
 
@@ -746,8 +803,8 @@ class ShapeDecoderGradients(_InputGradients):
             self.store.tape = None
         return self.vox
 
-    def backward(self, dvox) -> np.ndarray:
-        """dvox: dL/dvoxels [B,64,64,64,1] -> dL/dlatent [B,200] fp32 (NumPy)."""
+    def backward(self, dvox, on_device: bool = False):
+        """dvox: dL/dvoxels [B,64,64,64,1] -> dL/dlatent [B,200] fp32 (NumPy; a CUDA tensor if on_device)."""
         if self.tape is None:
             raise RuntimeError("call forward() first")
         dev = self.store.device
@@ -760,5 +817,5 @@ class ShapeDecoderGradients(_InputGradients):
             dz = grads.pop(_key(self.latent), None)
             if dz is None:
                 raise RuntimeError("the shape decoder's tape lost the link between the voxels and the latent vector")
-            out = dz.cpu().numpy()
+            out = dz if on_device else dz.cpu().numpy()
         return out

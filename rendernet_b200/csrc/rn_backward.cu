@@ -608,6 +608,90 @@ __global__ void __launch_bounds__(256) phong_composite_loss_grad_kernel(const fl
   }
 }
 
+// ------------------------------------------------------------------------------------------ Phong composite, any loss
+// The vector-Jacobian product of rn_phong_shade (phong_shade_kernel, rn_ops.cu) for an upstream gradient g = dL/d(compos):
+//   compos_c = albedo_c shade_c (albedo NULL: compos = shade)  ->  d_albedo_c = g_c shade_c,  dL/d(shade_c) = g_c albedo_c
+// and dL/d(shade) through the composite's own pixel function: tf_phong_pixel_backward (TF) or phong_pixel_backward (NumPy), each
+// fed the terms its forward recorded in this thread, so the shading differentiated is rn_phong_shade's bit for bit.  dL/dL is
+// reduced over the block and mapped through the forward's normalisation of the light: (I - L L^T) / |l| with the TF composite's
+// division by |l|, or times the NumPy composite's reciprocal 1 / |l|; one atomic per block and component.  One thread per pixel,
+// blockIdx.y = batch item.
+template <bool TF>
+__global__ void __launch_bounds__(256) phong_shade_backward_kernel(const float* __restrict__ normal, const float* __restrict__ albedo,
+                                                                   const float* __restrict__ light_dir,
+                                                                   const float* __restrict__ light_col, float ambient,
+                                                                   float k_diffuse, int white, int with_mask,
+                                                                   const float* __restrict__ g_compos, float* __restrict__ d_normal,
+                                                                   float* __restrict__ d_albedo, float* __restrict__ d_light, int HW) {
+  __shared__ float red[8][3];
+  const int b = blockIdx.y;
+  const float l0 = __ldg(light_dir + 3 * b), l1 = __ldg(light_dir + 3 * b + 1), l2 = __ldg(light_dir + 3 * b + 2);
+  const float col[3] = {__ldg(light_col + 3 * b), __ldg(light_col + 3 * b + 1), __ldg(light_col + 3 * b + 2)};
+  float L[3], lscale;                                                 // the normalised light; 1/|l| (NumPy) or |l| (TF)
+  if constexpr (TF) {
+    lscale = sqrtf(l0 * l0 + l1 * l1 + l2 * l2);                      // as phong_shade_kernel normalises it
+    L[0] = l0 / lscale; L[1] = l1 / lscale; L[2] = l2 / lscale;
+  } else {
+    lscale = 1.0f / sqrtf(l0 * l0 + l1 * l1 + l2 * l2);               // as phong_pixel normalises it
+    L[0] = l0 * lscale; L[1] = l1 * lscale; L[2] = l2 * lscale;
+  }
+  float dl[3] = {0.f, 0.f, 0.f};
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < HW) {
+    const size_t o = (static_cast<size_t>(b) * HW + p) * 3;
+    const float n[3] = {normal[o], normal[o + 1], normal[o + 2]};
+    float s[3], ds[3], dn[3];
+    const float g[3] = {g_compos[o], g_compos[o + 1], g_compos[o + 2]};
+    if constexpr (TF) {
+      TfPhongTerms t;
+      tf_phong_pixel(n[0], n[1], n[2], L, col, ambient, k_diffuse, !white, with_mask, s, &t);
+      if (albedo != nullptr) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) ds[c] = g[c] * albedo[o + c];
+      } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) ds[c] = g[c];
+      }
+      tf_phong_pixel_backward(n, L, t, col, ambient, k_diffuse, !white, with_mask, ds, dn, dl);
+    } else {
+      PhongTerms t;
+      phong_pixel(n[0], n[1], n[2], l0, l1, l2, col, ambient, k_diffuse, white, with_mask, s, &t);
+      if (albedo != nullptr) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) ds[c] = g[c] * albedo[o + c];
+      } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) ds[c] = g[c];
+      }
+      phong_pixel_backward(n[0], n[1], n[2], t, col, ambient, k_diffuse, white, with_mask, ds, dn, dl);
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) d_normal[o + i] = dn[i];
+    if (albedo != nullptr && d_albedo != nullptr) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) d_albedo[o + c] = g[c] * s[c];
+    }
+  }
+  if (d_light == nullptr) return;                                     // the same in every thread: the barrier below stays whole
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    float v = dl[i];
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    if (lane == 0) red[wib][i] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float v[3] = {0.f, 0.f, 0.f};
+    for (int w = 0; w < 8; ++w)
+      for (int i = 0; i < 3; ++i) v[i] += red[w][i];
+    const float ldv = L[0] * v[0] + L[1] * v[1] + L[2] * v[2];       // d (l/|l|) = (dL - L (L.dL)) / |l|
+    for (int i = 0; i < 3; ++i)
+      atomicAdd(d_light + 3 * b + i, TF ? (v[i] - L[i] * ldv) / lscale : (v[i] - L[i] * ldv) * lscale);
+  }
+}
+
 }  // namespace rn
 
 using namespace rn;
@@ -760,6 +844,26 @@ extern "C" int rn_phong_composite_loss_grad(const float* img, const float* targe
   const dim3 grid((HW + 255) / 256, B);
   phong_composite_loss_grad_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       img, target, light_dir, light_col, ambient, k_diffuse, background_white, with_mask, loss, d_img, d_light_dir, HW);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int rn_phong_shade_backward(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
+                                       float ambient, float k_diffuse, int composite, int background_white, int with_mask,
+                                       const float* g_compos, float* d_normal, float* d_albedo, float* d_light_dir, int B, int H,
+                                       int W, void* stream) {
+  if (!normal || !light_dir || !light_col || !g_compos || !d_normal || B < 1 || H < 1 || W < 1) return -1;
+  if (composite != RN_PHONG_NUMPY && composite != RN_PHONG_TF) return -1;
+  if (B > 65535 || static_cast<long long>(H) * W > 0x7fffffffLL - 255) return -2;
+  const int HW = H * W;
+  const dim3 grid((HW + 255) / 256, B);
+  const int white = background_white != 0, mask = with_mask != 0;
+  if (composite == RN_PHONG_TF)
+    phong_shade_backward_kernel<true><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, g_compos, d_normal, d_albedo, d_light_dir, HW);
+  else
+    phong_shade_backward_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, g_compos, d_normal, d_albedo, d_light_dir, HW);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }

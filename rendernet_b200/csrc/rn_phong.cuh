@@ -2,7 +2,9 @@
 // np_phong_composite, RenderNet_demo.py:54-58), shared by the stand-alone kernel (rn_ops.cu), the fused epilogue of the
 // last up-conv (rn_igemm_kernel.cuh) and the Shader fit's loss kernel (rn_backward.cu) so that all three produce the same bits;
 // and one pixel of TensorFlow's composite
-// (tf_phong_pixel), which the stand-alone kernel renders for face reconstruction.
+// (tf_phong_pixel), which the stand-alone kernel renders for face reconstruction.  Next to each, its backward for an arbitrary
+// upstream gradient (phong_pixel_backward, tf_phong_pixel_backward), which rn_phong_shade_backward (rn_backward.cu) runs on the
+// terms its own forward call recorded.
 #pragma once
 #include <cstdint>
 
@@ -53,31 +55,131 @@ __device__ __forceinline__ void phong_pixel(float r, float g, float bl, float lx
 }
 __device__ __forceinline__ uint8_t phong_u8(float v) { return static_cast<uint8_t>(fminf(fmaxf(255.f * v, 0.f), 255.f)); }
 
+// Backward of one phong_pixel call for an arbitrary upstream gradient ds = dL/d(out) (rn_phong_shade_backward): di = dL/d(r,g,b)
+// and dl = dL/dL, L = l / |l| the normalised light (the caller maps it through (I - L L^T) / |l|).  t: the call's own terms.
+// Conventions of phong_composite_loss_grad_kernel: max(x, 0) passes where x >= 0, a clip where lo <= x <= hi; the mask's
+// derivative m (1 - m) 255 (+-a / |a|) runs in double from the fp32 pixel.  At img = (0.5, 0.5, 0.5) t.d is NaN, max(d, 0)
+// passes nothing, and only the mask term reaches di (dl stays 0); where |a| = 0 the mask term is 0.
+__device__ __forceinline__ void phong_pixel_backward(float r, float g, float bl, const PhongTerms& t, const float* col,
+                                                     float ambient, float k_diffuse, int white, int with_mask, const float* ds,
+                                                     float* di, float* dl) {
+  float dndl = 0.f, dm = 0.f;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float dx = (t.x[c] >= 0.f && t.x[c] <= 1.f) ? ds[c] : 0.f;              // clip(compos, 0, 1)
+    if (with_mask) dm += dx * (ambient + t.diff[c] - 1.f);
+    const float ddiff = with_mask ? dx * t.mask : dx;
+    const float dpre = (t.pre[c] >= 0.f && t.pre[c] <= 1.f) ? ddiff : 0.f;         // clip(diffuse, 0, 1)
+    dndl += dpre * k_diffuse * col[c];
+  }
+  const float dd = t.d >= 0.f ? dndl : 0.f;                                         // max(d, 0); false for a NaN d
+#pragma unroll
+  for (int i = 0; i < 3; ++i) di[i] = dl[i] = 0.f;
+  if (dd != 0.f) {
+    const float u[3] = {(r - 0.5f) * t.inv, (g - 0.5f) * t.inv, (bl - 0.5f) * t.inv};
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      di[i] = dd * (t.L[i] - t.d * u[i]) * t.inv;
+      dl[i] = dd * u[i];
+    }
+  }
+  if (with_mask && dm != 0.f) {
+    const double a[3] = {white ? 1.0 - r : static_cast<double>(r), white ? 1.0 - g : static_cast<double>(g),
+                         white ? 1.0 - bl : static_cast<double>(bl)};
+    const double nrm = sqrt(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]);
+    if (nrm > 0.0) {
+      const double md = 1.0 / (1.0 + exp(-(255.0 * nrm - (white ? 80.0 : 150.0))));
+      const double dsg = static_cast<double>(dm) * md * (1.0 - md) * (white ? -255.0 : 255.0) / nrm;
+#pragma unroll
+      for (int i = 0; i < 3; ++i) di[i] += static_cast<float>(dsg * a[i]);
+    }
+  }
+}
+
+// The intermediate values of one tf_phong_pixel call, for its backward (tf_phong_pixel_backward).
+struct TfPhongTerms {
+  float u[3];      // (n - 0.5) / |n - 0.5|
+  float vn;        // |n - 0.5|
+  float d;         // u . L, before max(., 0)
+  float m;         // the fp32 mask (1 without mask)
+  double md, nnd;  // the mask and |n| in double
+  float pre[3];    // k_d max(d, 0) col_c, before the clip to [0, 1]
+  float dif[3];    // the clipped diffuse term
+  float x[3];      // the composite, before the clip to [0, 1]
+};
+
 // TensorFlow's composite (tools/Phong_shading.py:24-113 tf_mask / tf_mask_white / tf_phong_shading / tf_phong_composite), the
 // shading Reconstruct_RenderNet_Face.py:372-378 multiplies the albedo by.  (n0,n1,n2) = normal map in [0,1]; L = the light
 // direction ALREADY normalised as l / |l| (division, not a reciprocal); col = light colour.  The operation order, the fp32
 // rounding points and the mask in double are those of the forward half of phong_recon_loss_grad_kernel (rn_backward.cu), so the
 // image this returns is the one the reconstruction loss measures, bit for bit.  Unlike phong_pixel: the normal is not clamped
-// away from |n - 0.5| = 0, the white mask is sigmoid(255 (sqrt 3 - |n|) - 80) and the black one sigmoid(255 |n| - 80).
+// away from |n - 0.5| = 0, the white mask is sigmoid(255 (sqrt 3 - |n|) - 80) and the black one sigmoid(255 |n| - 80).  If `t` is
+// not NULL it receives the intermediates the gradient needs (recorded, not recomputed).
 __device__ __forceinline__ void tf_phong_pixel(float n0, float n1, float n2, const float* L, const float* col, float ambient,
-                                               float k_diffuse, int black, int with_mask, float* out) {
+                                               float k_diffuse, int black, int with_mask, float* out, TfPhongTerms* t = nullptr) {
   const float v[3] = {n0 - 0.5f, n1 - 0.5f, n2 - 0.5f};
   const float vn = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
   const float u[3] = {v[0] / vn, v[1] / vn, v[2] / vn};
   const float d = u[0] * L[0] + u[1] * L[1] + u[2] * L[2];
   const float dmax = fmaxf(d, 0.f);
   float m = 1.f;
+  double md = 1.0, nnd = 1.0;
   if (with_mask) {
-    const double nnd = sqrt(static_cast<double>(n0) * n0 + static_cast<double>(n1) * n1 + static_cast<double>(n2) * n2);
+    nnd = sqrt(static_cast<double>(n0) * n0 + static_cast<double>(n1) * n1 + static_cast<double>(n2) * n2);
     const double s = black ? 255.0 * nnd - 80.0 : 255.0 * (1.7320508075688772 - nnd) - 80.0;
-    m = static_cast<float>(1.0 / (1.0 + exp(-s)));
+    md = 1.0 / (1.0 + exp(-s));
+    m = static_cast<float>(md);
+  }
+  if (t != nullptr) {
+    t->u[0] = u[0]; t->u[1] = u[1]; t->u[2] = u[2];
+    t->vn = vn; t->d = d; t->m = m; t->md = md; t->nnd = nnd;
   }
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     const float pre = k_diffuse * dmax * col[c];
     const float dif = fminf(fmaxf(pre, 0.f), 1.f);
     const float x = with_mask ? m * (ambient + dif) + (1.f - m) : ambient + dif;
+    if (t != nullptr) { t->pre[c] = pre; t->dif[c] = dif; t->x[c] = x; }
     out[c] = fminf(fmaxf(x, 0.f), 1.f);
+  }
+}
+
+// Backward of one tf_phong_pixel call for an arbitrary upstream gradient ds = dL/d(out) (rn_phong_shade_backward): dn = dL/dn
+// and dl = dL/dL (L already normalised; the caller maps dl through (I - L L^T) / |l|).  n: the pixel, t: the call's own terms.
+// The chain rule of phong_recon_loss_grad_kernel's TF-1 conventions (max(x, 0) passes where x >= 0, a clip where lo <= x <= hi,
+// d|x|/dx = x / |x|), the mask's derivative in double.  Unlike that kernel, the normal's term is skipped where nothing passes
+// max(d, 0): at n = (0.5, 0.5, 0.5) u = 0/0 and d are NaN, and dn gets the mask term alone, dl nothing.  At |n| = 0 the mask
+// term is 0.
+__device__ __forceinline__ void tf_phong_pixel_backward(const float* n, const float* L, const TfPhongTerms& t, const float* col,
+                                                        float ambient, float k_diffuse, int black, int with_mask, const float* ds,
+                                                        float* dn, float* dl) {
+  float ddmax = 0.f, dm = 0.f;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float dx = (t.x[c] >= 0.f && t.x[c] <= 1.f) ? ds[c] : 0.f;              // clip_by_value(compos, 0, 1)
+    const float ddif = with_mask ? dx * t.m : dx;
+    if (with_mask) dm += dx * (ambient + t.dif[c] - 1.f);
+    const float dpre = (t.pre[c] >= 0.f && t.pre[c] <= 1.f) ? ddif : 0.f;         // clip_by_value(diffuse, 0, 1)
+    ddmax += dpre * k_diffuse * col[c];
+  }
+  const float dd = t.d >= 0.f ? ddmax : 0.f;                                        // tf.maximum(d, 0); false for a NaN d
+#pragma unroll
+  for (int i = 0; i < 3; ++i) dn[i] = dl[i] = 0.f;
+  if (dd != 0.f) {
+    float du[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      du[i] = dd * L[i];
+      dl[i] = dd * t.u[i];
+    }
+    const float udu = t.u[0] * du[0] + t.u[1] * du[1] + t.u[2] * du[2];           // d (v/|v|) = (du - u (u.du)) / |v|
+#pragma unroll
+    for (int i = 0; i < 3; ++i) dn[i] = (du[i] - t.u[i] * udu) / t.vn;
+  }
+  if (with_mask && dm != 0.f && t.nnd > 0.0) {                                     // sigmoid, then d|n|/dn = n/|n|
+    const double dsg = static_cast<double>(dm) * t.md * (1.0 - t.md) * (black ? 255.0 : -255.0) / t.nnd;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) dn[i] += static_cast<float>(dsg * n[i]);
   }
 }
 

@@ -779,6 +779,34 @@ def phong_shade(normal: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambi
     return shade, (shade if alias else compos), u8
 
 
+def phong_shade_backward(normal: torch.Tensor, g_compos: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambient: float = 0.0,
+                         k_diffuse: float = 1.0, albedo: Optional[torch.Tensor] = None, composite: str = "tf",
+                         background_white: bool = True, with_mask: bool = True, want_light_grad: bool = True):
+    """Vector-Jacobian product of phong_shade's compos (rn_phong_shade_backward) for g_compos = dL/d(compos): the arguments
+    are phong_shade's.  normal, albedo (or None), g_compos: fp32 [B,H,W,3] CUDA tensors; light_dir, light_col: 1 or B rows of
+    3.  Returns (d_normal, d_albedo or None without an albedo, d_light_dir [B,3] per item or None)."""
+    if composite not in PHONG_COMPOSITES:
+        raise ValueError(f"composite must be one of {sorted(PHONG_COMPOSITES)}, not {composite!r}")
+    if len(normal.shape) != 4 or normal.shape[3] != 3:
+        raise ValueError(f"phong_shade_backward: normal map must be [B,H,W,3], not {tuple(normal.shape)}")
+    B, H, W, _ = normal.shape
+    for name, t in (("albedo", albedo), ("g_compos", g_compos)):
+        if t is not None and tuple(t.shape) != tuple(normal.shape):
+            raise ValueError(f"phong_shade_backward: {name} {tuple(t.shape)} and normal map {tuple(normal.shape)} differ in shape")
+    ld = _light_rows(light_dir, B, normal.device, "light_dir")
+    lc = _light_rows(light_col, B, normal.device, "light_col")
+    normal, g_compos = _cuda(normal, torch.float32), _cuda(g_compos, torch.float32)
+    albedo = None if albedo is None else _cuda(albedo, torch.float32)
+    d_normal = torch.empty_like(normal)
+    d_albedo = None if albedo is None else torch.empty_like(normal)
+    d_light = torch.zeros((B, 3), device=normal.device, dtype=torch.float32) if want_light_grad else None
+    check(lib.rn_phong_shade_backward(normal.data_ptr(), _ptr(albedo), ld.data_ptr(), lc.data_ptr(), float(ambient),
+                                      float(k_diffuse), PHONG_COMPOSITES[composite], 1 if background_white else 0,
+                                      1 if with_mask else 0, g_compos.data_ptr(), d_normal.data_ptr(), _ptr(d_albedo),
+                                      _ptr(d_light), B, H, W, _stream()), "rn_phong_shade_backward")
+    return d_normal, d_albedo, d_light
+
+
 def bias_act(x, bias: Optional[torch.Tensor], alpha: Optional[torch.Tensor], act: Optional[str],
              residual=None, want32: bool = False, fmt: int = 0):
     """y = act(x + bias[c]) + residual on a 16-bit channel-last tensor (rn_bias_act_16).  An fp32 `x` is first cast to
