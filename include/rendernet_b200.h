@@ -404,6 +404,22 @@ int rn_conv3d_f32(const float* x, const float* w, const float* bias, float* out,
 /* fp32 activation derivative from the activation's OUTPUT y (n elements): act RN_ACT_ELU -> TF-1 EluGrad, y < 0 ? g * (y + 1) : g;
  * RN_ACT_SIGMOID -> SigmoidGrad, g * y * (1 - y) (rn_sigmoid_backward writes 16-bit only). */
 int rn_act_backward_f32(const float* g, const float* y, float* out, long long n, int act, void* stream);
+/* Weight and bias gradients of rn_conv3d_f32's layers, for fine-tuning the shape decoder (decoder_3d_pretrained(trainable=True),
+ * :31-75, whose conv3d_transpose layers pass `trainable` to their variables; replaces the filter and bias gradients that
+ * tf.gradients computes for them).  x fp32 [B,H,W,D,Cin] (the layer's input), gz = dL/d(pre-activation) fp32 [B,Ho,Wo,Do,Cout]
+ * (the layer's output grid: Ho = sH transposed, ceil(H/s) forward; anything else rc -2) ->
+ *   transposed = 1:  dw[kidx][co][ci] = sum over b and output voxels o of gz[b,o,co] x[b, i(o, k), ci]   [4,4,4,Cout,Cin]
+ *   transposed = 0:  dw[kidx][ci][co], the same sums                                                         [4,4,4,Cin,Cout]
+ *   db[co] = sum over b, o of gz[b,o,co]
+ * (SAME padding: taps that fall outside the input grid contribute zero), both overwritten.  The geometry rn_conv3d_f32 accepts:
+ * k = 4, B <= 32, 1..512 channels (rc -1 / -2).  A stride-2 transposed conv runs as its 8 output phases, each a GEMM over the
+ * phase's voxels (M = 8 taps x Cin, N = Cout) writing its own 8 taps of dw; K is split over CTAs.  Transposed stride 1 with
+ * Cin = 16, Cout = 1 (g_conv5) and a grid divisible by 4 x 4 x 16 runs a direct kernel.  `work` must hold
+ * rn_conv3d_f32_weight_grad_workspace(...) floats (always > 0; NULL: rc -4): the K slices' partial sums, added in a fixed order
+ * by a second kernel, which also sums db.  No float atomics: reproducible bit for bit. */
+long long rn_conv3d_f32_weight_grad_workspace(int B, int H, int W, int D, int Cin, int Cout, int stride, int transposed);
+int rn_conv3d_f32_weight_grad(const float* x, const float* gz, float* dw, float* db, float* work, int B, int H, int W, int D,
+                              int Cin, int Ho, int Wo, int Do, int Cout, int k, int stride, int transposed, void* stream);
 
 /* ---- backward pass, stage 2: weight gradients (training step, RenderNet_Shader.py:159-167) -------------------------------
  * dW of a stride-1 SAME conv2d (slim.conv2d / layer_util.conv2d, tools/layer_util.py:147-184) on the tensor cores:
@@ -440,7 +456,9 @@ int rn_prelu_alpha_grad(const void* g, const void* z, float* dalpha, long long n
  *   dw[k][n] = sum_b x[b][k] gz[b][n]               (TF layout [K,N])
  *   db[n]    = sum_b gz[b][n],   dalpha[n] = sum_{b: z<0} gy[b][n] z[b][n]
  * all overwritten.  B <= 32 (rc -2), N % 4 == 0 and 16-byte aligned rows (rc -3).  Sums over b in a fixed order, no atomics:
- * reproducible bit for bit. */
+ * reproducible bit for bit.  z == alpha == dalpha == NULL: an FC without activation (the shape decoder's g_gc1 = fully_connected
+ * with no activation, Reconstruct_RenderNet_Face.py:47-50), gz = gy: dw = x^T gy, db = sum_b gy; only some of the three NULL:
+ * rc -1. */
 int rn_fully_connected_param_grad(const float* x, const float* gy, const float* z, const float* alpha, float* gz, float* dw,
                                   float* db, float* dalpha, int B, int K, int N, void* stream);
 /* fp32 PReLU derivative with the bias and slope gradients of a thin texture-decoder conv (e_tex_conv0..2,

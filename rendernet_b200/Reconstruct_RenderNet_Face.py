@@ -37,11 +37,33 @@ from .layer_util import (conv2d, conv2d_transpose, conv3d, conv3d_transpose, ful
 from .tfcompat import realize
 
 
+# The shape decoder's 12 variables: (TF name, npz key = the TF name with '/' -> '_', shape or None where the array decides it --
+# the FC's width, as in the reference).  nn.ShapeDecoder's parameters are keyed by the TF name, its decoder_weight_dict() by the
+# npz key.
+DECODER_VARIABLES = (
+    ("g_zP/g_gc1/weights", "g_zP_g_gc1_weights", None), ("g_zP/g_gc1/biases", "g_zP_g_gc1_biases", None),
+    ("g_conv1/g_conv1/weights", "g_conv1_g_conv1_weights", (4, 4, 4, 128, 256)),
+    ("g_conv1/g_conv1/biases", "g_conv1_g_conv1_biases", (128,)),
+    ("g_conv2/g_conv2/weights", "g_conv2_g_conv2_weights", (4, 4, 4, 64, 128)),
+    ("g_conv2/g_conv2/biases", "g_conv2_g_conv2_biases", (64,)),
+    ("g_conv3/g_conv3/weights", "g_conv3_g_conv3_weights", (4, 4, 4, 32, 64)),
+    ("g_conv3/g_conv3/biases", "g_conv3_g_conv3_biases", (32,)),
+    ("g_conv4/g_conv4/weights", "g_conv4_g_conv4_weights", (4, 4, 4, 16, 32)),
+    ("g_conv4/g_conv4/biases", "g_conv4_g_conv4_biases", (16,)),
+    ("g_conv5/weights", "g_conv5_weights", (4, 4, 4, 1, 16)), ("g_conv5/biases", "g_conv5_biases", (1,)),
+)
+
+
 def decoder_3d_pretrained(z_in, weight_dict, trainable=False):
     """:31-75: latent [B,200] -> voxels [B,64,64,64,1] fp32 on the device: FC 200 -> 4^3 x 256, then conv3d_transpose k4 s2 + ELU
     down to 64^3 x 16 and conv3d_transpose k4 s1 + sigmoid.  Variable scopes and npz keys are the reference's ("g_zP_g_gc1_weights",
-    "g_conv1_g_conv1_biases", ..., "g_conv5_weights"); a missing key raises KeyError.  As in texture_decoder_pretrained, the FC's
-    width comes from its array."""
+    "g_conv1_g_conv1_biases", ..., "g_conv5_weights"; DECODER_VARIABLES); a missing key raises KeyError.  As in
+    texture_decoder_pretrained, the FC's width comes from its array.
+
+    `trainable` (the reference's flag "used in fine-tuning") is accepted and changes nothing here: the variables are always the
+    current store's fp32 masters (an existing variable wins over the array, like a restored checkpoint), and their gradients come
+    from the reverse walk over the recorded layers -- backward.ShapeDecoderGradients.backward(want_weight_grads=True), or
+    nn.ShapeDecoder(trainable=True) under torch autograd."""
     wd = weight_dict
     batch_size = z_in.shape[0]
     with tf.variable_scope('g_zP'):

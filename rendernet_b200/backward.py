@@ -31,7 +31,8 @@ to dL/d(texture vector).
 The face-reconstruction shape decoder (ShapeDecoderGradients, Reconstruct_RenderNet_Face.decoder_3d_pretrained) is walked the same
 way, in fp32: ELU / sigmoid derivatives from the stored outputs (rn_act_backward_f32), each conv3d_transpose's data gradient a
 conv3d on the same filter array (rn_conv3d_f32), the FC's rn_fully_connected_backward_data, down to dL/dlatent.  The voxel grid is
-the seam between it and TextureInputGradients; dL/dvoxels can stay on the device between the two.
+the seam between it and TextureInputGradients; dL/dvoxels can stay on the device between the two.  With want_weight_grads the same
+walk also gives the decoder's 12 parameter gradients (rn_conv3d_f32_weight_grad, rn_fully_connected_param_grad): fine-tuning.
 
 Gradients travel in the activations' 16-bit format (fp16, or fp16 hi/lo pairs in the exact mode) with a loss scale to keep
 them inside fp16's range; they are un-scaled when they leave the tensor-core part (fp32 from there on).  By default the scale
@@ -366,10 +367,13 @@ class _InputGradients:
         is the forward conv on it (same stride) -- rn_conv3d_small for the thin layers, rn_conv3d_f32 for the wide ones -- and
         the gradient of fully_connected is rn_fully_connected_backward_data.
 
-        want_weight_grads (Texture+Normal training, PReLU layers only): the pre-activation (kept on the tape, or re-run) gives
+        want_weight_grads (Texture+Normal training, PReLU layers): the pre-activation (kept on the tape, or re-run) gives
         dL/dz, db and dalpha in one pass (rn_prelu_grad_f32; the FC's rn_fully_connected_param_grad, which also gives dW), the
         filter gradient comes from the thin correlation kernel (fp32 operands).  The gradients reaching the decoder are unscaled
-        fp32, so no 1/scale is applied.  The FC's data gradient -- dL/d(texture vector), an input of the network -- is skipped."""
+        fp32, so no 1/scale is applied.  The FC's data gradient -- dL/d(texture vector), an input of the network -- is skipped
+        unless `_fc_dx` asks for it.  Shape decoder (fine-tuning): a conv_f32 layer's dL/dz from the stored output as above, dW and
+        db from rn_conv3d_f32_weight_grad, the data gradient as without weight gradients; the FC without activation gives dW and db
+        from rn_fully_connected_param_grad with gz = gy."""
         act = rec["act"]
         if want_weight_grads:
             self._decoder_weight_step(rec, g, grads, want_dx=self._fc_dx)
@@ -396,6 +400,12 @@ class _InputGradients:
 
     def _decoder_weight_step(self, rec, g, grads, want_dx: bool = False):
         alpha, w, b, x = rec["alpha"], rec["w"], rec["b"], rec["x"]
+        if rec["op"] == "conv_f32" and rec["act"] in ("elu", "sigmoid", None):
+            self._f32_conv_weight_step(rec, g, grads)
+            return
+        if rec["op"] == "fc" and rec["act"] is None:
+            self._fc_weight_step(rec, g, grads, want_dx)
+            return
         if rec["act"] != "prelu" or isinstance(alpha, str) or b is None or rec["op"] not in ("fc", "conv_small"):
             raise NotImplementedError(f"no weight gradients for a decoder {rec['op']} record with act {rec['act']!r}")
         wg = self.weight_grads
@@ -424,6 +434,32 @@ class _InputGradients:
         dx = ops.conv3d_small(g, self._w32(w), None, None, s, not rec["transposed"], want32=True)
         k = _key(x)
         grads[k] = grads[k] + dx if k in grads else dx
+
+    def _f32_conv_weight_step(self, rec, g, grads):
+        """A shape-decoder conv (rn_conv3d_f32, + bias, ELU / sigmoid / none): dL/dz from the stored output, dW and db in one
+        launch pair, then the data gradient exactly as the walk without weight gradients computes it."""
+        w, b, x, s = rec["w"], rec["b"], rec["x"], int(rec["stride"])
+        gz = ops.act_backward_f32(g, rec["y"], rec["act"]) if rec["act"] is not None else g
+        dw, db = ops.conv3d_f32_weight_grad(x, gz, s, rec["transposed"])
+        self.weight_grads[w._rn_name] = dw
+        if b is not None:
+            self.weight_grads[b._rn_name] = db
+        dx = ops.conv3d_f32(gz, self._w32(w), None, s, not rec["transposed"])
+        k = _key(x)
+        grads[k] = grads[k] + dx if k in grads else dx
+
+    def _fc_weight_step(self, rec, g, grads, want_dx: bool):
+        """An FC without activation (the shape decoder's g_gc1): dW = x^T g and db = sum_b g, and dL/dx = g W^T only if
+        want_dx."""
+        w, b, x = rec["w"], rec["b"], rec["x"]
+        _, dw, db, _ = ops.fully_connected_param_grad(x, g, None, None)
+        self.weight_grads[w._rn_name] = dw
+        if b is not None:
+            self.weight_grads[b._rn_name] = db
+        if want_dx:
+            dx = ops.fully_connected_backward_data(g, self._w32(w))
+            k = _key(x)
+            grads[k] = grads[k] + dx if k in grads else dx
 
     def _data_grad_of(self, rec, g, acc=None):
         """dL/dx of one recorded convolution layer from g = dL/d(its pre-activation) (16-bit, carrying the loss scale); `acc`, a
@@ -777,6 +813,7 @@ class ShapeDecoderGradients(_InputGradients):
         sdg = ShapeDecoderGradients(weight_dict_decoder, batch=5)
         vox = sdg.forward(latent)                 # [B,64,64,64,1] fp32 on the device (tape recorded)
         dlatent = sdg.backward(dvox)              # [B,200] fp32 (NumPy); dvox NumPy or a CUDA tensor
+        dlatent = sdg.backward(dvox, want_weight_grads=True)   # ... and sdg.weight_grads {tf name: dL/dvariable} (fine-tuning)
 
     Every layer is fp32 on the CUDA cores (rn_fully_connected, rn_conv3d_f32), whatever the Texture+Normal network's precision,
     so the object has no precision of its own.  `weight_dict`: the decoder's npz-keyed arrays (g_zP_g_gc1_weights, ...)."""
@@ -803,19 +840,33 @@ class ShapeDecoderGradients(_InputGradients):
             self.store.tape = None
         return self.vox
 
-    def backward(self, dvox, on_device: bool = False):
-        """dvox: dL/dvoxels [B,64,64,64,1] -> dL/dlatent [B,200] fp32 (NumPy; a CUDA tensor if on_device)."""
+    def backward(self, dvox, on_device: bool = False, want_weight_grads: bool = False, want_dlatent: bool = True):
+        """dvox: dL/dvoxels [B,64,64,64,1] -> dL/dlatent [B,200] fp32 (NumPy; a CUDA tensor if on_device), or None without
+        want_dlatent.  want_weight_grads: the same walk also fills `self.weight_grads` {tf name: fp32 device tensor in the
+        variable's layout} for the decoder's 12 variables (g_zP/g_gc1/weights, g_zP/g_gc1/biases, g_conv1/g_conv1/weights, ...,
+        g_conv5/biases); dL/dlatent is bit for bit the one the walk without weight gradients gives.  Without want_dlatent the FC's
+        data gradient is skipped."""
         if self.tape is None:
             raise RuntimeError("call forward() first")
+        if not (want_dlatent or want_weight_grads):
+            raise ValueError("nothing to compute: want_dlatent and want_weight_grads are both False")
         dev = self.store.device
         d = torch.as_tensor(np.asarray(dvox, np.float32) if not isinstance(dvox, torch.Tensor) else dvox).to(dev).float()
         if tuple(d.shape) != tuple(self.vox.shape):
             raise ValueError(f"dvox shape {tuple(d.shape)} != voxel shape {tuple(self.vox.shape)}")
         grads = {_key(self.vox): d.contiguous()}
-        with torch.cuda.device(self.device), tf.use_store(self.store):
-            self._reverse_walk(grads, False, True)
-            dz = grads.pop(_key(self.latent), None)
-            if dz is None:
-                raise RuntimeError("the shape decoder's tape lost the link between the voxels and the latent vector")
-            out = dz if on_device else dz.cpu().numpy()
+        if want_weight_grads:
+            self.weight_grads = {}
+        self._fc_dx = want_dlatent
+        try:
+            with torch.cuda.device(self.device), tf.use_store(self.store):
+                self._reverse_walk(grads, want_weight_grads, True)
+                dz = grads.pop(_key(self.latent), None)
+                if not want_dlatent:
+                    return None
+                if dz is None:
+                    raise RuntimeError("the shape decoder's tape lost the link between the voxels and the latent vector")
+                out = dz if on_device else dz.cpu().numpy()
+        finally:
+            self._fc_dx = False
         return out

@@ -199,7 +199,8 @@ __global__ void __launch_bounds__(256) prelu_alpha_grad_kernel(const void* __res
 // gy and z.  A thread owns four adjacent columns: gz = gy * (z > 0 ? 1 : alpha) of all BT (>= B, zero padded) rows stays in
 // registers, and dW[k][n..n+3] = sum_b x[b][k] gz[b][n..n+3] is one float4 store per k, x read as a broadcast from shared
 // memory.  blockIdx.x splits K (the CTAs of one column block run side by side and share gy / z in L2); only the K part 0
-// writes gz, db and dalpha.  Every sum runs over b in a fixed order: the result is reproducible bit for bit.
+// writes gz, db and dalpha.  Every sum runs over b in a fixed order: the result is reproducible bit for bit.  z == NULL: an FC
+// without activation (the shape decoder's g_gc1), gz = gy, no slope and no dalpha.
 template <int BT>
 __global__ void __launch_bounds__(128) fc_param_grad_kernel(const float* __restrict__ x, const float* __restrict__ gy,
                                                             const float* __restrict__ z, const float* __restrict__ alpha,
@@ -215,7 +216,8 @@ __global__ void __launch_bounds__(128) fc_param_grad_kernel(const float* __restr
   __syncthreads();
   const long long n = (static_cast<long long>(blockIdx.y) * blockDim.x + threadIdx.x) * 4;
   if (n >= N) return;
-  const float4 a = *reinterpret_cast<const float4*>(alpha + n);
+  const bool ident = z == nullptr;
+  const float4 a = ident ? make_float4(1.f, 1.f, 1.f, 1.f) : *reinterpret_cast<const float4*>(alpha + n);
   const bool first = blockIdx.x == 0;
   float4 g[BT];
   float4 sb = make_float4(0.f, 0.f, 0.f, 0.f), sa = sb;
@@ -224,7 +226,8 @@ __global__ void __launch_bounds__(128) fc_param_grad_kernel(const float* __restr
     g[b] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (b < B) {
       const long long o = static_cast<long long>(b) * N + n;
-      const float4 gv = *reinterpret_cast<const float4*>(gy + o), zv = *reinterpret_cast<const float4*>(z + o);
+      const float4 gv = *reinterpret_cast<const float4*>(gy + o);
+      const float4 zv = ident ? make_float4(1.f, 1.f, 1.f, 1.f) : *reinterpret_cast<const float4*>(z + o);
       g[b] = make_float4(zv.x > 0.f ? gv.x : gv.x * a.x, zv.y > 0.f ? gv.y : gv.y * a.y, zv.z > 0.f ? gv.z : gv.z * a.z,
                          zv.w > 0.f ? gv.w : gv.w * a.w);
       if (first) {
@@ -239,7 +242,7 @@ __global__ void __launch_bounds__(128) fc_param_grad_kernel(const float* __restr
   }
   if (first) {
     *reinterpret_cast<float4*>(db + n) = sb;
-    *reinterpret_cast<float4*>(dalpha + n) = sa;
+    if (dalpha) *reinterpret_cast<float4*>(dalpha + n) = sa;
   }
   for (int k = 0; k < kn; ++k) {
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -543,7 +546,9 @@ extern "C" int rn_prelu_alpha_grad(const void* g, const void* z, float* dalpha, 
 
 extern "C" int rn_fully_connected_param_grad(const float* x, const float* gy, const float* z, const float* alpha, float* gz,
                                              float* dw, float* db, float* dalpha, int B, int K, int N, void* stream) {
-  if (!x || !gy || !z || !alpha || !dw || !db || !dalpha || B < 1 || K < 1 || N < 1) return -1;
+  const bool ident = !z && !alpha && !dalpha;                                   // FC without activation: gz = gy
+  if (!x || !gy || !dw || !db || B < 1 || K < 1 || N < 1) return -1;
+  if (!ident && (!z || !alpha || !dalpha)) return -1;
   if (B > 32) return -2;
   if (N % 4 != 0) return -3;
   for (const void* q : {static_cast<const void*>(gy), static_cast<const void*>(z), static_cast<const void*>(alpha),

@@ -29,7 +29,11 @@ Semantics:
     the tape never refers back to the node.  Double backward is not supported.
   * The loss scale of the 16-bit walk is chosen per call as in the gradient objects; an overflow that survives the retries
     raises FloatingPointError out of backward().
-  * Dropout is never applied (train() does not turn it on); the pretrained models and the shape decoder are constants.
+  * Dropout is never applied (train() does not turn it on); the pretrained Texture+Normal model is a constant.
+  * ShapeDecoder(weight_dict_decoder, trainable=True) fine-tunes the face-reconstruction shape decoder: its 12 variables
+    (g_zP/g_gc1/weights ... g_conv5/biases) are Parameters under the same rules, their gradients come from
+    ShapeDecoderGradients' walk (rn_conv3d_f32_weight_grad, rn_fully_connected_param_grad), and decoder_weight_dict() returns
+    them under their npz keys, the dictionary ShapeDecoderGradients and FaceReconstruction take.
 """
 from __future__ import annotations
 
@@ -367,7 +371,7 @@ class TextureRenderer(_Renderer):
 # ----------------------------------------------------------------------------------------------- shape decoder
 class _ShapeDecoderFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, module, mode, latent):
+    def forward(ctx, module, mode, latent, *params):
         from .Reconstruct_RenderNet_Face import decoder_3d_pretrained
         B = latent.shape[0]
         sdg = module._object(B)
@@ -378,6 +382,7 @@ class _ShapeDecoderFn(torch.autograd.Function):
         _release(sdg)
         if mode:
             ctx.module, ctx.B = module, B
+            ctx.versions = [(p, p._version) for p in params]
             ctx.save_for_backward(latent, vox)
         return vox
 
@@ -385,36 +390,69 @@ class _ShapeDecoderFn(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, dvox):
         latent, _ = ctx.saved_tensors
+        _check_versions(ctx)
+        need = ctx.needs_input_grad
+        want_dlatent, want_w = need[2], any(need[3:])
         sdg = ctx.module._object(ctx.B)
         sdg._restore(_take_recording(ctx))
         try:
-            dz = sdg.backward(dvox, on_device=True)
+            dz = sdg.backward(dvox, on_device=True, want_weight_grads=want_w, want_dlatent=want_dlatent)
+            wg = sdg.weight_grads if want_w else {}
         finally:
             _release(sdg)
-        return None, None, dz.to(device=latent.device, dtype=latent.dtype).reshape(latent.shape)
+        gz = dz.to(device=latent.device, dtype=latent.dtype).reshape(latent.shape) if want_dlatent else None
+        return (None, None, gz) + tuple(wg[p._rn_name] if n else None for (p, _), n in zip(ctx.versions, need[3:]))
+
+
+def _check_decoder_weights(weight_dict_decoder) -> None:
+    """The decoder's 12 npz-keyed arrays, with the shapes decoder_3d_pretrained builds from them (checked on the host)."""
+    from .Reconstruct_RenderNet_Face import DECODER_VARIABLES
+    if not hasattr(weight_dict_decoder, "keys") or not hasattr(weight_dict_decoder, "__getitem__"):
+        raise TypeError(f"weight_dict_decoder must be a mapping of npz keys to arrays, not {type(weight_dict_decoder).__name__}")
+    missing = [k for _, k, _ in DECODER_VARIABLES if k not in weight_dict_decoder]
+    if missing:
+        raise KeyError(f"weight_dict_decoder lacks {missing}")
+    for _, k, shape in DECODER_VARIABLES:
+        got = tuple(np.shape(weight_dict_decoder[k]))
+        if shape is not None and got != shape:
+            raise ValueError(f"weight_dict_decoder[{k!r}] has shape {got}, not {shape}")
 
 
 class ShapeDecoder(_Renderer):
     """The face-reconstruction shape decoder (Reconstruct_RenderNet_Face.decoder_3d_pretrained) as an autograd layer:
     forward(latent [B,200]) -> voxels [B,64,64,64,1] fp32 on the device; dL/dlatent from ShapeDecoderGradients on the device.
-    Its weights (the npz-keyed `weight_dict_decoder`) are constants, as in the reference."""
+    `weight_dict_decoder`: the decoder's 12 npz-keyed arrays (g_zP_g_gc1_weights, ..., g_conv5_biases).  trainable=False: they
+    are constants, as in the reference's reconstruction.  trainable=True (fine-tuning, decoder_3d_pretrained(trainable=True)):
+    they are the 12 Parameters `params.<tf name>`, and the walk that gives dL/dlatent also gives their gradients.
+    decoder_weight_dict() returns the current values under their npz keys."""
 
-    def __init__(self, weight_dict_decoder: Dict[str, np.ndarray], device: str = "cuda"):
+    def __init__(self, weight_dict_decoder: Dict[str, np.ndarray], trainable: bool = False, device: str = "cuda"):
+        if not isinstance(trainable, (bool, np.bool_)):
+            raise TypeError(f"trainable must be a bool, not {type(trainable).__name__}")
+        _check_decoder_weights(weight_dict_decoder)
         super().__init__()
-        self._device = device
+        self._device, self.trainable = device, bool(trainable)
         base = ShapeDecoderGradients(weight_dict_decoder, 1, device=device)
         with torch.no_grad():
             _ShapeDecoderFn.forward(SimpleNamespace(), _Once(base), None, torch.zeros((1, 200), device=base.store.device))
-        self._setup(base, False)
+        self._setup(base, self.trainable)
 
     def _make(self, B):
         return ShapeDecoderGradients(self._base.weight_dict, B, device=self._device, store=self.store)
+
+    def decoder_weight_dict(self) -> Dict[str, np.ndarray]:
+        """{npz key: fp32 ndarray} of the 12 variables (the TF name with '/' -> '_'): the dictionary ShapeDecoder,
+        ShapeDecoderGradients and FaceReconstruction take, so fine-tuned weights can be fed back into the reconstruction."""
+        from .Reconstruct_RenderNet_Face import DECODER_VARIABLES
+        names = dict((t, k) for t, k, _ in DECODER_VARIABLES)
+        return {names[n]: t.detach().cpu().numpy().copy() for n, t in self.store.vars.items() if n in names}
 
     def forward(self, latent):
         if not isinstance(latent, torch.Tensor) or latent.dim() != 2 or latent.shape[0] < 1 or latent.shape[1] != 200:
             raise ValueError(f"latent must be a [B,200] tensor, not {getattr(latent, 'shape', type(latent))}")
         self._sync_packed()
-        return _ShapeDecoderFn.apply(self, _grad_mode([], latent), latent)
+        params = list(self.params.values())
+        return _ShapeDecoderFn.apply(self, _grad_mode(params, latent), latent, *params)
 
 
 # ----------------------------------------------------------------------------------------------- Phong composite

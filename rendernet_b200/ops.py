@@ -920,6 +920,39 @@ def conv3d_f32(x: torch.Tensor, w_tf: torch.Tensor, bias: Optional[torch.Tensor]
     return out
 
 
+def conv3d_f32_weight_grad(x: torch.Tensor, gz: torch.Tensor, stride: int, transposed: bool):
+    """(dw, db) of a conv3d_f32 layer (rn_conv3d_f32_weight_grad): x fp32 [B,H,W,D,Cin] (the layer's input), gz = dL/d(pre-
+    activation) fp32 [B,Ho,Wo,Do,Cout] on the layer's output grid -> dw fp32 in the TF filter layout the forward reads ([4,4,4,Cout,
+    Cin] transposed, [4,4,4,Cin,Cout] forward) and db fp32 [Cout].  Shapes are checked before any launch.  Reproducible bit for
+    bit."""
+    if not isinstance(x, torch.Tensor) or not isinstance(gz, torch.Tensor) or x.dim() != 5 or gz.dim() != 5:
+        raise ValueError(f"conv3d_f32_weight_grad: x and gz must be 5-D tensors [B,H,W,D,C], not "
+                         f"{tuple(getattr(x, 'shape', ()))} and {tuple(getattr(gz, 'shape', ()))}")
+    s = int(stride)
+    if s not in (1, 2):
+        raise ValueError(f"conv3d_f32_weight_grad: stride must be 1 or 2, not {stride}")
+    B, H, W, D, Cin = (int(v) for v in x.shape)
+    Cout = int(gz.shape[4])
+    grid = (H * s, W * s, D * s) if transposed else (-(-H // s), -(-W // s), -(-D // s))
+    if tuple(int(v) for v in gz.shape[:4]) != (B,) + grid:
+        raise ValueError(f"conv3d_f32_weight_grad: gz {tuple(gz.shape)} is not the output of a stride-{s} "
+                         f"{'transposed ' if transposed else ''}conv of x {tuple(x.shape)} (expected [{B},{grid[0]},{grid[1]},"
+                         f"{grid[2]},C])")
+    if not (1 <= B <= 32 and 1 <= Cin <= 512 and 1 <= Cout <= 512):
+        raise ValueError(f"conv3d_f32_weight_grad: B = {B} (1..32), Cin = {Cin}, Cout = {Cout} (1..512) out of range")
+    x, gz = _cuda(x, torch.float32), _cuda(gz, torch.float32)
+    tr = 1 if transposed else 0
+    nwork = int(lib.rn_conv3d_f32_weight_grad_workspace(B, H, W, D, Cin, Cout, s, tr))
+    if nwork < 0:
+        check(nwork, "rn_conv3d_f32_weight_grad_workspace")
+    work = torch.empty(nwork, device=x.device, dtype=torch.float32)
+    dw = torch.empty((4, 4, 4, Cout, Cin) if transposed else (4, 4, 4, Cin, Cout), device=x.device, dtype=torch.float32)
+    db = torch.empty(Cout, device=x.device, dtype=torch.float32)
+    check(lib.rn_conv3d_f32_weight_grad(x.data_ptr(), gz.data_ptr(), dw.data_ptr(), db.data_ptr(), work.data_ptr(), B, H, W, D,
+                                        Cin, *grid, Cout, 4, s, tr, _stream()), "rn_conv3d_f32_weight_grad")
+    return dw, db
+
+
 def act_backward_f32(g: torch.Tensor, y: torch.Tensor, act: str) -> torch.Tensor:
     """dL/dz from dL/dy and the activation's output y, fp32 (rn_act_backward_f32): "elu" -> y < 0 ? g (y + 1) : g (TF-1 EluGrad),
     "sigmoid" -> g y (1 - y)."""
@@ -1201,22 +1234,30 @@ def prelu_alpha_grad(g, z, scale: float = 1.0) -> torch.Tensor:
     return da
 
 
-def fully_connected_param_grad(x: torch.Tensor, gy: torch.Tensor, z: torch.Tensor, alpha: torch.Tensor, want_gz: bool = False):
+def fully_connected_param_grad(x: torch.Tensor, gy: torch.Tensor, z: Optional[torch.Tensor], alpha: Optional[torch.Tensor],
+                               want_gz: bool = False):
     """Parameter gradient of y = prelu(x @ w + b; alpha) (rn_fully_connected_param_grad): x fp32 [B,K], gy = dL/dy and the
     pre-activation z fp32 [B,N], alpha fp32 [N] -> (gz = dL/dz [B,N] or None, dW [K,N], db [N], dalpha [N]), fp32, reproducible
-    bit for bit.  B <= 32, N % 4 == 0."""
-    x, gy, z, alpha = (_cuda(t, torch.float32) for t in (x, gy, z, alpha))
+    bit for bit.  B <= 32, N % 4 == 0.  z = alpha = None: an FC without activation (y = x @ w + b, the shape decoder's g_gc1):
+    gz = gy and dalpha is None."""
+    if (z is None) != (alpha is None):
+        raise ValueError("fully_connected_param_grad: pass both z and alpha (PReLU) or neither (no activation)")
+    ident = z is None
+    x, gy = _cuda(x, torch.float32), _cuda(gy, torch.float32)
+    if not ident:
+        z, alpha = _cuda(z, torch.float32), _cuda(alpha, torch.float32)
     B, K = (int(v) for v in x.shape)
     N = int(gy.shape[1])
-    if tuple(gy.shape) != (B, N) or tuple(z.shape) != (B, N) or alpha.numel() != N:
-        raise ValueError(f"fully_connected_param_grad: x {tuple(x.shape)}, gy {tuple(gy.shape)}, z {tuple(z.shape)}, "
-                         f"alpha {tuple(alpha.shape)} do not match")
-    gz = torch.empty_like(gy) if want_gz else None
+    if tuple(gy.shape) != (B, N) or (not ident and (tuple(z.shape) != (B, N) or alpha.numel() != N)):
+        raise ValueError(f"fully_connected_param_grad: x {tuple(x.shape)}, gy {tuple(gy.shape)}, "
+                         f"z {tuple(getattr(z, 'shape', ()))}, alpha {tuple(getattr(alpha, 'shape', ()))} do not match")
+    gz = None if not want_gz else (gy if ident else torch.empty_like(gy))
     dw = torch.empty((K, N), device=x.device, dtype=torch.float32)
     db = torch.empty(N, device=x.device, dtype=torch.float32)
-    da = torch.empty(N, device=x.device, dtype=torch.float32)
-    check(lib.rn_fully_connected_param_grad(x.data_ptr(), gy.data_ptr(), z.data_ptr(), alpha.data_ptr(), _ptr(gz), dw.data_ptr(),
-                                            db.data_ptr(), da.data_ptr(), B, K, N, _stream()), "rn_fully_connected_param_grad")
+    da = None if ident else torch.empty(N, device=x.device, dtype=torch.float32)
+    check(lib.rn_fully_connected_param_grad(x.data_ptr(), gy.data_ptr(), _ptr(z), _ptr(alpha), None if ident else _ptr(gz),
+                                            dw.data_ptr(), db.data_ptr(), _ptr(da), B, K, N, _stream()),
+          "rn_fully_connected_param_grad")
     return gz, dw, db, da
 
 
