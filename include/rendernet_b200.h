@@ -354,7 +354,9 @@ int rn_prelu_backward_f32(const float* g, const float* z, const float* alpha, fl
  * tf_phong_composite(normal, light_dir, light_col, ambient, k_diffuse, black_background, with_mask), loss[b] += mean_{h,w,c}
  * (target - albedo * shade)^2, and in the same pass d_albedo, d_normal (fp32 [B,H,W,3], overwritten) and d_light_dir [B,3]
  * (ACCUMULATED into: zero it first; may be NULL).  loss (double [B]) is accumulated into as well.  TF-1 gradient conventions:
- * tf.maximum passes where x >= y, clip_by_value where lo <= x <= hi, d|x|/dx = x/|x|.  light_dir, light_col [B,3]. */
+ * tf.maximum passes where x >= y, clip_by_value where lo <= x <= hi, d|x|/dx = x/|x|.  At normal = (0.5, 0.5, 0.5) the pixel
+ * is shaded as unlit, only the mask term reaches d_normal and nothing reaches d_light; where |normal| = 0 the mask term is 0, so
+ * every output is finite for normal maps in [0, 1].  light_dir, light_col [B,3]. */
 int rn_phong_recon_loss_grad(const float* albedo, const float* normal, const float* target, const float* light_dir,
                              const float* light_col, float ambient, float k_diffuse, int black_background, int with_mask,
                              double* loss, float* d_albedo, float* d_normal, float* d_light_dir, int B, int H, int W,

@@ -417,13 +417,16 @@ __global__ void fc_bwd_data_reduce_kernel(const float* __restrict__ part, float*
 // ------------------------------------------------------------------------------------------ face reconstruction objective
 // Reconstruct_RenderNet_Face.py:372-383 over TensorFlow's Phong composite (tools/Phong_shading.py:24-113 tf_mask /
 // tf_mask_white / tf_phong_shading / tf_phong_composite -- NOT the NumPy composite of phong_pixel):
-//   L = l / |l|;  u = (n - 0.5) / |n - 0.5|;  dif_c = clip(k_d * max(u.L, 0) * col_c, 0, 1)
-//   m = sigmoid(255 |n| - 80) (black background) or sigmoid(255 (sqrt 3 - |n|) - 80) (white)
-//   shade_c = clip(m (ambient + dif_c) + 1 - m, 0, 1)   (with_mask; else clip(ambient + dif_c, 0, 1))
+//   shade = tf_phong_pixel(n, L = l / |l|, col, ambient, k_d, black, with_mask)     (rn_phong.cuh: the image rn_phong_shade renders)
 //   loss[b] = mean_{h,w,c} (target - albedo_c shade_c)^2
-// and its gradient, in one pass, with TF-1's gradient conventions: tf.maximum(x, y) passes to x where x >= y;
-// clip_by_value(x, lo, hi) passes where lo <= x <= hi; d|x|/dx = x/|x|.  One thread per pixel; blockIdx.y = batch item.  loss
-// is accumulated in double (one atomic per block); dL/dL is reduced over the block and mapped through the normalisation
+// and its gradient in one pass: with g_c = dL/d(compos_c) = 2 (compos_c - target_c) / (3 HW), compos = albedo shade in fp32,
+// d_albedo_c = g_c shade_c and dL/d(shade_c) = g_c albedo_c, the latter through tf_phong_pixel_backward on the terms the forward
+// call recorded.  g is formed in double and rounded once: it is the fp32 value autograd of a float64 MSE on rn_phong_shade's
+// compos hands rn_phong_shade_backward, so the fused and the composed objectives give the same image gradients.  TF-1's gradient
+// conventions: tf.maximum(x, y) passes to x where x >= y; clip_by_value(x, lo, hi) passes where lo <= x <= hi; d|x|/dx = x/|x|.
+// At n = (0.5, 0.5, 0.5) u = 0/0 and d are NaN: the forward shades the pixel as unlit, only the mask term reaches d_normal and
+// the pixel adds nothing to d_light.  Where |n| = 0 the mask term is 0.  One thread per pixel; blockIdx.y = batch item.  loss is
+// accumulated in double (one atomic per block); dL/dL is reduced over the block and mapped through the normalisation
 // (I - L L^T) / |l| before one atomic per block and component.
 __global__ void __launch_bounds__(256) phong_recon_loss_grad_kernel(const float* __restrict__ albedo, const float* __restrict__ normal,
                                                                     const float* __restrict__ target, const float* __restrict__ light_dir,
@@ -437,60 +440,26 @@ __global__ void __launch_bounds__(256) phong_recon_loss_grad_kernel(const float*
   const float lnorm = sqrtf(l0 * l0 + l1 * l1 + l2 * l2);
   const float L[3] = {l0 / lnorm, l1 / lnorm, l2 / lnorm};
   const float col[3] = {__ldg(light_col + 3 * b), __ldg(light_col + 3 * b + 1), __ldg(light_col + 3 * b + 2)};
-  const float inv_n = 2.f / (3.f * static_cast<float>(HW));          // d mean / d pred, times the 2 of the square
+  const double inv_n = 1.0 / (3.0 * static_cast<double>(HW));         // d mean / d compos
   float part[4] = {0.f, 0.f, 0.f, 0.f};                                // loss, dL/dL (3)
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p < HW) {
     const size_t o = (static_cast<size_t>(b) * HW + p) * 3;
     const float n[3] = {normal[o], normal[o + 1], normal[o + 2]};
-    const float v[3] = {n[0] - 0.5f, n[1] - 0.5f, n[2] - 0.5f};
-    const float vn = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
-    const float u[3] = {v[0] / vn, v[1] / vn, v[2] / vn};
-    const float d = u[0] * L[0] + u[1] * L[1] + u[2] * L[2];
-    const float dmax = fmaxf(d, 0.f);
-    // The mask's argument 255 |n| - 80 multiplies |n|'s rounding by 255 and its derivative by another 255: evaluated in fp32 it
-    // alone moves the shading by ~1e-5.  It is a handful of operations per pixel, so it runs in double.
-    float m = 1.f;
-    double md = 1.0, nnd = 1.0;
-    if (with_mask) {
-      nnd = sqrt(static_cast<double>(n[0]) * n[0] + static_cast<double>(n[1]) * n[1] + static_cast<double>(n[2]) * n[2]);
-      const double s = black ? 255.0 * nnd - 80.0 : 255.0 * (1.7320508075688772 - nnd) - 80.0;
-      md = 1.0 / (1.0 + exp(-s));
-      m = static_cast<float>(md);
-    }
-    float ddmax = 0.f, dm = 0.f;
+    float shade[3], ds[3], dn[3];
+    TfPhongTerms t;
+    tf_phong_pixel(n[0], n[1], n[2], L, col, ambient, k_diffuse, black, with_mask, shade, &t);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float pre = k_diffuse * dmax * col[c];
-      const float dif = fminf(fmaxf(pre, 0.f), 1.f);
-      const float x = with_mask ? m * (ambient + dif) + (1.f - m) : ambient + dif;
-      const float shade = fminf(fmaxf(x, 0.f), 1.f);
       const float a = albedo[o + c];
-      const float r = a * shade - target[o + c];
+      const float compos = __fmul_rn(a, shade[c]);                     // the fp32 compos rn_phong_shade returns
+      const float r = __fsub_rn(compos, target[o + c]);
       part[0] += r * r;
-      const float dpred = inv_n * r;
-      d_albedo[o + c] = dpred * shade;
-      const float dx = (x >= 0.f && x <= 1.f) ? dpred * a : 0.f;          // clip_by_value(compos, 0, 1)
-      const float ddif = with_mask ? dx * m : dx;
-      if (with_mask) dm += dx * (ambient + dif - 1.f);
-      const float dpre = (pre >= 0.f && pre <= 1.f) ? ddif : 0.f;         // clip_by_value(diffuse, 0, 1)
-      ddmax += dpre * k_diffuse * col[c];
+      const float dpred = static_cast<float>(2.0 * __dmul_rn(inv_n, __dsub_rn(compos, target[o + c])));
+      d_albedo[o + c] = dpred * shade[c];
+      ds[c] = dpred * a;
     }
-    const float dd = d >= 0.f ? ddmax : 0.f;                              // tf.maximum(d, 0): passes where d >= 0
-    float du[3], dn[3];
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-      du[i] = dd * L[i];
-      part[1 + i] += dd * u[i];
-    }
-    const float udu = u[0] * du[0] + u[1] * du[1] + u[2] * du[2];       // d (v/|v|) = (du - u (u.du)) / |v|
-#pragma unroll
-    for (int i = 0; i < 3; ++i) dn[i] = (du[i] - u[i] * udu) / vn;
-    if (with_mask) {                                                      // sigmoid, then d|n|/dn = n/|n|
-      const double ds = static_cast<double>(dm) * md * (1.0 - md) * (black ? 255.0 : -255.0) / nnd;
-#pragma unroll
-      for (int i = 0; i < 3; ++i) dn[i] += static_cast<float>(ds * n[i]);
-    }
+    tf_phong_pixel_backward(n, L, t, col, ambient, k_diffuse, black, with_mask, ds, dn, part + 1);
 #pragma unroll
     for (int i = 0; i < 3; ++i) d_normal[o + i] = dn[i];
   }

@@ -2,9 +2,10 @@
 // np_phong_composite, RenderNet_demo.py:54-58), shared by the stand-alone kernel (rn_ops.cu), the fused epilogue of the
 // last up-conv (rn_igemm_kernel.cuh) and the Shader fit's loss kernel (rn_backward.cu) so that all three produce the same bits;
 // and one pixel of TensorFlow's composite
-// (tf_phong_pixel), which the stand-alone kernel renders for face reconstruction.  Next to each, its backward for an arbitrary
-// upstream gradient (phong_pixel_backward, tf_phong_pixel_backward), which rn_phong_shade_backward (rn_backward.cu) runs on the
-// terms its own forward call recorded.
+// (tf_phong_pixel), which the stand-alone kernel renders for face reconstruction and the reconstruction loss (rn_backward.cu)
+// measures.  Next to each, its backward for an arbitrary upstream gradient (phong_pixel_backward, tf_phong_pixel_backward), which
+// rn_phong_shade_backward and, for tf_phong_pixel, the reconstruction loss (rn_backward.cu) run on the terms their own forward
+// call recorded.
 #pragma once
 #include <cstdint>
 
@@ -110,24 +111,28 @@ struct TfPhongTerms {
 
 // TensorFlow's composite (tools/Phong_shading.py:24-113 tf_mask / tf_mask_white / tf_phong_shading / tf_phong_composite), the
 // shading Reconstruct_RenderNet_Face.py:372-378 multiplies the albedo by.  (n0,n1,n2) = normal map in [0,1]; L = the light
-// direction ALREADY normalised as l / |l| (division, not a reciprocal); col = light colour.  The operation order, the fp32
-// rounding points and the mask in double are those of the forward half of phong_recon_loss_grad_kernel (rn_backward.cu), so the
-// image this returns is the one the reconstruction loss measures, bit for bit.  Unlike phong_pixel: the normal is not clamped
+// direction ALREADY normalised as l / |l| (division, not a reciprocal); col = light colour.  phong_recon_loss_grad_kernel
+// (rn_backward.cu) shades with this function, so the image it returns is the one the reconstruction loss measures, bit for bit.
+// The mask's argument multiplies |n|'s rounding by 255 (and its derivative by another 255), so the mask runs in double.  At
+// n = (0.5, 0.5, 0.5) u and d are NaN and fmaxf shades the pixel as unlit.  Unlike phong_pixel: the normal is not clamped
 // away from |n - 0.5| = 0, the white mask is sigmoid(255 (sqrt 3 - |n|) - 80) and the black one sigmoid(255 |n| - 80).  If `t` is
 // not NULL it receives the intermediates the gradient needs (recorded, not recomputed).
 __device__ __forceinline__ void tf_phong_pixel(float n0, float n1, float n2, const float* L, const float* col, float ambient,
                                                float k_diffuse, int black, int with_mask, float* out, TfPhongTerms* t = nullptr) {
+  // Every rounding is spelled out (the _rn intrinsics are never contracted or reassociated): left to the compiler, a sum of
+  // products is contracted into FMAs in an order that depends on the calling kernel, and the callers would differ in the last bit.
   const float v[3] = {n0 - 0.5f, n1 - 0.5f, n2 - 0.5f};
-  const float vn = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
-  const float u[3] = {v[0] / vn, v[1] / vn, v[2] / vn};
-  const float d = u[0] * L[0] + u[1] * L[1] + u[2] * L[2];
+  const float vn = __fsqrt_rn(__fmaf_rn(v[2], v[2], __fmaf_rn(v[0], v[0], __fmul_rn(v[1], v[1]))));
+  const float u[3] = {__fdiv_rn(v[0], vn), __fdiv_rn(v[1], vn), __fdiv_rn(v[2], vn)};
+  const float d = __fmaf_rn(u[2], L[2], __fmaf_rn(u[0], L[0], __fmul_rn(u[1], L[1])));
   const float dmax = fmaxf(d, 0.f);
   float m = 1.f;
   double md = 1.0, nnd = 1.0;
   if (with_mask) {
-    nnd = sqrt(static_cast<double>(n0) * n0 + static_cast<double>(n1) * n1 + static_cast<double>(n2) * n2);
-    const double s = black ? 255.0 * nnd - 80.0 : 255.0 * (1.7320508075688772 - nnd) - 80.0;
-    md = 1.0 / (1.0 + exp(-s));
+    const double e[3] = {n0, n1, n2};
+    nnd = __dsqrt_rn(__fma_rn(e[2], e[2], __fma_rn(e[0], e[0], __dmul_rn(e[1], e[1]))));
+    const double s = __fma_rn(black ? nnd : __dsub_rn(1.7320508075688772, nnd), 255.0, -80.0);
+    md = __drcp_rn(__dadd_rn(1.0, exp(-s)));
     m = static_cast<float>(md);
   }
   if (t != nullptr) {
@@ -136,20 +141,19 @@ __device__ __forceinline__ void tf_phong_pixel(float n0, float n1, float n2, con
   }
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float pre = k_diffuse * dmax * col[c];
+    const float pre = __fmul_rn(__fmul_rn(k_diffuse, dmax), col[c]);
     const float dif = fminf(fmaxf(pre, 0.f), 1.f);
-    const float x = with_mask ? m * (ambient + dif) + (1.f - m) : ambient + dif;
+    const float x = with_mask ? __fmaf_rn(m, __fadd_rn(ambient, dif), __fsub_rn(1.f, m)) : __fadd_rn(ambient, dif);
     if (t != nullptr) { t->pre[c] = pre; t->dif[c] = dif; t->x[c] = x; }
     out[c] = fminf(fmaxf(x, 0.f), 1.f);
   }
 }
 
-// Backward of one tf_phong_pixel call for an arbitrary upstream gradient ds = dL/d(out) (rn_phong_shade_backward): dn = dL/dn
-// and dl = dL/dL (L already normalised; the caller maps dl through (I - L L^T) / |l|).  n: the pixel, t: the call's own terms.
-// The chain rule of phong_recon_loss_grad_kernel's TF-1 conventions (max(x, 0) passes where x >= 0, a clip where lo <= x <= hi,
-// d|x|/dx = x / |x|), the mask's derivative in double.  Unlike that kernel, the normal's term is skipped where nothing passes
-// max(d, 0): at n = (0.5, 0.5, 0.5) u = 0/0 and d are NaN, and dn gets the mask term alone, dl nothing.  At |n| = 0 the mask
-// term is 0.
+// Backward of one tf_phong_pixel call for an arbitrary upstream gradient ds = dL/d(out) (rn_phong_shade_backward,
+// phong_recon_loss_grad_kernel): dn = dL/dn and dl = dL/dL (L already normalised; the caller maps dl through (I - L L^T) / |l|).
+// n: the pixel, t: the call's own terms.  TF-1's conventions (max(x, 0) passes where x >= 0, a clip where lo <= x <= hi,
+// d|x|/dx = x / |x|), the mask's derivative in double.  The normal's term is skipped where nothing passes max(d, 0): at
+// n = (0.5, 0.5, 0.5) u = 0/0 and d are NaN, and dn gets the mask term alone, dl nothing.  At |n| = 0 the mask term is 0.
 __device__ __forceinline__ void tf_phong_pixel_backward(const float* n, const float* L, const TfPhongTerms& t, const float* col,
                                                         float ambient, float k_diffuse, int black, int with_mask, const float* ds,
                                                         float* dn, float* dl) {

@@ -23,7 +23,7 @@ def _d(a):
 
 def _normals(B, H, W, seed):
     """Random normal maps in [0,1] plus black (0) and white (1) background pixels, exact 0 / 1 components, pixels on the kinks
-    of light (0,0,2) (u.L = 1 and u.L = 0) and mask transitions.  No pixel is (0.5, 0.5, 0.5)."""
+    of light (0,0,2) (u.L = 1 and u.L = 0), mask transitions and n = (0.5, 0.5, 0.5), which is shaded as unlit."""
     rng = np.random.default_rng(seed)
     n = rng.random((B, H, W, 3)).astype(np.float32)
     n[:, 0, :8] = 0.0
@@ -34,6 +34,7 @@ def _normals(B, H, W, seed):
     n[:, 4, :8] = 0.97 + 0.03 * n[:, 4, :8]
     n[:, 5, 0:8] = [0.5, 0.5, 0.75]
     n[:, 5, 8:16] = [0.75, 0.5, 0.5]
+    n[:, 6, :8] = 0.5
     return n
 
 
@@ -119,9 +120,7 @@ def test_tf_shading_is_the_image_the_loss_measures(black, mask, ambient, kd):
     (bit-identical images).  A random albedo against target 0: the loss is the float64 mean of compos^2 (1e-6 relative)."""
     from rendernet_b200 import ops
     B = 2
-    n = _normals(B, 64, 64, 12)
-    n[:, 0, :8] = 0.02       # d|n|/dn = n/|n| is 0/0 at n = 0 in the loss kernel's mask derivative (as at n = 0.5 in u's)
-    n = _d(n)
+    n = _d(_normals(B, 64, 64, 12))
     ld, lc = (_d(a) for a in _lights(B, 13))
     shade, _, _ = ops.phong_shade(n, ld, lc, ambient, kd, composite="tf", background_white=not black, with_mask=mask,
                                   want_compos=False, want_u8=False)
