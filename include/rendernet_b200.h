@@ -146,6 +146,9 @@ typedef struct rn_conv_desc {
    * consumer warpgroups storing their own rows directly */
   int epi_groups, res_prefetch, tma_store;
   const rn_phong* phong;    /* NULL, or the fused Phong epilogue (act = RN_ACT_SIGMOID, N = F pixels x 3 channels <= 16) */
+  /* > 0 (ntaps == 1 only): image b reads filter tap b / b_tap_div of w_packed, which then holds B / b_tap_div taps -- the
+   * 16 per-position GEMMs of a Winograd convolution as one launch.  0 = off. */
+  int b_tap_div;
 } rn_conv_desc;
 int rn_conv_igemm(const rn_conv_desc* d, void* stream);
 /* Per-call overrides of the launch heuristics for the reference-shaped wrappers below (their last argument before
@@ -154,6 +157,7 @@ int rn_conv_igemm(const rn_conv_desc* d, void* stream);
  * Every combination computes bit-identical results (tests/test_gpu_kernels.py::*_bit_identical). */
 typedef struct rn_tuning {
   int cluster, cta_group, kps, msub, epilogue_groups, res_prefetch, tma_store, yhalo;
+  int winograd;             /* rn_conv2d_winograd_eligible: 1 = on, -1 = off (the direct kernel), 0 = default (RN_TUNE) */
 } rn_tuning;
 /* The launch plan rn_conv_igemm would use for `d`, without touching the device (works on a host without a GPU; the SM
  * count then defaults to 132).  Pointers in `d` are only tested for null / 16-byte alignment.  out[0..n_out) receives
@@ -200,6 +204,28 @@ int rn_conv3d_sliced_same(const void* x, const void* w_sliced, const float* bias
                           const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W, int D,
                           int Cin, int Cout, int fmt, void* stream);
 int rn_conv3d_sliced_plan(int B, int H, int W, int D, int fmt, int* out, int n_out);
+
+/* 3x3 SAME stride-1 conv2d, C -> C channels, RN_FMT_F16X2 only, as Winograd F(2x2, 3x3) (rn_winograd.cu): 16 products per
+ * 2x2 output block instead of 36, and 16 accumulations of K = C instead of one of K = 9C.
+ *   rn_winograd_in:   x [2][B,H,W,C] hi/lo -> V [2][16][B,H/2,W/2,C] hi/lo, V = B^T d B of every 4x4 input patch (SAME zero
+ *                     padding), summed in fp32 from hi + lo and split once.
+ *   rn_winograd_gemm: M [16][B,H/2,W/2,C] fp32 = V . U per position: one igemm launch (b_tap_div = B), no bias or activation.
+ *                     u [2][16][C][C] hi/lo: U = G g G^T of the filter per position, [position][Cout][Cin] (ops.winograd_filter).
+ *   rn_winograd_out:  y = A^T M A of every 2x2 block, then bias, PReLU / none, the residual and the stores exactly as the
+ *                     igemm epilogue does them (out16 hi/lo and/or out32).
+ * rn_conv2d_winograd runs the three on `workspace` (rn_winograd_workspace_bytes(B, H, W, C) bytes: V then M).
+ * rn_conv2d_winograd_eligible says whether ops.conv2d takes the Winograd path for a layer of this shape (fmt 2,
+ * 3x3, H and W even, Cin = Cout = a multiple of 64 >= 1024, tune->winograd / RN_TUNE winograd not off; tune->winograd = 1
+ * also takes Cin < 1024).  Host-only. */
+long long rn_winograd_workspace_bytes(int B, int H, int W, int C);
+int rn_conv2d_winograd_eligible(int fmt, int kh, int kw, int H, int W, int Cin, int Cout, int cout_pad, const rn_tuning* tune);
+int rn_winograd_in(const void* x, void* v, int B, int H, int W, int C, void* stream);
+int rn_winograd_gemm(const void* v, const void* u, float* m, int B, int H, int W, int C, const rn_tuning* tune, void* stream);
+int rn_winograd_out(const float* m, const float* bias, const float* alpha, int act, const void* residual, int residual_is_f32,
+                    void* out16, float* out32, int B, int H, int W, int C, void* stream);
+int rn_conv2d_winograd(const void* x, const void* u, const float* bias, const float* alpha, int act, const void* residual,
+                       int residual_is_f32, void* out16, float* out32, int B, int H, int W, int C, void* workspace,
+                       long long workspace_bytes, const rn_tuning* tune, void* stream);
 
 /* slim.conv2d_transpose / layer_util.conv2d_transpose (layer_util.py:186; RenderNet_Shader.py:106-129),
  * SAME, out = in*stride.  w_packed holds the stride^2 phase filters back to back, as produced by

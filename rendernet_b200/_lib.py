@@ -29,7 +29,7 @@ class rn_conv_desc(C.Structure):
         ("o_nsplit", C.c_int), ("o_nhi", C.c_longlong),
         ("x_plane", C.c_longlong), ("w_plane", C.c_longlong), ("o_plane", C.c_longlong),
         ("epi_groups", C.c_int), ("res_prefetch", C.c_int), ("tma_store", C.c_int),
-        ("phong", C.c_void_p),
+        ("phong", C.c_void_p), ("b_tap_div", C.c_int),
     ]
 
 
@@ -39,7 +39,8 @@ class rn_phong(C.Structure):
 
 
 class rn_tuning(C.Structure):
-    _fields_ = [(n, C.c_int) for n in ("cluster", "cta_group", "kps", "msub", "epilogue_groups", "res_prefetch", "tma_store", "yhalo")]
+    _fields_ = [(n, C.c_int) for n in ("cluster", "cta_group", "kps", "msub", "epilogue_groups", "res_prefetch", "tma_store", "yhalo",
+                                       "winograd")]
 
 
 _vp, _i, _f, _ll = C.c_void_p, C.c_int, C.c_float, C.c_longlong
@@ -70,6 +71,12 @@ SIGNATURES = {
     "rn_pack_conv3d_sliced": (_i, [_vp, _vp, _i, _vp]),
     "rn_conv3d_sliced_same": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "rn_conv3d_sliced_plan": (_i, [_i, _i, _i, _i, _i, C.POINTER(C.c_int), _i]),
+    "rn_winograd_workspace_bytes": (_ll, [_i, _i, _i, _i]),
+    "rn_conv2d_winograd_eligible": (_i, [_i] * 8 + [_tp]),
+    "rn_winograd_in": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "rn_winograd_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _tp, _vp]),
+    "rn_winograd_out": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "rn_conv2d_winograd": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _ll, _tp, _vp]),
     "rn_pack_conv2d_transpose_weights": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "rn_conv2d_transpose_same": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _tp, _vp]),
     "rn_pack_conv2d_transpose_s2_merged": (_i, [_vp, _vp, _i, _i, _i, _vp]),

@@ -196,7 +196,7 @@ class _InputGradients:
         if kind == "conv2d":                       # [kh,kw,Ci,Co] -> mirrored, channel roles swapped: [kh,kw,Co,Ci]
             k = int(w.shape[0])
             wd = torch.flip(wt, dims=(0, 1)).permute(0, 1, 3, 2).contiguous()
-            L = ops.pack_conv("conv2d", wd, None, None, device=dev, fmt=fmt)
+            L = ops.pack_conv("conv2d", wd, None, None, device=dev, fmt=fmt, winograd=False)
             pb = (k - 1) // 2
             L.taps = [(kx - (k - 1 - pb), ky - (k - 1 - pb)) for ky in range(k) for kx in range(k)]   # offset of mirrored tap
         elif kind == "conv3d":                     # 3^3, stride 1: depth-folded gradient conv
@@ -209,7 +209,7 @@ class _InputGradients:
             cp = ops.round_up(co, 16)
             wd = torch.zeros((w.shape[0], w.shape[1], cp, w.shape[3]), device=dev, dtype=torch.float32)
             wd[:, :, :co] = wt
-            L = ops.pack_conv("conv2d", wd, None, None, device=dev, fmt=fmt)
+            L = ops.pack_conv("conv2d", wd, None, None, device=dev, fmt=fmt, winograd=False)
             L.taps = None
         elif kind == "conv2d_transpose" and stride == 2:
             # o = 2i + k - 1.  With g2[i,j,(ay,ax,co)] = g[2i+ay, 2j+ax, co]:  dx[i] = sum_{dy,dx in -1..1} g2[i+dy, j+dx] . Wd[dy+1][dx+1]
@@ -227,7 +227,7 @@ class _InputGradients:
                             kx = 2 * dx + ax + 1
                             if 0 <= kx < 4:
                                 wd[dy + 1, dx + 1, ay, ax] = wt[ky, kx]
-            L = ops.pack_conv("conv2d", wd.reshape(3, 3, 4 * co, ci), None, None, device=dev, fmt=fmt)
+            L = ops.pack_conv("conv2d", wd.reshape(3, 3, 4 * co, ci), None, None, device=dev, fmt=fmt, winograd=False)
             L.taps = None
         else:
             raise NotImplementedError(f"no data-gradient path for {kind} stride {stride}")

@@ -91,6 +91,7 @@ static Tuning parse_tuning() {
   get("yhalo", &t.yhalo, 0, 1);
   get("tiled_tex_conv", &t.tiled_tex_conv, 0, 1);
   get("pdl", &t.pdl, 0, 1);
+  get("winograd", &t.winograd, 0, 1);
   return t;
 }
 const Tuning& tuning() {
@@ -147,6 +148,7 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
   if (d->out16 == nullptr && d->out32 == nullptr) return -6;
   const int D = d->ndim == 3 ? d->D : 1;
   if (d->B < 1 || d->H < 1 || d->W < 1 || D < 1) return -7;
+  if (d->b_tap_div < 0 || (d->b_tap_div > 0 && (d->ntaps != 1 || d->w_banded || d->B % d->b_tap_div != 0))) return -23;
 
   const Tuning& tn = tuning();
   const bool split = d->fmt == 2;
@@ -196,6 +198,7 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
     p.band_half = 1;                        // the packed filter is in processing order even when no block is a half block
     for (int i = 0; i < L.kblocks; ++i) { p.kb_order[i] = L.order[i]; p.kb_half[i] = L.half[i]; }
   }
+  p.b_tap_div = d->b_tap_div;
   p.rank = d->ndim == 3 ? 5 : 4;
   p.W = d->W; p.H = d->H; p.D = D; p.B = d->B;
   int grid = 0, CL = 1, sub = 0;
@@ -359,7 +362,8 @@ extern "C" int rn_conv_igemm(const rn_conv_desc* d, void* stream_v) {
       r = enc(&p.tmB2, dt, 3, const_cast<uint16_t*>(w_lo), dims, strides, box, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
               swizzle_of(p.row_bytes), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   } else {
-    const cuuint64_t dims[3] = {(cuuint64_t)d->Cin, (cuuint64_t)d->cout_pad, (cuuint64_t)d->ntaps};
+    const int btaps = d->b_tap_div > 0 ? d->ntaps * (d->B / d->b_tap_div) : d->ntaps;   // taps of the packed filter
+    const cuuint64_t dims[3] = {(cuuint64_t)d->Cin, (cuuint64_t)d->cout_pad, (cuuint64_t)btaps};
     const cuuint64_t strides[2] = {(cuuint64_t)d->Cin * 2, (cuuint64_t)d->Cin * 2 * d->cout_pad};
     const cuuint32_t box[3] = {(cuuint32_t)KB, (cuuint32_t)(BN / CL), 1};  // each CTA of a cluster fetches 1/CL of B
     r = enc(&p.tmB, dt, 3, const_cast<uint16_t*>(w_hi), dims, strides, box, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,

@@ -71,6 +71,8 @@ struct alignas(64) IgemmParams {
   int phong_F, phong_white, phong_mask;
   int o_nsplit;                   // > 0: column n lands at (n / o_nsplit) * o_nhi + (n % o_nsplit) instead of n (merged
   long long o_nhi;                //      phases of a stride-2 transposed conv: n = (ay, ax, co))
+  int b_tap_div;                  // > 0 (one-tap convs only): image b of the tile reads filter tap b / b_tap_div -- the 16
+                                  // per-position GEMMs of a Winograd conv as one launch over [16*B, H/2, W/2, C]
 };
 
 // Band structure of the depth-folded 3^3 conv3d (rn_conv3d_banded_same): N tile = 128/Cout output depths x Cout, K per tap =
@@ -119,6 +121,7 @@ struct Tuning {
   int tiled_tex_conv = 1; // shared-memory tiled kernel for the texture decoder's 4^3 8->4 conv (0: generic kernel; A/B, tests)
   int pdl = 0;            // programmatic dependent launch: igemm launches carry the programmatic-stream-serialization attribute,
                           // trigger their dependents after the prologue and griddepcontrol.wait before touching global memory
+  int winograd = 1;       // exact-mode 3x3 trunk convs as Winograd F(2x2, 3x3) (rn_winograd.cu; 0: the direct kernel, for A/B)
 };
 const Tuning& tuning();
 

@@ -304,6 +304,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
         const TileCoord t = decode_tile(p, tile_of(ct), BN);
         const int a_c0 = p.a_c_base + (t.n0 / BN) * p.a_c_ntile;
         const int bn0 = t.n0 + b_row;
+        const int tap0 = p.b_tap_div > 0 ? t.b / p.b_tap_div : 0;
         int left = total_k, j = 0, n_here = 0;
         uint32_t dst = 0, bar = 0;
         for (int kx = 0; kx < nx; ++kx) {      // tap(ky, kx) = ky*nx + kx; entry kx holds (dx, dy of ky = 0, dz)
@@ -326,6 +327,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
               int tap = ky * nx + kx;
               const uint64_t mapB = (split && (p.tap[tap][3] & 2)) ? mapB_lo : mapB_hi;
               if (split) tap = p.tap_b[tap];
+              tap += tap0;
               if constexpr (CL > 1) {
                 if (banded) tma_a_3d_mc(bdst + b_off, mapB, bar, kMask, 0, b_row, tap * kblocks + kb);
                 else tma_a_3d_mc(bdst + b_off, mapB, bar, kMask, bk, bn0, tap);

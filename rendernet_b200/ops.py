@@ -201,6 +201,11 @@ class PackedConv:
     alpha: Optional[torch.Tensor]  # fp32 [cout_pad]
     dtype: torch.dtype
     fmt: int = 0                   # RN_FMT_*: 0 fp16, 1 bf16, 2 fp16 hi/lo pairs (w then holds [2][...])
+    # exact-mode 3x3 C -> C convs: the fp32 filter the Winograd filter U is made from on first use (winograd_filter), the
+    # version it had when w was packed, and U itself.  U lives and dies with this object, so a re-pack drops it with w.
+    master: Optional[torch.Tensor] = None
+    master_version: int = 0
+    wino: Optional[torch.Tensor] = None
 
 
 def _pad_vec(v: Optional[torch.Tensor], n: int, n_pad: int, device) -> Optional[torch.Tensor]:
@@ -212,9 +217,10 @@ def _pad_vec(v: Optional[torch.Tensor], n: int, n_pad: int, device) -> Optional[
 
 
 def pack_conv(kind: str, w_tf: torch.Tensor, bias: Optional[torch.Tensor], alpha: Optional[torch.Tensor],
-              stride: int = 1, dtype: torch.dtype = torch.float16, device="cuda", fmt: Optional[int] = None) -> PackedConv:
+              stride: int = 1, dtype: torch.dtype = torch.float16, device="cuda", fmt: Optional[int] = None,
+              winograd: bool = True) -> PackedConv:
     """w_tf in TF filter layout: conv2d [kh,kw,Cin,Cout]; conv3d [k,k,k,Cin,Cout];
-    conv2d_transpose [kh,kw,Cout,Cin]."""
+    conv2d_transpose [kh,kw,Cout,Cin].  winograd=False keeps an exact-mode 3x3 C -> C conv on the direct kernel."""
     w_tf = torch.as_tensor(w_tf, dtype=torch.float32).to(device).contiguous()
     fmt = fmt_of(dtype) if fmt is None else int(fmt)
     if kind == "conv2d_transpose":
@@ -243,7 +249,30 @@ def pack_conv(kind: str, w_tf: torch.Tensor, bias: Optional[torch.Tensor], alpha
                                        fmt, _stream()), "pack")
     b = _pad_vec(bias if bias is not None else torch.zeros(cout), cout, cout_pad, device)
     a = _pad_vec(alpha, cout, cout_pad, device)
-    return PackedConv(kind, ks, stride, cin, cout, cout_pad, packed, b, a, dtype, fmt)
+    L = PackedConv(kind, ks, stride, cin, cout, cout_pad, packed, b, a, dtype, fmt)
+    if winograd and kind == "conv2d" and fmt == 2 and tuple(ks) == (3, 3) and cin == cout:
+        L.master, L.master_version = w_tf, w_tf._version
+    return L
+
+
+_WINO_G = ((1.0, 0.0, 0.0), (0.5, 0.5, 0.5), (0.5, -0.5, 0.5), (0.0, 0.0, 1.0))
+
+
+def winograd_filter_f32(w_tf: torch.Tensor) -> torch.Tensor:
+    """Winograd F(2x2, 3x3) filter transform U = G g G^T of a TF 3x3 filter [3,3,Cin,Cout], computed in float64 and rounded
+    once: fp32 [16 = (row, column) of the 4x4 tile][Cout][Cin], the packed-filter layout with 16 "taps" (rn_winograd.cu)."""
+    w = w_tf.detach().to(torch.float64)
+    G = torch.tensor(_WINO_G, dtype=torch.float64, device=w.device)
+    U = torch.einsum("ak,klio,bl->aboi", G, w, G)
+    return U.reshape(16, w.shape[3], w.shape[2]).float().contiguous()
+
+
+def winograd_filter(L: PackedConv) -> torch.Tensor:
+    """U of an exact-mode 3x3 layer as fp16 hi/lo planes [2][16][Cout][Cin], made on first use (an engine's warm-up, before
+    graph capture) from the filter L was packed from."""
+    if L.wino is None:
+        L.wino = cast_to_16(winograd_filter_f32(L.master), fmt=2).planes
+    return L.wino
 
 
 def _out_buffers(shape, dtype, device, want16, want32, out16, out32, fmt: int = 0):
@@ -287,6 +316,17 @@ def conv2d(x: torch.Tensor, L: PackedConv, act: Optional[str] = None, residual: 
     if residual is not None:
         assert tuple(residual.shape[-4:]) == (B, H, W, L.cout)
     a = _ACT[act]
+    kh, kw = L.ksize
+    if L.master is not None and lib.rn_conv2d_winograd_eligible(L.fmt, kh, kw, H, W, Cin, L.cout, L.cout_pad, _tune(tune)):
+        if L.master._version != L.master_version:
+            raise RuntimeError("the filter changed after it was packed: re-pack the layer (pack_conv) before running it")
+        # the caching allocator hands the same workspace block to every trunk layer in turn (also inside a graph capture)
+        ws = torch.empty(lib.rn_winograd_workspace_bytes(B, H, W, Cin), device=x.device, dtype=torch.uint8)
+        check(lib.rn_conv2d_winograd(x.data_ptr(), winograd_filter(L).data_ptr(), L.bias.data_ptr(),
+                                     _ptr(alpha if alpha is not None else L.alpha) if a == ACT_PRELU else None, a,
+                                     _ptr(residual), res_f32, _ptr(out16), _ptr(out32), B, H, W, Cin, ws.data_ptr(),
+                                     ws.numel(), _tune(tune), _stream()), "rn_conv2d_winograd")
+        return _ret(out16, out32, want16, want32, L.fmt)
     check(lib.rn_conv2d_same(x.data_ptr(), L.w.data_ptr(), L.bias.data_ptr(),
                              _ptr(alpha if alpha is not None else L.alpha) if a == ACT_PRELU else None, a, _ptr(residual), res_f32,
                              _ptr(out16), _ptr(out32), B, H, W, Cin, L.cout, L.cout_pad, L.ksize[0], L.ksize[1],

@@ -1,0 +1,101 @@
+#!/usr/bin/env python
+"""Time the exact-mode 3x3 C -> C trunk convolution at B = 24, 64 x 64 (res2: C = 1024, res3: C = 512) through the direct
+igemm kernel and the Winograd F(2x2, 3x3) path (rn_winograd.cu), alternated in one process: three rounds of 20 launches
+each, CUDA events; then each Winograd stage alone (input transform, the 16 per-position GEMMs at the default and at two K
+blocks per pipeline stage, output transform).  Prints the card's name, power limit and clocks, ms per launch, algorithmic
+TFLOP/s (2 * B*H*W * C * 9C per conv, the direct conv's MACs), issued TFLOP/s of the GEMM stage (3 products per MAC) and
+the transforms' GB/s from the bytes they must move, as JSON on stdout and, with --out, to a file.
+  python scripts/winograd_time.py [--launches 20] [--rounds 3] [--out FILE]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from rendernet_b200 import ops  # noqa: E402
+from rendernet_b200._lib import check, lib  # noqa: E402
+
+B, H, W = 24, 64, 64
+
+
+def card():
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    try:
+        return subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True,
+                              timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        return f"nvidia-smi unavailable: {e}"
+
+
+def timed(fn, launches):
+    fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(launches):
+        fn()
+    e1.record()
+    e1.synchronize()
+    return e0.elapsed_time(e1) / launches
+
+
+def one_width(C, launches, rounds):
+    g = torch.Generator().manual_seed(C)
+    x = ops.cast_to_16(((torch.rand(B, H, W, C, generator=g) * 2 - 1) * 3).to("cuda"), fmt=2)
+    w = (torch.rand(3, 3, C, C, generator=g) * 2 - 1) * (6.0 / (18 * C)) ** 0.5
+    al = torch.rand(C, generator=g) * 0.3
+    L = ops.pack_conv("conv2d", w, torch.zeros(C), al, device="cuda", fmt=2)
+    y = ops.conv2d(x, L, act="prelu")
+    on, off = dict(winograd=1), dict(winograd=-1)
+    arms = {"direct": lambda: ops.conv2d(x, L, act="prelu", out16=y, tune=off),
+            "winograd": lambda: ops.conv2d(x, L, act="prelu", out16=y, tune=on)}
+    times = {k: [] for k in arms}
+    for _ in range(rounds):
+        for k, fn in arms.items():
+            times[k].append(timed(fn, launches))
+    # stages alone, on a workspace of their own
+    U = ops.winograd_filter(L)
+    ws = torch.empty(lib.rn_winograd_workspace_bytes(B, H, W, C), device="cuda", dtype=torch.uint8)
+    pos = B * (H // 2) * (W // 2) * C
+    v = ws[:16 * pos * 4]
+    m = ws[16 * pos * 4:].view(torch.float32)
+    st = torch.cuda.current_stream().cuda_stream
+    stages = {
+        "in": lambda: check(lib.rn_winograd_in(x.data_ptr(), v.data_ptr(), B, H, W, C, st)),
+        "gemm": lambda: check(lib.rn_winograd_gemm(v.data_ptr(), U.data_ptr(), m.data_ptr(), B, H, W, C, None, st)),
+        "gemm_kps2": lambda: check(lib.rn_winograd_gemm(v.data_ptr(), U.data_ptr(), m.data_ptr(), B, H, W, C,
+                                                         ops._tune(dict(kps=2)), st)),
+        "out": lambda: check(lib.rn_winograd_out(m.data_ptr(), L.bias.data_ptr(), L.alpha.data_ptr(), 1, None, 0,
+                                                 y.planes.data_ptr(), None, B, H, W, C, st)),
+    }
+    st_ms = {k: min(timed(fn, launches) for _ in range(rounds)) for k, fn in stages.items()}
+    flop = 2.0 * B * H * W * C * 9 * C
+    issued_gemm = 3 * 2.0 * 16 * pos * C
+    act_bytes = B * H * W * C * 4                       # one hi/lo activation (two fp16 planes)
+    gbs = {"in": (act_bytes + 16 * pos * 4) / st_ms["in"] / 1e6,      # read x pair, write V pair
+           "out": (16 * pos * 4 + act_bytes) / st_ms["out"] / 1e6}    # read M fp32, write y pair (no residual here)
+    res = {"C": C, "direct_ms": times["direct"], "winograd_ms": times["winograd"], "stage_ms": st_ms,
+           "direct_tflops_alg": flop / min(times["direct"]) / 1e9, "winograd_tflops_alg": flop / min(times["winograd"]) / 1e9,
+           "gemm_tflops_issued": issued_gemm / min(st_ms["gemm"], st_ms["gemm_kps2"]) / 1e9, "transform_gbs": gbs}
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--launches", type=int, default=20)
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--out", type=str, default=None, help="also write the JSON result to this file")
+    a = ap.parse_args()
+    out = {"card": card(), "widths": [one_width(C, a.launches, a.rounds) for C in (1024, 512)], "card_after": card()}
+    print(json.dumps(out, indent=1))
+    if a.out:
+        with open(a.out, "w") as f:
+            json.dump(out, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
