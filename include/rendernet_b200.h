@@ -110,7 +110,9 @@ typedef struct rn_conv_desc {
   const int8_t* taps;       /* HOST pointer: ntaps x (dx, dy, dz) */
   const void* x;            /* 16-bit [B,H,W,(D),Cin] */
   const void* w_packed;     /* 16-bit [ntaps][cout_pad][Cin] */
-  const float* bias;        /* fp32 [cout_pad] */
+  const float* bias;        /* fp32 [cout_pad], or NULL: the raw fp32 sums, stored straight from the accumulators (out32
+                             * only, act none, no residual, Cout = cout_pad, 8-byte aligned rows; a kernel variant built for
+                             * it, today the exact-mode N = 256 one of rn_winograd_gemm, else an error) */
   const float* alpha;       /* fp32 [cout_pad] or NULL */
   int act;                  /* RN_ACT_* */
   const void* residual;     /* NULL, or same indexing as the output */
@@ -209,13 +211,14 @@ int rn_conv3d_sliced_plan(int B, int H, int W, int D, int fmt, int* out, int n_o
  * 2x2 output block instead of 36, and 16 accumulations of K = C instead of one of K = 9C.
  *   rn_winograd_in:   x [2][B,H,W,C] hi/lo -> V [2][16][B,H/2,W/2,C] hi/lo, V = B^T d B of every 4x4 input patch (SAME zero
  *                     padding), summed in fp32 from hi + lo and split once.
- *   rn_winograd_gemm: M [16][B,H/2,W/2,C] fp32 = V . U per position: one igemm launch (b_tap_div = B), no bias or activation.
+ *   rn_winograd_gemm: M [16][B,H/2,W/2,C] fp32 = V . U per position: one igemm launch (b_tap_div = B, bias NULL: the raw
+ *                     sums, stored straight from the accumulators), C a multiple of 256.
  *                     u [2][16][C][C] hi/lo: U = G g G^T of the filter per position, [position][Cout][Cin] (ops.winograd_filter).
  *   rn_winograd_out:  y = A^T M A of every 2x2 block, then bias, PReLU / none, the residual and the stores exactly as the
  *                     igemm epilogue does them (out16 hi/lo and/or out32).
  * rn_conv2d_winograd runs the three on `workspace` (rn_winograd_workspace_bytes(B, H, W, C) bytes: V then M).
  * rn_conv2d_winograd_eligible says whether ops.conv2d takes the Winograd path for a layer of this shape (fmt 2,
- * 3x3, H and W even, Cin = Cout = a multiple of 64 >= 1024, tune->winograd / RN_TUNE winograd not off; tune->winograd = 1
+ * 3x3, H and W even, Cin = Cout = a multiple of 256 >= 1024, tune->winograd / RN_TUNE winograd not off; tune->winograd = 1
  * also takes Cin < 1024).  Host-only. */
 long long rn_winograd_workspace_bytes(int B, int H, int W, int C);
 int rn_conv2d_winograd_eligible(int fmt, int kh, int kw, int H, int W, int Cin, int Cout, int cout_pad, const rn_tuning* tune);

@@ -28,16 +28,17 @@
 
 namespace rn {
 
-// launch_ms<BN, CL, MS, SPLIT, HALF> is defined in rn_igemm_kernel.cuh and explicitly instantiated once per variant
+// launch_ms<BN, CL, MS, SPLIT, HALF, RAW> is defined in rn_igemm_kernel.cuh and explicitly instantiated once per variant
 // (rn_igemm_inst.cu x the Makefile's VARIANTS list); this table must list exactly those variants.
-template <int BN, int CL, int MS, bool SPLIT, bool HALF>
+template <int BN, int CL, int MS, bool SPLIT, bool HALF, bool RAW>
 cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t stream);
 
-static cudaError_t launch_variant(int BN, int CL, int MS, int SP, int HF, const IgemmParams& p, int grid, size_t smem,
+static cudaError_t launch_variant(int BN, int CL, int MS, int SP, int HF, int RW, const IgemmParams& p, int grid, size_t smem,
                                   cudaStream_t stream) {
-#define RN_V(bn, cl, ms, sp, hf) \
-  if (BN == bn && CL == cl && MS == ms && SP == sp && HF == hf) \
-    return launch_ms<bn, cl, ms, (sp != 0), (hf != 0)>(p, grid, smem, stream);
+#define RN_V(bn, cl, ms, sp, hf) RN_VR(bn, cl, ms, sp, hf, 0)
+#define RN_VR(bn, cl, ms, sp, hf, rw) \
+  if (BN == bn && CL == cl && MS == ms && SP == sp && HF == hf && RW == rw) \
+    return launch_ms<bn, cl, ms, (sp != 0), (hf != 0), (rw != 0)>(p, grid, smem, stream);
   RN_V(256, 1, 1, 0, 0) RN_V(256, 2, 1, 0, 0) RN_V(256, 4, 1, 0, 0)
   RN_V(128, 1, 1, 0, 0) RN_V(128, 2, 1, 0, 0) RN_V(128, 4, 1, 0, 0) RN_V(128, 1, 2, 0, 0) RN_V(128, 2, 2, 0, 0) RN_V(128, 4, 2, 0, 0)
   RN_V(64, 1, 1, 0, 0) RN_V(64, 1, 2, 0, 0) RN_V(32, 1, 1, 0, 0) RN_V(32, 1, 2, 0, 0) RN_V(16, 1, 1, 0, 0) RN_V(16, 1, 2, 0, 0)
@@ -47,7 +48,10 @@ static cudaError_t launch_variant(int BN, int CL, int MS, int SP, int HF, const 
   // banded filters (N tile 128) with half-tile K blocks
   RN_V(128, 1, 1, 0, 1) RN_V(128, 2, 1, 0, 1) RN_V(128, 4, 1, 0, 1) RN_V(128, 1, 2, 0, 1) RN_V(128, 2, 2, 0, 1)
   RN_V(128, 4, 2, 0, 1) RN_V(128, 1, 1, 1, 1) RN_V(128, 1, 2, 1, 1)
+  // raw fp32 output (no bias): the exact-mode Winograd per-position GEMM
+  RN_VR(256, 1, 1, 1, 0, 1)
 #undef RN_V
+#undef RN_VR
   return cudaErrorInvalidDeviceFunction;   // plan_conv chose a variant that is not built
 }
 
@@ -128,6 +132,7 @@ extern "C" long long rn_launch_count(void) { return rn::g_launch_count.load(std:
 namespace rn {
 struct ConvPlan {
   int BN, CL, grid, sub, KB, D;
+  bool raw;   // no bias: plain fp32 output stored straight from the accumulators (no staging panel)
   size_t smem;
 };
 
@@ -135,7 +140,12 @@ struct ConvPlan {
 // size, pipeline depth, shared-memory size.  Pure host arithmetic on the
 // descriptor (pointers are only tested for null / alignment), so rn_conv_plan can report it on a machine without a GPU.
 static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
-  if (d == nullptr || d->x == nullptr || d->w_packed == nullptr || d->bias == nullptr) return -1;
+  if (d == nullptr || d->x == nullptr || d->w_packed == nullptr) return -1;
+  // bias == NULL: raw fp32 output, the accumulators as they are (only out32, every column a real one)
+  const bool raw = d->bias == nullptr;
+  if (raw && (d->act != ACT_NONE || d->residual != nullptr || d->out16 != nullptr || d->out32 == nullptr ||
+              d->phong != nullptr || d->o_nsplit != 0 || d->Cout != d->cout_pad))
+    return -24;
   if (d->ndim != 2 && d->ndim != 3) return -2;
   if (d->ntaps < 1 || d->ntaps * (d->fmt == 2 ? 3 : 1) > kMaxTaps) return -3;
   if (d->fmt < 0 || d->fmt > 2) return -17;
@@ -207,7 +217,8 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
   int want_ms = d->msub > 0 ? d->msub : (tn.msub > 0 ? tn.msub : 2);
   if (want_ms > 2) return -16;
   if (BN > 128 || d->ndim != 2) want_ms = 1;
-  const int budget = kMaxSmem - 1024 - 256 - kStgBytes;
+  const int stg_bytes = raw ? 0 : kStgBytes;   // the epilogue's staging panel
+  const int budget = kMaxSmem - 1024 - 256 - stg_bytes;
   for (int attempt = 0; attempt < 3; ++attempt) {
     p.ms = want_ms;
     int rem = kTileM;
@@ -291,8 +302,8 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
       }
     }
   }
-  pl.BN = BN; pl.CL = CL; pl.grid = grid; pl.sub = sub; pl.KB = KB; pl.D = D;
-  pl.smem = static_cast<size_t>(p.stages) * p.kps * sub + 1024 + 256 + kStgBytes;
+  pl.BN = BN; pl.CL = CL; pl.grid = grid; pl.sub = sub; pl.KB = KB; pl.D = D; pl.raw = raw;
+  pl.smem = static_cast<size_t>(p.stages) * p.kps * sub + 1024 + 256 + stg_bytes;
   return 0;
 }
 }  // namespace rn
@@ -392,7 +403,8 @@ extern "C" int rn_conv_igemm(const rn_conv_desc* d, void* stream_v) {
                         (d->o_z % 8 == 0);
   auto al16 = [](const void* q) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   p.vec_ok = strides8 && al16(d->out16) && al16(d->out32) && al16(d->residual) ? 1 : 0;
+  if (pl.raw && !p.vec_ok) return -24;    // the raw epilogue stores float2 pairs without a scalar fallback
 
-  const cudaError_t e = launch_variant(BN, CL, p.ms, p.split, p.band_half, p, grid, smem, stream);
+  const cudaError_t e = launch_variant(BN, CL, p.ms, p.split, p.band_half, pl.raw ? 1 : 0, p, grid, smem, stream);
   return e == cudaSuccess ? 0 : static_cast<int>(e);
 }

@@ -17,7 +17,7 @@
 //     CTAs share the same activation rows in L2.  The producer runs ahead into the next tile while the consumers drain.
 //
 // This header holds the device code and the per-variant launcher template `launch_ms`.  It is included by rn_igemm_inst.cu,
-// which the Makefile compiles once per <BN, CL, MS, SPLIT, HALF> variant (one object each, so that `make -j` spreads them
+// which the Makefile compiles once per <BN, CL, MS, SPLIT, HALF, RAW> variant (one object each, so that `make -j` spreads them
 // over the cores), and by rn_conv3d_sliced.cu, whose kernel shares `epilogue_chunk`; rn_igemm.cu (host side: validation,
 // tile/pipeline sizing, tensor maps) declares the template and dispatches to the instantiated variants.
 #pragma once
@@ -229,7 +229,10 @@ __device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const float
 // HALF = banded filter with half-tile K blocks (IgemmParams::band_half): the accumulator is kept as two N = BN/2 halves in
 // separate register arrays, and an edge K block issues only the MMAs of the half it feeds.  (Selecting the MMA width at run
 // time on one array makes ptxas serialise every wgmma of the kernel, so the other kernels do not carry this path.)
-template <int BN, int CL, int MS, bool SPLIT, bool HALF>
+// RAW = plain fp32 output (no bias, activation, residual or 16-bit planes; the Winograd per-position GEMM): every consumer
+// thread stores its own accumulator fragments, without the staging panel and its barriers, and goes straight on to the
+// next tile's MMAs.
+template <int BN, int CL, int MS, bool SPLIT, bool HALF, bool RAW>
 __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
   static_assert(MS == 1 || (MS == 2 && BN <= 128), "two accumulators per tile need 2 x BN/2 <= 128 registers per thread");
   constexpr int NP = HALF ? 2 : 1;                             // accumulator parts per M sub-tile
@@ -247,7 +250,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
   const int stage_bytes = p.kps * sub_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + static_cast<size_t>(p.stages) * stage_bytes);
   uint64_t* empty_bar = full_bar + p.stages;
-  float* stg_all = reinterpret_cast<float*>(smem + static_cast<size_t>(p.stages) * stage_bytes + 256);
+  float* stg_all = reinterpret_cast<float*>(smem + static_cast<size_t>(p.stages) * stage_bytes + 256);   // !RAW only
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA);
@@ -375,6 +378,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
     const int xl = (m / p.BD) % p.BW;
     const int yl = m / (p.BD * p.BW);
     const int bar_id = 1 + wg;
+    uint64_t pol = 0;
+    if constexpr (RAW) pol = l2_policy_evict_first();
     float acc[MS][NP][NACC];
     int stage = 0;
     uint32_t phase = 0;
@@ -447,8 +452,30 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
       }
       wgmma_wait<0>();
       release(prev);
-      // epilogue: accumulator fragments -> staging panel (SC columns at a time) -> one row per thread -> epilogue_chunk
       const TileCoord t = decode_tile(p, tile_of(ct), BN);
+      if constexpr (RAW) {
+        // rows fr and fr + 8 of every M sub-tile straight from the fragments: one float2 (columns fc, fc + 1) per 8-column
+        // block, so a warp store fills 8 whole 32-byte sectors.  The output is read once, by the next kernel: evict-first
+        // keeps it from pushing the operand tiles that the co-running CTAs share out of L2.
+#pragma unroll
+        for (int s = 0; s < MS; ++s) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int mr = 64 * wg + fr + 8 * h;    // row of the M sub-tile (recomputed: nothing extra stays live in the MMA loop)
+            const int x = t.x0 + (mr / p.BD) % p.BW, y = t.y0 + s * p.BH + mr / (p.BD * p.BW), z = t.z0 + mr % p.BD;
+            if (x < p.W && y < p.H && z < p.D) {
+              float* o = p.out32 + (p.o_base + t.b * p.o_b + y * p.o_y + x * p.o_x + z * p.o_z + t.n0 + fc);
+#pragma unroll
+              for (int j = 0; j < BN / 8; ++j) {
+                const float* d = acc[s][j / JP] + 4 * (j % JP) + 2 * h;
+                st_global_v2_hint(o + 8 * j, d[0], d[1], pol);
+              }
+            }
+          }
+        }
+        continue;                                   // no barrier: the next tile's first MMAs overwrite acc after wgmma_fence
+      }
+      // epilogue: accumulator fragments -> staging panel (SC columns at a time) -> one row per thread -> epilogue_chunk
       const int x = t.x0 + xl, z = t.z0 + zl;
 #pragma unroll
       for (int s = 0; s < MS; ++s) {
@@ -489,7 +516,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
 
 // One explicit instantiation per kernel variant lives in its own object file (rn_igemm_inst.cu compiled with
 // -DRN_BN=.. etc., see the Makefile's VARIANTS list); rn_igemm.cu holds the matching dispatch table.
-template <int BN, int CL, int MS, bool SPLIT, bool HALF>
+template <int BN, int CL, int MS, bool SPLIT, bool HALF, bool RAW>
 cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t stream) {
   // cudaFuncSetAttribute is per DEVICE (and per kernel variant): one flag per device ordinal
   static std::atomic<bool> attr_set[kMaxDevices];
@@ -497,7 +524,7 @@ cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t 
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
   if (!attr_set[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(igemm_kernel<BN, CL, MS, SPLIT, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    cudaError_t e = cudaFuncSetAttribute(igemm_kernel<BN, CL, MS, SPLIT, HALF, RAW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e != cudaSuccess) return e;
     attr_set[dev].store(true, std::memory_order_release);
   }
@@ -524,7 +551,7 @@ cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t 
   }
   cfg.attrs = attr;
   cfg.numAttrs = na;
-  return cudaLaunchKernelEx(&cfg, igemm_kernel<BN, CL, MS, SPLIT, HALF>, p);
+  return cudaLaunchKernelEx(&cfg, igemm_kernel<BN, CL, MS, SPLIT, HALF, RAW>, p);
 }
 
 }  // namespace rn

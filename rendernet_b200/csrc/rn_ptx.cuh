@@ -115,6 +115,16 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// ------------------------------------------------------------------ global stores with an L2 eviction-priority hint
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ void st_global_v2_hint(float* p, float a, float b, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.v2.f32 [%0], {%1, %2}, %3;" ::"l"(p), "f"(a), "f"(b), "l"(pol) : "memory");
+}
+
 // ------------------------------------------------------------------ cluster
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;

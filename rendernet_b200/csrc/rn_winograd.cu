@@ -10,7 +10,7 @@
 //     [16][B,H/2,W/2,C];
 //   * the 16 GEMMs as ONE igemm launch of a 1x1 conv over V viewed as [16*B, H/2, W/2, C] whose image b reads filter "tap"
 //     b / B (IgemmParams::b_tap_div) of U = G g G^T, packed [16][Cout][Cin] (ops.winograd_filter); exact-mode pseudo-tap
-//     order, raw fp32 output M, no bias;
+//     order, raw fp32 output M (the igemm variant without bias that stores straight from its accumulators);
 //   * winograd_out_kernel: A^T M A in fp32, then the igemm epilogue itself (epilogue_chunk: bias, PReLU, residual, hi/lo and
 //     fp32 stores, one rounding).
 // The transforms only use 0, +-1 and +-1/2, so they add a few fp32 roundings and no cancellation-prone coefficients.
@@ -22,9 +22,7 @@
 namespace rn {
 
 constexpr int kWinoMinC = 1024;   // smallest C routed to Winograd (res2 trunk; scripts/winograd_time.py times 512 as well)
-constexpr int kWinoMaxC = 4096;   // size of the zero bias the GEMM stage adds
-
-__device__ const float g_wino_zero_bias[kWinoMaxC] = {};
+constexpr int kWinoGemmN = 256;   // N tile of the per-position GEMM: its raw-output igemm variant is built for this one only
 
 __device__ __forceinline__ void load8(const uint16_t* __restrict__ hi, long long plane, long long off, float* v) {
   const uint4 h = __ldg(reinterpret_cast<const uint4*>(hi + off));
@@ -161,7 +159,7 @@ static int wino_grid(long long n) {
 }
 
 static bool wino_shape_ok(int B, int H, int W, int C) {
-  return B >= 1 && H >= 2 && W >= 2 && H % 2 == 0 && W % 2 == 0 && C % 64 == 0 && C <= kWinoMaxC;
+  return B >= 1 && H >= 2 && W >= 2 && H % 2 == 0 && W % 2 == 0 && C % 64 == 0;
 }
 
 }  // namespace rn
@@ -180,7 +178,7 @@ extern "C" int rn_conv2d_winograd_eligible(int fmt, int kh, int kw, int H, int W
   const bool forced = tune != nullptr && tune->winograd > 0;
   const bool on = forced || (tune != nullptr && tune->winograd < 0 ? false : tuning().winograd != 0);
   return on && fmt == 2 && kh == 3 && kw == 3 && Cin == Cout && Cout == cout_pad && (forced || Cin >= kWinoMinC) &&
-         wino_shape_ok(1, H, W, Cin);
+         Cin % kWinoGemmN == 0 && wino_shape_ok(1, H, W, Cin);
 }
 
 extern "C" int rn_winograd_in(const void* x, void* v, int B, int H, int W, int C, void* stream) {
@@ -194,22 +192,20 @@ extern "C" int rn_winograd_in(const void* x, void* v, int B, int H, int W, int C
 
 extern "C" int rn_winograd_gemm(const void* v, const void* u, float* m, int B, int H, int W, int C, const rn_tuning* tune,
                                 void* stream) {
-  if (v == nullptr || u == nullptr || m == nullptr || !wino_shape_ok(B, H, W, C)) return -1;
-  void* zero = nullptr;
-  cudaError_t e = cudaGetSymbolAddress(&zero, g_wino_zero_bias);
-  if (e != cudaSuccess) return static_cast<int>(e);
+  if (v == nullptr || u == nullptr || m == nullptr || !wino_shape_ok(B, H, W, C) || C % kWinoGemmN != 0) return -1;
   const int8_t tap[3] = {0, 0, 0};
   const int H2 = H / 2, W2 = W / 2;
   rn_conv_desc d;
   memset(&d, 0, sizeof(d));
   d.ndim = 2; d.B = 16 * B; d.H = H2; d.W = W2; d.D = 1; d.Cin = C; d.Cout = C; d.cout_pad = C;
-  d.ntaps = 1; d.taps = tap; d.x = v; d.w_packed = u; d.bias = static_cast<const float*>(zero); d.alpha = nullptr; d.act = ACT_NONE;
+  d.ntaps = 1; d.taps = tap; d.x = v; d.w_packed = u; d.bias = nullptr; d.alpha = nullptr; d.act = ACT_NONE;
   d.out32 = m;
   d.o_x = C; d.o_y = static_cast<long long>(W2) * C; d.o_b = static_cast<long long>(H2) * W2 * C;
   d.fmt = 2;
   d.x_plane = 16LL * B * H2 * W2 * C;
   d.w_plane = 16LL * C * C;
   d.b_tap_div = B;
+  d.force_bn = kWinoGemmN;
   if (tune != nullptr) { d.force_kps = tune->kps; d.msub = tune->msub; }
   return rn_conv_igemm(&d, stream);
 }

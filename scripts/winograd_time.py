@@ -3,8 +3,9 @@
 igemm kernel and the Winograd F(2x2, 3x3) path (rn_winograd.cu), alternated in one process: three rounds of 20 launches
 each, CUDA events; then each Winograd stage alone (input transform, the 16 per-position GEMMs at the default and at two K
 blocks per pipeline stage, output transform).  Prints the card's name, power limit and clocks, ms per launch, algorithmic
-TFLOP/s (2 * B*H*W * C * 9C per conv, the direct conv's MACs), issued TFLOP/s of the GEMM stage (3 products per MAC) and
-the transforms' GB/s from the bytes they must move, as JSON on stdout and, with --out, to a file.
+TFLOP/s (2 * B*H*W * C * 9C per conv, the direct conv's MACs), issued TFLOP/s of the GEMM stage (3 products per MAC), its
+time per 128 x 256 tile on one SM (tiles / SMs run one after another on each SM) and the transforms' GB/s from the bytes they
+must move, as JSON on stdout and, with --out, to a file.
   python scripts/winograd_time.py [--launches 20] [--rounds 3] [--out FILE]"""
 import argparse
 import json
@@ -75,12 +76,16 @@ def one_width(C, launches, rounds):
     st_ms = {k: min(timed(fn, launches) for _ in range(rounds)) for k, fn in stages.items()}
     flop = 2.0 * B * H * W * C * 9 * C
     issued_gemm = 3 * 2.0 * 16 * pos * C
+    gemm_ms = min(st_ms["gemm"], st_ms["gemm_kps2"])
+    tiles = 16 * pos // 128 // 256                      # 128-row x 256-column tiles of the one GEMM launch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
     act_bytes = B * H * W * C * 4                       # one hi/lo activation (two fp16 planes)
     gbs = {"in": (act_bytes + 16 * pos * 4) / st_ms["in"] / 1e6,      # read x pair, write V pair
            "out": (16 * pos * 4 + act_bytes) / st_ms["out"] / 1e6}    # read M fp32, write y pair (no residual here)
     res = {"C": C, "direct_ms": times["direct"], "winograd_ms": times["winograd"], "stage_ms": st_ms,
            "direct_tflops_alg": flop / min(times["direct"]) / 1e9, "winograd_tflops_alg": flop / min(times["winograd"]) / 1e9,
-           "gemm_tflops_issued": issued_gemm / min(st_ms["gemm"], st_ms["gemm_kps2"]) / 1e9, "transform_gbs": gbs}
+           "gemm_tflops_issued": issued_gemm / gemm_ms / 1e9, "gemm_tiles": tiles,
+           "gemm_us_per_tile": gemm_ms * 1e3 / (tiles / sms), "transform_gbs": gbs}
     return res
 
 
