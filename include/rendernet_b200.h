@@ -160,6 +160,8 @@ int rn_conv_igemm(const rn_conv_desc* d, void* stream);
 typedef struct rn_tuning {
   int cluster, cta_group, kps, msub, epilogue_groups, res_prefetch, tma_store, yhalo;
   int winograd;             /* rn_conv2d_winograd_eligible: 1 = on, -1 = off (the direct kernel), 0 = default (RN_TUNE) */
+  int wino_tile;            /* rn_conv2d_winograd_tile: 4 = F(4x4, 3x3) where H, W % 4 == 0, 2 = F(2x2, 3x3), 0 = default
+                             * (RN_TUNE wino_tile, else 4) */
 } rn_tuning;
 /* The launch plan rn_conv_igemm would use for `d`, without touching the device (works on a host without a GPU; the SM
  * count then defaults to 132).  Pointers in `d` are only tested for null / 16-byte alignment.  out[0..n_out) receives
@@ -229,6 +231,26 @@ int rn_winograd_out(const float* m, const float* bias, const float* alpha, int a
 int rn_conv2d_winograd(const void* x, const void* u, const float* bias, const float* alpha, int act, const void* residual,
                        int residual_is_f32, void* out16, float* out32, int B, int H, int W, int C, void* workspace,
                        long long workspace_bytes, const rn_tuning* tune, void* stream);
+
+/* The same convolution as Winograd F(4x4, 3x3): 36 products per 4x4 output block (2.25 per pixel instead of 4), V and M
+ * 2.25x the activation instead of 4x.  Interpolation points 0, +-1, +-1/2, infinity; powers of two keep V and U in range
+ * without adding a rounding (rn_winograd.cu).  H and W multiples of 4.
+ *   rn_winograd4_in:   x [2][B,H,W,C] hi/lo -> V [2][36][B,H/4,W/4,C] hi/lo, V = 1/2 B^T d B of every 6x6 input patch.
+ *   rn_winograd4_gemm: M [36][B,H/4,W/4,C] fp32 = V . U per position, one igemm launch as rn_winograd_gemm;
+ *                      u [2][36][C][C] hi/lo: U = 2^u_exp G g G^T, [position][Cout][Cin] (ops.winograd_filter(L, 4)).
+ *   rn_winograd4_out:  y = 2^(1 - u_exp) A^T M A of every 4x4 block (|u_exp| <= 100), then the igemm epilogue.
+ * rn_conv2d_winograd4 runs the three on `workspace` (rn_winograd4_workspace_bytes(B, H, W, C) bytes: V then M).
+ * rn_conv2d_winograd_tile: 0 where rn_conv2d_winograd_eligible says no, else the output tile ops.conv2d runs: 4 where H and W
+ * are multiples of 4 and tune->wino_tile / RN_TUNE wino_tile is not 2, else 2.  Host-only. */
+int rn_conv2d_winograd_tile(int fmt, int kh, int kw, int H, int W, int Cin, int Cout, int cout_pad, const rn_tuning* tune);
+long long rn_winograd4_workspace_bytes(int B, int H, int W, int C);
+int rn_winograd4_in(const void* x, void* v, int B, int H, int W, int C, void* stream);
+int rn_winograd4_gemm(const void* v, const void* u, float* m, int B, int H, int W, int C, const rn_tuning* tune, void* stream);
+int rn_winograd4_out(const float* m, const float* bias, const float* alpha, int act, const void* residual, int residual_is_f32,
+                     void* out16, float* out32, int B, int H, int W, int C, int u_exp, void* stream);
+int rn_conv2d_winograd4(const void* x, const void* u, int u_exp, const float* bias, const float* alpha, int act,
+                        const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W, int C,
+                        void* workspace, long long workspace_bytes, const rn_tuning* tune, void* stream);
 
 /* slim.conv2d_transpose / layer_util.conv2d_transpose (layer_util.py:186; RenderNet_Shader.py:106-129),
  * SAME, out = in*stride.  w_packed holds the stride^2 phase filters back to back, as produced by

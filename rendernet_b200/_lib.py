@@ -40,7 +40,7 @@ class rn_phong(C.Structure):
 
 class rn_tuning(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("cluster", "cta_group", "kps", "msub", "epilogue_groups", "res_prefetch", "tma_store", "yhalo",
-                                       "winograd")]
+                                       "winograd", "wino_tile")]
 
 
 _vp, _i, _f, _ll = C.c_void_p, C.c_int, C.c_float, C.c_longlong
@@ -77,6 +77,12 @@ SIGNATURES = {
     "rn_winograd_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _tp, _vp]),
     "rn_winograd_out": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp]),
     "rn_conv2d_winograd": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _ll, _tp, _vp]),
+    "rn_conv2d_winograd_tile": (_i, [_i] * 8 + [_tp]),
+    "rn_winograd4_workspace_bytes": (_ll, [_i, _i, _i, _i]),
+    "rn_winograd4_in": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "rn_winograd4_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _tp, _vp]),
+    "rn_winograd4_out": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "rn_conv2d_winograd4": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _ll, _tp, _vp]),
     "rn_pack_conv2d_transpose_weights": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "rn_conv2d_transpose_same": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _tp, _vp]),
     "rn_pack_conv2d_transpose_s2_merged": (_i, [_vp, _vp, _i, _i, _i, _vp]),

@@ -96,6 +96,8 @@ static Tuning parse_tuning() {
   get("tiled_tex_conv", &t.tiled_tex_conv, 0, 1);
   get("pdl", &t.pdl, 0, 1);
   get("winograd", &t.winograd, 0, 1);
+  get("wino_tile", &t.wino_tile, 2, 4);
+  if (t.wino_tile != 2) t.wino_tile = 4;
   return t;
 }
 const Tuning& tuning() {

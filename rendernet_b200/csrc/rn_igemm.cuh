@@ -122,6 +122,7 @@ struct Tuning {
   int pdl = 0;            // programmatic dependent launch: igemm launches carry the programmatic-stream-serialization attribute,
                           // trigger their dependents after the prologue and griddepcontrol.wait before touching global memory
   int winograd = 1;       // exact-mode 3x3 trunk convs as Winograd F(2x2, 3x3) (rn_winograd.cu; 0: the direct kernel, for A/B)
+  int wino_tile = 4;      // Winograd output tile: 4 = F(4x4, 3x3) where H and W are multiples of 4, 2 = always F(2x2, 3x3)
 };
 const Tuning& tuning();
 

@@ -202,10 +202,11 @@ class PackedConv:
     dtype: torch.dtype
     fmt: int = 0                   # RN_FMT_*: 0 fp16, 1 bf16, 2 fp16 hi/lo pairs (w then holds [2][...])
     # exact-mode 3x3 C -> C convs: the fp32 filter the Winograd filter U is made from on first use (winograd_filter), the
-    # version it had when w was packed, and U itself.  U lives and dies with this object, so a re-pack drops it with w.
+    # version it had when w was packed, and U itself: {output tile (2 or 4): (U hi/lo planes, power-of-two exponent of U)}.
+    # U lives and dies with this object, so a re-pack drops it with w.
     master: Optional[torch.Tensor] = None
     master_version: int = 0
-    wino: Optional[torch.Tensor] = None
+    wino: Optional[dict] = None
 
 
 def _pad_vec(v: Optional[torch.Tensor], n: int, n_pad: int, device) -> Optional[torch.Tensor]:
@@ -267,12 +268,67 @@ def winograd_filter_f32(w_tf: torch.Tensor) -> torch.Tensor:
     return U.reshape(16, w.shape[3], w.shape[2]).float().contiguous()
 
 
-def winograd_filter(L: PackedConv) -> torch.Tensor:
-    """U of an exact-mode 3x3 layer as fp16 hi/lo planes [2][16][Cout][Cin], made on first use (an engine's warm-up, before
-    graph capture) from the filter L was packed from."""
+# finite interpolation points of F(4x4, 3x3) (infinity is the sixth): with these V stays within 4.5 |x|, where the textbook
+# 0, +-1, +-2 grow it to 42 |x| (DESIGN.md §4)
+WINO4_POINTS = (0.0, 1.0, -1.0, 0.5, -0.5)
+
+
+def wino4_matrices(p=WINO4_POINTS):
+    """(B^T [6,6], G [6,3], A^T [4,6]) of F(4x4, 3x3) in float64, derived from five finite points p (Toom-Cook: row j of B^T
+    holds the coefficients of prod_{l != j} (x - p_l), G[j] = p_j^k / prod_{l != j} (p_j - p_l), A^T[i][j] = p_j^i; the point
+    at infinity adds the last row of B^T and G and the last column of A^T)."""
+    import numpy as np
+    n = len(p) + 1
+    BT, Gm, AT = np.zeros((n, n)), np.zeros((n, 3)), np.zeros((4, n))
+    for j in range(n):
+        roots = [q for l, q in enumerate(p) if l != j]                 # j = n-1 (infinity): every finite point
+        BT[j, :len(roots) + 1] = np.polynomial.polynomial.polyfromroots(roots) if roots else [1.0]
+        if j < n - 1:
+            Gm[j] = [p[j] ** k / np.prod([p[j] - q for q in roots]) for k in range(3)]
+            AT[:, j] = [p[j] ** i for i in range(4)]
+    Gm[n - 1, 2] = 1.0
+    AT[3, n - 1] = 1.0
+    return BT, Gm, AT
+
+
+def wino4_exponent(u_max: float) -> int:
+    """Power-of-two exponent s of the F(4x4) filter: max |2^s G g G^T| lands in (2^11, 2^12], so the lo halves of the
+    trunk's small filter values stay out of fp16's subnormals and the hi halves far from its range limit."""
+    if not u_max > 0.0:
+        return 0
+    m, e = math.frexp(u_max)                                           # u_max = m 2^e, m in [1/2, 1)
+    return max(-100, min(100, (13 if m == 0.5 else 12) - e))
+
+
+def winograd4_filter_f32(w_tf: torch.Tensor):
+    """Winograd F(4x4, 3x3) filter transform U = 2^s G g G^T of a TF 3x3 filter [3,3,Cin,Cout], computed in float64 and rounded
+    once: (fp32 [36 = (row, column) of the 6x6 tile][Cout][Cin], s) with s = wino4_exponent(max |G g G^T|)."""
+    w = w_tf.detach().to(torch.float64)
+    G = torch.from_numpy(wino4_matrices()[1]).to(w.device)
+    U = torch.einsum("ak,klio,bl->aboi", G, w, G)
+    s = wino4_exponent(float(U.abs().max()) if U.numel() else 0.0)
+    return (U * 2.0 ** s).reshape(36, w.shape[3], w.shape[2]).float().contiguous(), s   # a power of two: exact in float64
+
+
+def winograd_filter_exp(L: PackedConv, tile: int = 2):
+    """(U as fp16 hi/lo planes [2][tile+2 squared][Cout][Cin], its power-of-two exponent: 0 for F(2x2)) of an exact-mode 3x3
+    layer, made on first use (an engine's warm-up, before graph capture) from the filter L was packed from."""
     if L.wino is None:
-        L.wino = cast_to_16(winograd_filter_f32(L.master), fmt=2).planes
-    return L.wino
+        L.wino = {}
+    if tile not in L.wino:
+        if tile == 2:
+            U, s = winograd_filter_f32(L.master), 0
+        elif tile == 4:
+            U, s = winograd4_filter_f32(L.master)
+        else:
+            raise ValueError(f"Winograd output tile {tile}: 2 or 4")
+        L.wino[tile] = (cast_to_16(U, fmt=2).planes, s)
+    return L.wino[tile]
+
+
+def winograd_filter(L: PackedConv, tile: int = 2) -> torch.Tensor:
+    """U of an exact-mode 3x3 layer as fp16 hi/lo planes [2][16 or 36][Cout][Cin] (winograd_filter_exp)."""
+    return winograd_filter_exp(L, tile)[0]
 
 
 def _out_buffers(shape, dtype, device, want16, want32, out16, out32, fmt: int = 0):
@@ -317,15 +373,23 @@ def conv2d(x: torch.Tensor, L: PackedConv, act: Optional[str] = None, residual: 
         assert tuple(residual.shape[-4:]) == (B, H, W, L.cout)
     a = _ACT[act]
     kh, kw = L.ksize
-    if L.master is not None and lib.rn_conv2d_winograd_eligible(L.fmt, kh, kw, H, W, Cin, L.cout, L.cout_pad, _tune(tune)):
+    tile = lib.rn_conv2d_winograd_tile(L.fmt, kh, kw, H, W, Cin, L.cout, L.cout_pad, _tune(tune)) if L.master is not None else 0
+    if tile:
         if L.master._version != L.master_version:
             raise RuntimeError("the filter changed after it was packed: re-pack the layer (pack_conv) before running it")
+        U, s = winograd_filter_exp(L, tile)
+        al = _ptr(alpha if alpha is not None else L.alpha) if a == ACT_PRELU else None
         # the caching allocator hands the same workspace block to every trunk layer in turn (also inside a graph capture)
-        ws = torch.empty(lib.rn_winograd_workspace_bytes(B, H, W, Cin), device=x.device, dtype=torch.uint8)
-        check(lib.rn_conv2d_winograd(x.data_ptr(), winograd_filter(L).data_ptr(), L.bias.data_ptr(),
-                                     _ptr(alpha if alpha is not None else L.alpha) if a == ACT_PRELU else None, a,
-                                     _ptr(residual), res_f32, _ptr(out16), _ptr(out32), B, H, W, Cin, ws.data_ptr(),
-                                     ws.numel(), _tune(tune), _stream()), "rn_conv2d_winograd")
+        if tile == 4:
+            ws = torch.empty(lib.rn_winograd4_workspace_bytes(B, H, W, Cin), device=x.device, dtype=torch.uint8)
+            check(lib.rn_conv2d_winograd4(x.data_ptr(), U.data_ptr(), s, L.bias.data_ptr(), al, a, _ptr(residual), res_f32,
+                                          _ptr(out16), _ptr(out32), B, H, W, Cin, ws.data_ptr(), ws.numel(), _tune(tune),
+                                          _stream()), "rn_conv2d_winograd4")
+        else:
+            ws = torch.empty(lib.rn_winograd_workspace_bytes(B, H, W, Cin), device=x.device, dtype=torch.uint8)
+            check(lib.rn_conv2d_winograd(x.data_ptr(), U.data_ptr(), L.bias.data_ptr(), al, a, _ptr(residual), res_f32,
+                                         _ptr(out16), _ptr(out32), B, H, W, Cin, ws.data_ptr(), ws.numel(), _tune(tune),
+                                         _stream()), "rn_conv2d_winograd")
         return _ret(out16, out32, want16, want32, L.fmt)
     check(lib.rn_conv2d_same(x.data_ptr(), L.w.data_ptr(), L.bias.data_ptr(),
                              _ptr(alpha if alpha is not None else L.alpha) if a == ACT_PRELU else None, a, _ptr(residual), res_f32,

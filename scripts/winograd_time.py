@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """Time the exact-mode 3x3 C -> C trunk convolution at B = 24, 64 x 64 (res2: C = 1024, res3: C = 512) through the direct
-igemm kernel and the Winograd F(2x2, 3x3) path (rn_winograd.cu), alternated in one process: three rounds of 20 launches
-each, CUDA events; then each Winograd stage alone (input transform, the 16 per-position GEMMs at the default and at two K
-blocks per pipeline stage, output transform).  Prints the card's name, power limit and clocks, ms per launch, algorithmic
-TFLOP/s (2 * B*H*W * C * 9C per conv, the direct conv's MACs), issued TFLOP/s of the GEMM stage (3 products per MAC), its
-time per 128 x 256 tile on one SM (tiles / SMs run one after another on each SM) and the transforms' GB/s from the bytes they
-must move, as JSON on stdout and, with --out, to a file.
+igemm kernel and the Winograd F(2x2, 3x3) and F(4x4, 3x3) paths (rn_winograd.cu), alternated in one process: three rounds
+of 20 launches each, CUDA events; then each Winograd stage of both tiles alone (input transform, the 16 or 36 per-position
+GEMMs at the default and at two K blocks per pipeline stage, output transform).  Prints the card's name, power limit and
+clocks, ms per launch, algorithmic TFLOP/s (2 * B*H*W * C * 9C per conv, the direct conv's MACs), issued TFLOP/s of the GEMM
+stage (3 products per MAC), its time per 128 x 256 tile on one SM (tiles / SMs run one after another on each SM) and the
+transforms' GB/s from the bytes they must move, as JSON on stdout and, with --out, to a file.
   python scripts/winograd_time.py [--launches 20] [--rounds 3] [--out FILE]"""
 import argparse
 import json
@@ -44,6 +44,38 @@ def timed(fn, launches):
     return e0.elapsed_time(e1) / launches
 
 
+def _stages(tile, L, x, y, C, launches, rounds):
+    """Each stage of one Winograd tile alone, on a workspace of its own: ms per launch, the GEMM's issued TFLOP/s and time per
+    128 x 256 tile on one SM (tiles / SMs run one after another on each SM), and the transforms' GB/s from the bytes they must
+    move."""
+    n = (tile + 2) ** 2                                 # positions of the tile
+    U, s = ops.winograd_filter_exp(L, tile)
+    sfx = "" if tile == 2 else "4"
+    ws = torch.empty(getattr(lib, f"rn_winograd{sfx}_workspace_bytes")(B, H, W, C), device="cuda", dtype=torch.uint8)
+    pos = B * (H // tile) * (W // tile) * C
+    v = ws[:n * pos * 4]
+    m = ws[n * pos * 4:].view(torch.float32)
+    st = torch.cuda.current_stream().cuda_stream
+    f_in, f_gemm = getattr(lib, f"rn_winograd{sfx}_in"), getattr(lib, f"rn_winograd{sfx}_gemm")
+    out_args = (m.data_ptr(), L.bias.data_ptr(), L.alpha.data_ptr(), 1, None, 0, y.planes.data_ptr(), None, B, H, W, C)
+    stages = {
+        "in": lambda: check(f_in(x.data_ptr(), v.data_ptr(), B, H, W, C, st)),
+        "gemm": lambda: check(f_gemm(v.data_ptr(), U.data_ptr(), m.data_ptr(), B, H, W, C, None, st)),
+        "gemm_kps2": lambda: check(f_gemm(v.data_ptr(), U.data_ptr(), m.data_ptr(), B, H, W, C, ops._tune(dict(kps=2)), st)),
+        "out": (lambda: check(lib.rn_winograd_out(*out_args, st))) if tile == 2 else
+               (lambda: check(lib.rn_winograd4_out(*out_args, s, st))),
+    }
+    st_ms = {k: min(timed(fn, launches) for _ in range(rounds)) for k, fn in stages.items()}
+    gemm_ms = min(st_ms["gemm"], st_ms["gemm_kps2"])
+    tiles = n * pos // 128 // 256                       # 128-row x 256-column tiles of the one GEMM launch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    act_bytes = B * H * W * C * 4                       # one hi/lo activation (two fp16 planes)
+    gbs = {"in": (act_bytes + n * pos * 4) / st_ms["in"] / 1e6,      # read x pair, write V pair
+           "out": (n * pos * 4 + act_bytes) / st_ms["out"] / 1e6}    # read M fp32, write y pair (no residual here)
+    return {"stage_ms": st_ms, "gemm_tflops_issued": 3 * 2.0 * n * pos * C / gemm_ms / 1e9, "gemm_tiles": tiles,
+            "gemm_us_per_tile": gemm_ms * 1e3 / (tiles / sms), "transform_gbs": gbs}
+
+
 def one_width(C, launches, rounds):
     g = torch.Generator().manual_seed(C)
     x = ops.cast_to_16(((torch.rand(B, H, W, C, generator=g) * 2 - 1) * 3).to("cuda"), fmt=2)
@@ -51,41 +83,18 @@ def one_width(C, launches, rounds):
     al = torch.rand(C, generator=g) * 0.3
     L = ops.pack_conv("conv2d", w, torch.zeros(C), al, device="cuda", fmt=2)
     y = ops.conv2d(x, L, act="prelu")
-    on, off = dict(winograd=1), dict(winograd=-1)
-    arms = {"direct": lambda: ops.conv2d(x, L, act="prelu", out16=y, tune=off),
-            "winograd": lambda: ops.conv2d(x, L, act="prelu", out16=y, tune=on)}
+    tunes = {"direct": dict(winograd=-1), "winograd": dict(winograd=1, wino_tile=2), "winograd4": dict(winograd=1, wino_tile=4)}
+    arms = {k: (lambda t=t: ops.conv2d(x, L, act="prelu", out16=y, tune=t)) for k, t in tunes.items()}
     times = {k: [] for k in arms}
     for _ in range(rounds):
         for k, fn in arms.items():
             times[k].append(timed(fn, launches))
-    # stages alone, on a workspace of their own
-    U = ops.winograd_filter(L)
-    ws = torch.empty(lib.rn_winograd_workspace_bytes(B, H, W, C), device="cuda", dtype=torch.uint8)
-    pos = B * (H // 2) * (W // 2) * C
-    v = ws[:16 * pos * 4]
-    m = ws[16 * pos * 4:].view(torch.float32)
-    st = torch.cuda.current_stream().cuda_stream
-    stages = {
-        "in": lambda: check(lib.rn_winograd_in(x.data_ptr(), v.data_ptr(), B, H, W, C, st)),
-        "gemm": lambda: check(lib.rn_winograd_gemm(v.data_ptr(), U.data_ptr(), m.data_ptr(), B, H, W, C, None, st)),
-        "gemm_kps2": lambda: check(lib.rn_winograd_gemm(v.data_ptr(), U.data_ptr(), m.data_ptr(), B, H, W, C,
-                                                         ops._tune(dict(kps=2)), st)),
-        "out": lambda: check(lib.rn_winograd_out(m.data_ptr(), L.bias.data_ptr(), L.alpha.data_ptr(), 1, None, 0,
-                                                 y.planes.data_ptr(), None, B, H, W, C, st)),
-    }
-    st_ms = {k: min(timed(fn, launches) for _ in range(rounds)) for k, fn in stages.items()}
     flop = 2.0 * B * H * W * C * 9 * C
-    issued_gemm = 3 * 2.0 * 16 * pos * C
-    gemm_ms = min(st_ms["gemm"], st_ms["gemm_kps2"])
-    tiles = 16 * pos // 128 // 256                      # 128-row x 256-column tiles of the one GEMM launch
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    act_bytes = B * H * W * C * 4                       # one hi/lo activation (two fp16 planes)
-    gbs = {"in": (act_bytes + 16 * pos * 4) / st_ms["in"] / 1e6,      # read x pair, write V pair
-           "out": (16 * pos * 4 + act_bytes) / st_ms["out"] / 1e6}    # read M fp32, write y pair (no residual here)
-    res = {"C": C, "direct_ms": times["direct"], "winograd_ms": times["winograd"], "stage_ms": st_ms,
-           "direct_tflops_alg": flop / min(times["direct"]) / 1e9, "winograd_tflops_alg": flop / min(times["winograd"]) / 1e9,
-           "gemm_tflops_issued": issued_gemm / gemm_ms / 1e9, "gemm_tiles": tiles,
-           "gemm_us_per_tile": gemm_ms * 1e3 / (tiles / sms), "transform_gbs": gbs}
+    res = {"C": C}
+    res.update({f"{k}_ms": v for k, v in times.items()})
+    res.update({f"{k}_tflops_alg": flop / min(v) / 1e9 for k, v in times.items()})
+    res["f2x2"] = _stages(2, L, x, y, C, launches, rounds)
+    res["f4x4"] = _stages(4, L, x, y, C, launches, rounds)
     return res
 
 
