@@ -1,5 +1,5 @@
 // rn_ptx.cuh -- thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor, incl. cluster multicast),
-// cluster barriers, register reallocation and the wgmma shared-memory matrix descriptor (rn_wgmma.cuh holds the MMAs).
+// cp.async, cluster barriers, register reallocation and the wgmma shared-memory matrix descriptor (rn_wgmma.cuh holds the MMAs).
 // Hand-written for this project; bit layouts follow the PTX ISA "matrix descriptor format" table for wgmma.
 #pragma once
 #include <cstdint>
@@ -110,6 +110,13 @@ __device__ __forceinline__ void tma_a_3d_mc(uint32_t dst, uint64_t map, uint32_t
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, "
       "%5, %6}], [%2], %3;" ::"r"(dst), "l"(map), "r"(bar), "h"(mask), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
+
+// ------------------------------------------------------------------ cp.async (16 bytes, L2 only; bytes = 0 zero-fills)
+__device__ __forceinline__ void cp_async16(void* dst, const void* src, uint32_t bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -166,19 +166,6 @@ __global__ void __launch_bounds__(128) winograd_out_kernel(const __grid_constant
   }
 }
 
-__device__ __forceinline__ void load4(const uint16_t* __restrict__ hi, long long plane, long long off, float* v) {
-  const uint2 h = __ldg(reinterpret_cast<const uint2*>(hi + off));
-  const uint2 l = __ldg(reinterpret_cast<const uint2*>(hi + plane + off));
-  const uint32_t wh[2] = {h.x, h.y}, wl[2] = {l.x, l.y};
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&wh[j]));
-    const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&wl[j]));
-    v[2 * j] = fh.x + fl.x;
-    v[2 * j + 1] = fh.y + fl.y;
-  }
-}
-
 // B^T applied to one column (or row) of a 6-point patch, in place.
 __device__ __forceinline__ void bt6(float& d0, float& d1, float& d2, float& d3, float& d4, float& d5) {
   const float p = fmaf(-0.25f, d2, d4), q = fmaf(-0.25f, d1, d3);   // d4 - d2/4, d3 - d1/4
@@ -187,65 +174,92 @@ __device__ __forceinline__ void bt6(float& d0, float& d1, float& d2, float& d3, 
   d0 = t0; d1 = p + q; d2 = p - q; d3 = r + s; d4 = r - s; d5 = t5;
 }
 
-// F(4x4, 3x3).  One thread: 4 channels of one 4x4 output block (8 would hold 288 patch values and spill).  Reads the 6x6
-// patch (zero outside the image), writes V = 1/2 B^T d B to 36 positions.
-__global__ void __launch_bounds__(128) winograd4_in_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ v, int B,
-                                                           int H, int W, int C) {
-  const int H4 = H / 4, W4 = W / 4, CG = C / 4;
-  const long long n = static_cast<long long>(B) * H4 * W4 * CG;
+// F(4x4, 3x3) input transform, streamed: every input row is read from HBM once per CTA.  One CTA: one image, kWi4Cs
+// channels, kWi4Tw block columns (4 kWi4Tw + 2 input columns with the halo) and a band of block rows, swept top to bottom.
+// Block row ty reads input rows 4ty-1 .. 4ty+4; the last two are the next block row's first two, so each step loads only
+// 4 new rows.  The rows land by cp.async (zero-filled outside the image: the SAME padding) in a ring of kWi4Ring
+// shared-memory rows, the next block row's 4 while this one is transformed.  One warp: one block column, 2 channels per
+// lane, so each V store of a warp is 128 contiguous bytes.  Each element of V takes the same fp32 operations in the same
+// order (hi + lo, bt6 down the columns, bt6 along the rows, x 1/2, split) whatever the tiling, band split or batch.
+constexpr int kWi4Tw = 8;                     // block columns per CTA = warps
+constexpr int kWi4Cs = 64;                    // channels per CTA
+constexpr int kWi4Cols = 4 * kWi4Tw + 2;      // input columns per CTA
+constexpr int kWi4Ring = 10;                  // input rows in shared memory: 6 being read + 4 being loaded
+constexpr int kWi4Smem = kWi4Ring * 2 * kWi4Cols * kWi4Cs * 2;   // [row][hi, lo][column][channel] fp16
+
+__global__ void __launch_bounds__(32 * kWi4Tw, 2) winograd4_in_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ v,
+                                                                   int B, int H, int W, int C, int band) {
+  constexpr int ROW = kWi4Cols * kWi4Cs;      // fp16 elements of one plane of one input row
+  constexpr int CH = kWi4Cs / 8;              // 16-byte chunks per pixel and plane
+  extern __shared__ __align__(16) uint16_t ring[];
+  const int H4 = H / 4, W4 = W / 4;
+  const int nslice = C / kWi4Cs, ntw = (W4 + kWi4Tw - 1) / kWi4Tw, nband = (H4 + band - 1) / band;
+  int r = blockIdx.x;
+  const int c0 = (r % nslice) * kWi4Cs;
+  r /= nslice;
+  const int tx0 = (r % ntw) * kWi4Tw;
+  r /= ntw;
+  const int ty0 = (r % nband) * band, ty1 = min(H4, ty0 + band);
+  const int b = r / nband;
   const long long x_plane = static_cast<long long>(B) * H * W * C;
+  const uint16_t* xb = x + static_cast<long long>(b) * H * W * C + c0;
+  auto load_rows = [&](int y0, int nrows) {   // input rows y0 .. y0 + nrows - 1 -> ring row (y + 1) % kWi4Ring
+    for (int i = threadIdx.x; i < nrows * 2 * kWi4Cols * CH; i += blockDim.x) {
+      int q = i;
+      const int ch = q % CH;
+      q /= CH;
+      const int col = q % kWi4Cols;
+      q /= kWi4Cols;
+      const int pl = q & 1, y = y0 + (q >> 1), xx = 4 * tx0 - 1 + col;
+      const bool in = y >= 0 && y < H && xx >= 0 && xx < W;
+      const uint16_t* src = in ? xb + pl * x_plane + (static_cast<long long>(y) * W + xx) * C + ch * 8 : x;
+      cp_async16(ring + ((y + 1) % kWi4Ring * 2 + pl) * ROW + col * kWi4Cs + ch * 8, src, in ? 16 : 0);
+    }
+    cp_async_commit();
+  };
+  load_rows(4 * ty0 - 1, 6);
+  const int warp = threadIdx.x / 32, cl = 2 * (threadIdx.x % 32);
+  const int tx = tx0 + warp;
   const long long pos = static_cast<long long>(B) * H4 * W4 * C;   // one position of V
   const long long v_plane = 36 * pos;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int cg = static_cast<int>(i % CG);
-    long long r = i / CG;
-    const int tx = static_cast<int>(r % W4);
-    r /= W4;
-    const int ty = static_cast<int>(r % H4);
-    const int b = static_cast<int>(r / H4);
-    float t[6][6][4];
+  for (int ty = ty0; ty < ty1; ++ty) {
+    cp_async_wait_all();
+    __syncthreads();                          // rows of ty landed; every warp is done reading ty - 1's
+    if (ty + 1 < ty1) load_rows(4 * ty + 5, 4);
+    if (tx >= W4) continue;
+    float t[6][6][2];
+    const int s0 = 4 * ty % kWi4Ring;         // ring row of input row 4ty - 1
 #pragma unroll
     for (int a = 0; a < 6; ++a) {
-      const int yy = 4 * ty - 1 + a;
+      const uint16_t* row = ring + (s0 + a < kWi4Ring ? s0 + a : s0 + a - kWi4Ring) * 2 * ROW + 4 * warp * kWi4Cs + cl;
 #pragma unroll
       for (int c = 0; c < 6; ++c) {
-        const int xx = 4 * tx - 1 + c;
-        if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
-          load4(x, x_plane, ((static_cast<long long>(b) * H + yy) * W + xx) * C + cg * 4, t[a][c]);
-        } else {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) t[a][c][k] = 0.f;
-        }
+        const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(row + c * kWi4Cs));
+        const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(row + ROW + c * kWi4Cs));
+        t[a][c][0] = fh.x + fl.x;
+        t[a][c][1] = fh.y + fl.y;
       }
     }
 #pragma unroll
-    for (int c = 0; c < 6; ++c)            // rows: B^T d
+    for (int c = 0; c < 6; ++c)              // columns: B^T d
 #pragma unroll
-      for (int k = 0; k < 4; ++k) bt6(t[0][c][k], t[1][c][k], t[2][c][k], t[3][c][k], t[4][c][k], t[5][c][k]);
+      for (int k = 0; k < 2; ++k) bt6(t[0][c][k], t[1][c][k], t[2][c][k], t[3][c][k], t[4][c][k], t[5][c][k]);
+    const long long o = ((static_cast<long long>(b) * H4 + ty) * W4 + tx) * C + c0 + cl;
 #pragma unroll
-    for (int a = 0; a < 6; ++a)            // columns: (B^T d) B
+    for (int a = 0; a < 6; ++a) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) bt6(t[a][0][k], t[a][1][k], t[a][2][k], t[a][3][k], t[a][4][k], t[a][5][k]);
-    const long long o = ((static_cast<long long>(b) * H4 + ty) * W4 + tx) * C + cg * 4;
+      for (int k = 0; k < 2; ++k) bt6(t[a][0][k], t[a][1][k], t[a][2][k], t[a][3][k], t[a][4][k], t[a][5][k]);   // rows
 #pragma unroll
-    for (int a = 0; a < 6; ++a)
-#pragma unroll
-      for (int c = 0; c < 6; ++c) {
-        uint32_t wh[2], wl[2];
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {   // v = t / 2 (exact), hi = fp16(v), lo = fp16(v - hi)
-          const float v0 = 0.5f * t[a][c][2 * j], v1 = 0.5f * t[a][c][2 * j + 1];
-          const __half2 h = __floats2half2_rn(v0, v1);
-          const float2 hf = __half22float2(h);
-          const __half2 l = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
-          wh[j] = *reinterpret_cast<const uint32_t*>(&h);
-          wl[j] = *reinterpret_cast<const uint32_t*>(&l);
-        }
-        uint2* dst = reinterpret_cast<uint2*>(v + (6 * a + c) * pos + o);
-        dst[0] = make_uint2(wh[0], wh[1]);
-        dst[v_plane >> 2] = make_uint2(wl[0], wl[1]);
+      for (int e = 0; e < 6; ++e) {          // v = t / 2 (exact), hi = fp16(v), lo = fp16(v - hi)
+        const float v0 = 0.5f * t[a][e][0], v1 = 0.5f * t[a][e][1];
+        const __half2 h = __floats2half2_rn(v0, v1);
+        const float2 hf = __half22float2(h);
+        const __half2 l = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+        uint32_t* dst = reinterpret_cast<uint32_t*>(v + (6 * a + e) * pos + o);
+        dst[0] = *reinterpret_cast<const uint32_t*>(&h);
+        dst[v_plane >> 1] = *reinterpret_cast<const uint32_t*>(&l);
       }
+    }
   }
 }
 
@@ -427,9 +441,25 @@ extern "C" long long rn_winograd4_workspace_bytes(int B, int H, int W, int C) {
 
 extern "C" int rn_winograd4_in(const void* x, void* v, int B, int H, int W, int C, void* stream) {
   if (x == nullptr || v == nullptr || !wino4_shape_ok(B, H, W, C)) return -1;
-  const long long n = static_cast<long long>(B) * (H / 4) * (W / 4) * (C / 4);
-  winograd4_in_kernel<<<wino_grid(n), 128, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint16_t*>(x), static_cast<uint16_t*>(v), B, H, W, C);
+  static std::atomic<bool> attr_set[kMaxDevices];   // cudaFuncSetAttribute is per device
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
+  if (!attr_set[dev].load(std::memory_order_acquire)) {
+    const cudaError_t e = cudaFuncSetAttribute(winograd4_in_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWi4Smem);
+    if (e != cudaSuccess) return static_cast<int>(e);
+    attr_set[dev].store(true, std::memory_order_release);
+  }
+  // Split the height into bands only when (image, channel slice, width tile) alone leave SMs idle: each band re-reads a
+  // 2-row halo.
+  const int H4 = H / 4;
+  const long long base = static_cast<long long>(B) * (C / kWi4Cs) * ((W / 4 + kWi4Tw - 1) / kWi4Tw);
+  const long long want = (2LL * num_sms() + base - 1) / base;   // 2 CTAs fit on an SM
+  const int nband = static_cast<int>(want < H4 ? want : H4), band = (H4 + nband - 1) / nband;
+  const long long grid = base * ((H4 + band - 1) / band);
+  if (grid > 0x7fffffffLL) return -1;
+  winograd4_in_kernel<<<static_cast<unsigned>(grid), 32 * kWi4Tw, kWi4Smem, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint16_t*>(x), static_cast<uint16_t*>(v), B, H, W, C, band);
   g_launch_count.fetch_add(1, std::memory_order_relaxed);
   return static_cast<int>(cudaGetLastError());
 }
