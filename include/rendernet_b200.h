@@ -555,6 +555,47 @@ long long rn_voxel_fit_grad_workspace(int S);
 int rn_voxel_fit_grad(const float* dvox, const float* occ, const unsigned char* keep, float* g, double* reg, double* work, int V,
                       int S, float lambda_smooth, float lambda_bin, void* stream);
 
+/* ---- fixed-order twins (what rendernet_b200.ops calls under torch.use_deterministic_algorithms) ------------------------------
+ * Twins of the input-gradient kernels that reduce with float atomics.  Each result is a function of its own item's inputs alone:
+ * bit-identical from run to run, and for an item whatever batch it is part of.  Each takes a caller-owned workspace of at least
+ * the matching *_workspace(...) bytes (rc -4 if smaller), allocates nothing and does not synchronise (a CUDA graph may capture
+ * it).  Unlike the atomic kernels, every output is OVERWRITTEN: nothing needs zeroing.  Per-pixel outputs are the atomic
+ * kernels' bit for bit; only the reductions differ.
+ *   rn_resample_backward_fixed_f32 / rn_resample5_backward_fixed_f32 (whole grid): dvox / dtex are summed in 64-bit fixed point
+ *   (per item and channel of gout a power of two 2^k with new_size^3 max|gout| 2^k < 2^62, so no sum can overflow; each fp32
+ *   corner contribution w g is scaled by 2^k in double and rounded once to an integer, then added with an integer atomic), dminv
+ *   from per-block partial sums added in block order.  An item whose gout holds an Inf or NaN gets NaN in all its outputs.
+ *   rn_fixed_point_exponent(max_abs, new_size) is the k the resampler twins use (0 for max_abs 0 or non-finite).
+ *   Phong objectives and rn_image_loss_grad_items_fixed: loss and d_light from per-block partials added in block order in double;
+ *   the image loss uses a block count per item that does not depend on the batch. */
+int rn_fixed_point_exponent(float max_abs, int new_size);
+long long rn_resample_backward_fixed_workspace(int B, int C, int size, int new_size, int want_dvox);
+int rn_resample_backward_fixed_f32(const float* vox, const float* minv, const float* gout, float* dvox, float* dminv, int B, int C,
+                                   int size, int new_size, int transform, void* work, long long work_bytes, void* stream);
+long long rn_resample5_backward_fixed_workspace(int B, int size, int new_size, int want_dvox, int want_dtex);
+int rn_resample5_backward_fixed_f32(const float* vox, const float* tex, const float* minv, const float* gout, float* dvox,
+                                    float* dtex, float* dminv, int B, int size, int new_size, void* work, long long work_bytes,
+                                    void* stream);
+long long rn_phong_recon_loss_grad_fixed_workspace(int B, int H, int W);
+int rn_phong_recon_loss_grad_fixed(const float* albedo, const float* normal, const float* target, const float* light_dir,
+                                   const float* light_col, float ambient, float k_diffuse, int black_background, int with_mask,
+                                   double* loss, float* d_albedo, float* d_normal, float* d_light_dir, int B, int H, int W,
+                                   void* work, long long work_bytes, void* stream);
+long long rn_phong_composite_loss_grad_fixed_workspace(int B, int H, int W);
+int rn_phong_composite_loss_grad_fixed(const float* img, const float* target, const float* light_dir, const float* light_col,
+                                       float ambient, float k_diffuse, int background_white, int with_mask, double* loss,
+                                       float* d_img, float* d_light_dir, int B, int H, int W, void* work, long long work_bytes,
+                                       void* stream);
+/* work may be NULL when d_light_dir is NULL */
+long long rn_phong_shade_backward_fixed_workspace(int B, int H, int W);
+int rn_phong_shade_backward_fixed(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
+                                  float ambient, float k_diffuse, int composite, int background_white, int with_mask,
+                                  const float* g_compos, float* d_normal, float* d_albedo, float* d_light_dir, int B, int H, int W,
+                                  void* work, long long work_bytes, void* stream);
+long long rn_image_loss_grad_items_fixed_workspace(long long npix, int C, int batch);
+int rn_image_loss_grad_items_fixed(const float* img, const float* target, float* dimg, double* loss, long long npix, int C,
+                                   int batch, int kind, void* work, long long work_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

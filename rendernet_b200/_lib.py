@@ -131,6 +131,19 @@ SIGNATURES = {
     "rn_phong_composite": (_i, [_vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _i, _i, _i, _vp]),
     "rn_phong_shade": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "rn_phong_shade_backward": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "rn_fixed_point_exponent": (_i, [_f, _i]),
+    "rn_resample_backward_fixed_workspace": (_ll, [_i] * 5),
+    "rn_resample_backward_fixed_f32": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _ll, _vp]),
+    "rn_resample5_backward_fixed_workspace": (_ll, [_i] * 5),
+    "rn_resample5_backward_fixed_f32": (_i, [_vp] * 7 + [_i, _i, _i, _vp, _ll, _vp]),
+    "rn_phong_recon_loss_grad_fixed_workspace": (_ll, [_i] * 3),
+    "rn_phong_recon_loss_grad_fixed": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _ll, _vp]),
+    "rn_phong_composite_loss_grad_fixed_workspace": (_ll, [_i] * 3),
+    "rn_phong_composite_loss_grad_fixed": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _ll, _vp]),
+    "rn_phong_shade_backward_fixed_workspace": (_ll, [_i] * 3),
+    "rn_phong_shade_backward_fixed": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _ll, _vp]),
+    "rn_image_loss_grad_items_fixed_workspace": (_ll, [_ll, _i, _i]),
+    "rn_image_loss_grad_items_fixed": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _i, _vp, _ll, _vp]),
 }
 RN_PHONG_NUMPY, RN_PHONG_TF = 0, 1
 

@@ -152,6 +152,105 @@ __global__ void __launch_bounds__(256) conv3d_bwd_data_kernel(const uint16_t* __
   }
 }
 
+// ------------------------------------------------------------------------------------------ fixed-order twins: helpers
+// The resampler backward's scatter-add in fixed point (the twins run under torch.use_deterministic_algorithms, DESIGN §8b).
+// Per batch item and channel, m = max |G| (an integer max of the fp32 bit patterns: order-free, and NaN sorts above Inf) fixes a
+// power of two 2^k with m 2^k < 2^(62 - L), 2^L >= new_size^3.  Every corner weight is <= 1 and each sample point adds to each of
+// its 8 corners once, so a corner takes at most new_size^3 contributions, each rounded to an integer of magnitude <= 2^(62 - L):
+// the int64 sum stays within 2^62 for every pose.  Integer addition is associative, so the sum does not depend on the order of
+// the atomics; one contribution is rounded by at most 2^-k / 2 <= 2^(L - 62) m, 2^-41 m at new_size = 128.
+constexpr unsigned FX_NONFINITE = 0x7f800000u;                       // |G| bit patterns at or above this are Inf / NaN
+
+__host__ __device__ inline int fx_exponent(float max_abs, int lg_points) {
+  if (!(max_abs > 0.f) || !(max_abs <= 3.402823466e38f)) return 0;    // 0, or non-finite (handled by the caller)
+  int e;
+  frexpf(max_abs, &e);                                                 // max_abs < 2^e (subnormals included)
+  return 62 - lg_points - e;
+}
+
+__device__ __forceinline__ double fx_scale(unsigned amax_bits, int lg_points) {
+  return amax_bits >= FX_NONFINITE ? 0.0 : ldexp(1.0, fx_exponent(__uint_as_float(amax_bits), lg_points));
+}
+
+// one contribution: the fp32 product w g of the atomic kernel, scaled in double and rounded once; two's complement wraps, so
+// unsigned addition is int64 addition
+template <bool FX>
+__device__ __forceinline__ void scatter_add(float* __restrict__ dst, unsigned long long* __restrict__ acc, size_t i, float v,
+                                            double scale) {
+  if constexpr (FX) atomicAdd(acc + i, static_cast<unsigned long long>(__double2ll_rn(static_cast<double>(v) * scale)));
+  else atomicAdd(dst + i, v);
+}
+
+// amax[b * C + c] = max over the item's points of |G[b, point, c]|'s bit pattern (amax zeroed by the caller); blockIdx.y = item.
+template <int C>
+__global__ void __launch_bounds__(256) absmax_bits_kernel(const float* __restrict__ g, unsigned* __restrict__ amax,
+                                                          long long points) {
+  __shared__ unsigned red[8][C];
+  const unsigned* gb = reinterpret_cast<const unsigned*>(g) + static_cast<size_t>(blockIdx.y) * points * C;
+  unsigned m[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) m[c] = 0u;
+  for (long long p = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; p < points;
+       p += static_cast<long long>(gridDim.x) * blockDim.x) {
+#pragma unroll
+    for (int c = 0; c < C; ++c) m[c] = max(m[c], gb[p * C + c] & 0x7fffffffu);
+  }
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+#pragma unroll
+  for (int c = 0; c < C; ++c) {
+    unsigned v = m[c];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
+    if (lane == 0) red[wib][c] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < C) {
+    unsigned v = 0u;
+    for (int w = 0; w < 8; ++w) v = max(v, red[w][threadIdx.x]);
+    atomicMax(amax + blockIdx.y * C + threadIdx.x, v);
+  }
+}
+
+// out[b][i] = acc[b][i] 2^-k as fp32, k from amax[b * C_amax + c0 + i % Cout]; NaN for the whole item when any of its C_amax
+// channels holds a non-finite G.  blockIdx.y = item.
+__global__ void __launch_bounds__(256) fx_finalize_kernel(const unsigned long long* __restrict__ acc, const unsigned* __restrict__ amax,
+                                                          int C_amax, int c0, int lg_points, float* __restrict__ out,
+                                                          long long per_item, int Cout) {
+  const unsigned* am = amax + blockIdx.y * C_amax;
+  bool bad = false;
+  for (int c = 0; c < C_amax; ++c) bad |= am[c] >= FX_NONFINITE;
+  const size_t base = static_cast<size_t>(blockIdx.y) * per_item;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < per_item;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(i % Cout);
+    const double inv = ldexp(1.0, -fx_exponent(__uint_as_float(am[c0 + c]), lg_points));
+    out[base + i] = bad ? __int_as_float(0x7fffffff)
+                        : __double2float_rn(__ll2double_rn(static_cast<long long>(acc[base + i])) * inv);
+  }
+}
+
+// The fixed-order second stage of every twin: per item b and entry j < width, the sum over the item's nblk block partials
+// part[(b * nblk + k) * width + j] in double.  One warp per (b, j): lane l adds k = l, l + 32, ... in order, then a fixed
+// butterfly.  Entries j < nd go to out_d[b * nd + j] (double), the rest to out_f[b * (width - nd) + j - nd] (fp32; may be NULL).
+// amax (may be NULL): the item's sums become NaN when any of its namax channels holds a non-finite G.
+__global__ void __launch_bounds__(256) slot_sum_kernel(const double* __restrict__ part, int B, int nblk, int width, int nd,
+                                                       double* __restrict__ out_d, float* __restrict__ out_f,
+                                                       const unsigned* __restrict__ amax, int namax) {
+  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (w >= B * width) return;                                          // whole warps leave together
+  const int b = w / width, j = w % width;
+  double s = 0.0;
+  for (int k = lane; k < nblk; k += 32) s += part[(static_cast<size_t>(b) * nblk + k) * width + j];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane != 0) return;
+  if (amax != nullptr)
+    for (int c = 0; c < namax; ++c)
+      if (amax[b * namax + c] >= FX_NONFINITE) s = __longlong_as_double(0x7ff8000000000000LL);
+  if (j < nd) out_d[b * nd + j] = s;
+  else if (out_f != nullptr) out_f[b * (width - nd) + j - nd] = static_cast<float>(s);
+}
+
 // ------------------------------------------------------------------------------------------ resampler backward
 // Forward (rn_resample_f32, transform = 1): N[b,p,q,r,c] = sum_corners w_k(x,y,z) V[b, corner_k, c] with
 // (x,y,z) = Minv[b] . (r, new-1-p, q, 1), zero outside [0, size-1)^3.  Given G = dL/dN:
@@ -160,11 +259,15 @@ __global__ void __launch_bounds__(256) conv3d_bwd_data_kernel(const uint16_t* __
 // The floor() inside the weights is piecewise constant, so the derivative is the one of the trilinear patch the point
 // lies in (what tf.gradients produces for tools/resampling_voxel_grid.py:465-485).  One warp per output row; the 12 matrix
 // partial sums are reduced in the warp, then in the block, then one atomicAdd per block and entry.
-template <int C>
+// FX (the fixed-order twin): dvox and dminv are unused; the scatter adds fixed-point integers to acc [B,size^3,C] (scale from amax,
+// see scatter_add) and each block writes its 12 partial sums to slots[blockIdx.x][12] (a block's rows lie in one item).
+template <int C, bool FX>
 __global__ void __launch_bounds__(256) resample_backward_kernel(const float* __restrict__ vox, const float* __restrict__ minv,
                                                                 const float* __restrict__ gout, float* __restrict__ dvox,
                                                                 float* __restrict__ dminv, int B, int size, int nsz,
-                                                                int transform) {
+                                                                int transform, unsigned long long* __restrict__ acc,
+                                                                const unsigned* __restrict__ amax, int lg_points,
+                                                                double* __restrict__ slots) {
   __shared__ float red[8][12];
   const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -186,6 +289,10 @@ __global__ void __launch_bounds__(256) resample_backward_kernel(const float* __r
     const float lim = static_cast<float>(size - 1);
     const float* vb = vox + static_cast<size_t>(b) * size * size * size * C;
     float* dvb = dvox != nullptr ? dvox + static_cast<size_t>(b) * size * size * size * C : nullptr;
+    unsigned long long* avb = FX && acc != nullptr ? acc + static_cast<size_t>(b) * size * size * size * C : nullptr;
+    double sc[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) sc[c] = FX ? fx_scale(__ldg(amax + b * C + c), lg_points) : 0.0;
     const float* grow = gout + static_cast<size_t>(warp_global) * nsz * C;
     for (int r = lane; r < nsz; r += 32) {
       const float gx = static_cast<float>(r);
@@ -212,15 +319,15 @@ __global__ void __launch_bounds__(256) resample_backward_kernel(const float* __r
         dvx += gv * (ay * az * (Ic - Ia) + by * az * (Id - Ib) + ay * bz * (Ig - Ie) + by * bz * (Ih - If));
         dvy += gv * (ax * az * (Ib - Ia) + bx * az * (Id - Ic) + ax * bz * (If - Ie) + bx * bz * (Ih - Ig));
         dvz += gv * (ax * ay * (Ie - Ia) + ax * by * (If - Ib) + bx * ay * (Ig - Ic) + bx * by * (Ih - Id));
-        if (dvb != nullptr) {
-          atomicAdd(dvb + i000 + c, ax * ay * az * gv);
-          atomicAdd(dvb + i000 + sy + c, ax * by * az * gv);
-          atomicAdd(dvb + i000 + C + c, bx * ay * az * gv);
-          atomicAdd(dvb + i000 + sy + C + c, bx * by * az * gv);
-          atomicAdd(dvb + i000 + sz + c, ax * ay * bz * gv);
-          atomicAdd(dvb + i000 + sz + sy + c, ax * by * bz * gv);
-          atomicAdd(dvb + i000 + sz + C + c, bx * ay * bz * gv);
-          atomicAdd(dvb + i000 + sz + sy + C + c, bx * by * bz * gv);
+        if (FX ? avb != nullptr : dvb != nullptr) {
+          scatter_add<FX>(dvb, avb, i000 + c, ax * ay * az * gv, sc[c]);
+          scatter_add<FX>(dvb, avb, i000 + sy + c, ax * by * az * gv, sc[c]);
+          scatter_add<FX>(dvb, avb, i000 + C + c, bx * ay * az * gv, sc[c]);
+          scatter_add<FX>(dvb, avb, i000 + sy + C + c, bx * by * az * gv, sc[c]);
+          scatter_add<FX>(dvb, avb, i000 + sz + c, ax * ay * bz * gv, sc[c]);
+          scatter_add<FX>(dvb, avb, i000 + sz + sy + c, ax * by * bz * gv, sc[c]);
+          scatter_add<FX>(dvb, avb, i000 + sz + C + c, bx * ay * bz * gv, sc[c]);
+          scatter_add<FX>(dvb, avb, i000 + sz + sy + C + c, bx * by * bz * gv, sc[c]);
         }
       }
       dm[0] += dvx * gx; dm[1] += dvx * gy; dm[2] += dvx * gz; dm[3] += dvx;
@@ -228,7 +335,7 @@ __global__ void __launch_bounds__(256) resample_backward_kernel(const float* __r
       dm[8] += dvz * gx; dm[9] += dvz * gy; dm[10] += dvz * gz; dm[11] += dvz;
     }
   }
-  if (dminv == nullptr) return;
+  if (FX ? slots == nullptr : dminv == nullptr) return;
   // rows of one block belong to one batch item when nsz*nsz % 8 == 0 (checked by the host): reduce within the block
 #pragma unroll
   for (int i = 0; i < 12; ++i) {
@@ -242,7 +349,8 @@ __global__ void __launch_bounds__(256) resample_backward_kernel(const float* __r
     float v = 0.f;
     for (int wv = 0; wv < 8; ++wv) v += red[wv][threadIdx.x];
     const int first_row = (blockIdx.x * blockDim.x) >> 5;
-    if (first_row < rows && v != 0.f) atomicAdd(dminv + (first_row / (nsz * nsz)) * 12 + threadIdx.x, v);
+    if constexpr (FX) slots[static_cast<size_t>(blockIdx.x) * 12 + threadIdx.x] = v;
+    else if (first_row < rows && v != 0.f) atomicAdd(dminv + (first_row / (nsz * nsz)) * 12 + threadIdx.x, v);
   }
 }
 
@@ -253,12 +361,17 @@ __global__ void __launch_bounds__(256) resample_backward_kernel(const float* __r
 // dM^-1 collects all five channels.  Per corner the five channels are first contracted to s_k = G0 V_k + G1..4 . T_k, so
 // d/dx = sum_k (dw_k/dx) s_k.  Same warp-per-row layout and block reduction as resample_backward_kernel.  G covers the window
 // of rows [wy0, wy0+wh) x columns [wx0, wx0+ww) (all depths; the whole grid: 0, 0, nsz, nsz), [B,wh,ww,nsz,5]: only the
-// points of that window scatter.
+// points of that window scatter.  FX (the fixed-order twin, whole grid): as resample_backward_kernel's, with acc_vox [B,size^3],
+// acc_tex [B,size^3,4] and one scale per item and channel of G (amax [B,5]).
+template <bool FX>
 __global__ void __launch_bounds__(256) resample5_backward_kernel(const float* __restrict__ vox, const float* __restrict__ tex,
                                                                  const float* __restrict__ minv, const float* __restrict__ gout,
                                                                  float* __restrict__ dvox, float* __restrict__ dtex,
                                                                  float* __restrict__ dminv, int B, int size, int nsz, int wy0,
-                                                                 int wx0, int wh, int ww) {
+                                                                 int wx0, int wh, int ww, unsigned long long* __restrict__ acc_vox,
+                                                                 unsigned long long* __restrict__ acc_tex,
+                                                                 const unsigned* __restrict__ amax, int lg_points,
+                                                                 double* __restrict__ slots) {
   __shared__ float red[8][12];
   const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -281,6 +394,11 @@ __global__ void __launch_bounds__(256) resample5_backward_kernel(const float* __
     const float4* tb = reinterpret_cast<const float4*>(tex) + static_cast<size_t>(b) * vol;
     float* dvb = dvox != nullptr ? dvox + static_cast<size_t>(b) * vol : nullptr;
     float* dtb = dtex != nullptr ? dtex + static_cast<size_t>(b) * vol * 4 : nullptr;
+    unsigned long long* avb = FX && acc_vox != nullptr ? acc_vox + static_cast<size_t>(b) * vol : nullptr;
+    unsigned long long* atb = FX && acc_tex != nullptr ? acc_tex + static_cast<size_t>(b) * vol * 4 : nullptr;
+    double sc[5];
+#pragma unroll
+    for (int c = 0; c < 5; ++c) sc[c] = FX ? fx_scale(__ldg(amax + b * 5 + c), lg_points) : 0.0;
     const size_t sy = static_cast<size_t>(size), sz = static_cast<size_t>(size) * size;
     const float* grow = gout + static_cast<size_t>(warp_global) * nsz * 5;
     for (int r = lane; r < nsz; r += 32) {
@@ -310,11 +428,11 @@ __global__ void __launch_bounds__(256) resample5_backward_kernel(const float* __
       const float dvz = ax * ay * (s[4] - s[0]) + ax * by * (s[5] - s[1]) + bx * ay * (s[6] - s[2]) + bx * by * (s[7] - s[3]);
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
-        if (dvb != nullptr && g0 != 0.f) atomicAdd(dvb + off[k], wk[k] * g0);
-        if (dtb != nullptr) {
-          float* d = dtb + off[k] * 4;
-          atomicAdd(d + 0, wk[k] * g1); atomicAdd(d + 1, wk[k] * g2);
-          atomicAdd(d + 2, wk[k] * g3); atomicAdd(d + 3, wk[k] * g4);
+        if ((FX ? avb != nullptr : dvb != nullptr) && g0 != 0.f) scatter_add<FX>(dvb, avb, off[k], wk[k] * g0, sc[0]);
+        if (FX ? atb != nullptr : dtb != nullptr) {
+          const size_t d = off[k] * 4;
+          scatter_add<FX>(dtb, atb, d + 0, wk[k] * g1, sc[1]); scatter_add<FX>(dtb, atb, d + 1, wk[k] * g2, sc[2]);
+          scatter_add<FX>(dtb, atb, d + 2, wk[k] * g3, sc[3]); scatter_add<FX>(dtb, atb, d + 3, wk[k] * g4, sc[4]);
         }
       }
       dm[0] += dvx * gx; dm[1] += dvx * gy; dm[2] += dvx * gz; dm[3] += dvx;
@@ -322,7 +440,7 @@ __global__ void __launch_bounds__(256) resample5_backward_kernel(const float* __
       dm[8] += dvz * gx; dm[9] += dvz * gy; dm[10] += dvz * gz; dm[11] += dvz;
     }
   }
-  if (dminv == nullptr) return;
+  if (FX ? slots == nullptr : dminv == nullptr) return;
 #pragma unroll
   for (int i = 0; i < 12; ++i) {
     float v = dm[i];
@@ -335,7 +453,8 @@ __global__ void __launch_bounds__(256) resample5_backward_kernel(const float* __
     float v = 0.f;
     for (int wv = 0; wv < 8; ++wv) v += red[wv][threadIdx.x];
     const int first_row = (blockIdx.x * blockDim.x) >> 5;
-    if (first_row < rows && v != 0.f) atomicAdd(dminv + (first_row / (wh * ww)) * 12 + threadIdx.x, v);
+    if constexpr (FX) slots[static_cast<size_t>(blockIdx.x) * 12 + threadIdx.x] = v;
+    else if (first_row < rows && v != 0.f) atomicAdd(dminv + (first_row / (wh * ww)) * 12 + threadIdx.x, v);
   }
 }
 
@@ -427,13 +546,15 @@ __global__ void fc_bwd_data_reduce_kernel(const float* __restrict__ part, float*
 // At n = (0.5, 0.5, 0.5) u = 0/0 and d are NaN: the forward shades the pixel as unlit, only the mask term reaches d_normal and
 // the pixel adds nothing to d_light.  Where |n| = 0 the mask term is 0.  One thread per pixel; blockIdx.y = batch item.  loss is
 // accumulated in double (one atomic per block); dL/dL is reduced over the block and mapped through the normalisation
-// (I - L L^T) / |l| before one atomic per block and component.
+// (I - L L^T) / |l| before one atomic per block and component.  FX (the fixed-order twin): the block's loss and d_light terms go
+// to slots[b][blockIdx.x][4] instead, summed in block order by slot_sum_kernel; the per-pixel code is the same.
+template <bool FX>
 __global__ void __launch_bounds__(256) phong_recon_loss_grad_kernel(const float* __restrict__ albedo, const float* __restrict__ normal,
                                                                     const float* __restrict__ target, const float* __restrict__ light_dir,
                                                                     const float* __restrict__ light_col, float ambient, float k_diffuse,
                                                                     int black, int with_mask, double* __restrict__ loss,
                                                                     float* __restrict__ d_albedo, float* __restrict__ d_normal,
-                                                                    float* __restrict__ d_light, int HW) {
+                                                                    float* __restrict__ d_light, int HW, double* __restrict__ slots) {
   __shared__ float red[8][4];
   const int b = blockIdx.y;
   const float l0 = __ldg(light_dir + 3 * b), l1 = __ldg(light_dir + 3 * b + 1), l2 = __ldg(light_dir + 3 * b + 2);
@@ -476,10 +597,16 @@ __global__ void __launch_bounds__(256) phong_recon_loss_grad_kernel(const float*
     float t[4] = {0.f, 0.f, 0.f, 0.f};
     for (int w = 0; w < 8; ++w)
       for (int i = 0; i < 4; ++i) t[i] += red[w][i];
-    atomicAdd(loss + b, static_cast<double>(t[0]) / (3.0 * HW));
     const float ldt = L[0] * t[1] + L[1] * t[2] + L[2] * t[3];           // d (l/|l|) = (dL - L (L.dL)) / |l|
-    if (d_light != nullptr)
-      for (int i = 0; i < 3; ++i) atomicAdd(d_light + 3 * b + i, (t[1 + i] - L[i] * ldt) / lnorm);
+    if constexpr (FX) {
+      double* sl = slots + (static_cast<size_t>(b) * gridDim.x + blockIdx.x) * 4;
+      sl[0] = static_cast<double>(t[0]) / (3.0 * HW);
+      for (int i = 0; i < 3; ++i) sl[1 + i] = (t[1 + i] - L[i] * ldt) / lnorm;
+    } else {
+      atomicAdd(loss + b, static_cast<double>(t[0]) / (3.0 * HW));
+      if (d_light != nullptr)
+        for (int i = 0; i < 3; ++i) atomicAdd(d_light + 3 * b + i, (t[1 + i] - L[i] * ldt) / lnorm);
+    }
   }
 }
 
@@ -494,12 +621,14 @@ __global__ void __launch_bounds__(256) phong_recon_loss_grad_kernel(const float*
 // = dd u is reduced over the block and mapped through the light's normalisation (I - L L^T) / |l|.  At img = (0.5, 0.5, 0.5)
 // d is 0 * inf = NaN; phong_pixel's fmaxf turns it into 0 (the pixel is shaded as if unlit) and the gradient passes nothing
 // through the normal there (only the mask term reaches d_img; nothing reaches d_light).  Where |a| = 0 the mask term is 0.
+// FX: slots[b][blockIdx.x][4] as phong_recon_loss_grad_kernel's.
+template <bool FX>
 __global__ void __launch_bounds__(256) phong_composite_loss_grad_kernel(const float* __restrict__ img, const float* __restrict__ target,
                                                                         const float* __restrict__ light_dir,
                                                                         const float* __restrict__ light_col, float ambient,
                                                                         float k_diffuse, int white, int with_mask,
                                                                         double* __restrict__ loss, float* __restrict__ d_img,
-                                                                        float* __restrict__ d_light, int HW) {
+                                                                        float* __restrict__ d_light, int HW, double* __restrict__ slots) {
   __shared__ double red_loss[8];
   __shared__ float red[8][3];
   const int b = blockIdx.y;
@@ -569,10 +698,17 @@ __global__ void __launch_bounds__(256) phong_composite_loss_grad_kernel(const fl
       s += red_loss[w];
       for (int i = 0; i < 3; ++i) v[i] += red[w][i];
     }
-    atomicAdd(loss + b, s / (3.0 * HW));
-    if (d_light != nullptr) {                                          // d (l/|l|) = (dL - L (L.dL)) / |l|
+    if constexpr (FX) {
+      double* sl = slots + (static_cast<size_t>(b) * gridDim.x + blockIdx.x) * 4;
+      sl[0] = s / (3.0 * HW);
       const float ldv = t.L[0] * v[0] + t.L[1] * v[1] + t.L[2] * v[2];
-      for (int i = 0; i < 3; ++i) atomicAdd(d_light + 3 * b + i, (v[i] - t.L[i] * ldv) * t.linv);
+      for (int i = 0; i < 3; ++i) sl[1 + i] = (v[i] - t.L[i] * ldv) * t.linv;
+    } else {
+      atomicAdd(loss + b, s / (3.0 * HW));
+      if (d_light != nullptr) {                                        // d (l/|l|) = (dL - L (L.dL)) / |l|
+        const float ldv = t.L[0] * v[0] + t.L[1] * v[1] + t.L[2] * v[2];
+        for (int i = 0; i < 3; ++i) atomicAdd(d_light + 3 * b + i, (v[i] - t.L[i] * ldv) * t.linv);
+      }
     }
   }
 }
@@ -584,14 +720,15 @@ __global__ void __launch_bounds__(256) phong_composite_loss_grad_kernel(const fl
 // fed the terms its forward recorded in this thread, so the shading differentiated is rn_phong_shade's bit for bit.  dL/dL is
 // reduced over the block and mapped through the forward's normalisation of the light: (I - L L^T) / |l| with the TF composite's
 // division by |l|, or times the NumPy composite's reciprocal 1 / |l|; one atomic per block and component.  One thread per pixel,
-// blockIdx.y = batch item.
-template <bool TF>
+// blockIdx.y = batch item.  FX: the block's three d_light terms go to slots[b][blockIdx.x][3] (summed by slot_sum_kernel).
+template <bool TF, bool FX>
 __global__ void __launch_bounds__(256) phong_shade_backward_kernel(const float* __restrict__ normal, const float* __restrict__ albedo,
                                                                    const float* __restrict__ light_dir,
                                                                    const float* __restrict__ light_col, float ambient,
                                                                    float k_diffuse, int white, int with_mask,
                                                                    const float* __restrict__ g_compos, float* __restrict__ d_normal,
-                                                                   float* __restrict__ d_albedo, float* __restrict__ d_light, int HW) {
+                                                                   float* __restrict__ d_albedo, float* __restrict__ d_light, int HW,
+                                                                   double* __restrict__ slots) {
   __shared__ float red[8][3];
   const int b = blockIdx.y;
   const float l0 = __ldg(light_dir + 3 * b), l1 = __ldg(light_dir + 3 * b + 1), l2 = __ldg(light_dir + 3 * b + 2);
@@ -641,7 +778,7 @@ __global__ void __launch_bounds__(256) phong_shade_backward_kernel(const float* 
       for (int c = 0; c < 3; ++c) d_albedo[o + c] = g[c] * s[c];
     }
   }
-  if (d_light == nullptr) return;                                     // the same in every thread: the barrier below stays whole
+  if (FX ? slots == nullptr : d_light == nullptr) return;             // the same in every thread: the barrier below stays whole
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
@@ -656,8 +793,11 @@ __global__ void __launch_bounds__(256) phong_shade_backward_kernel(const float* 
     for (int w = 0; w < 8; ++w)
       for (int i = 0; i < 3; ++i) v[i] += red[w][i];
     const float ldv = L[0] * v[0] + L[1] * v[1] + L[2] * v[2];       // d (l/|l|) = (dL - L (L.dL)) / |l|
-    for (int i = 0; i < 3; ++i)
-      atomicAdd(d_light + 3 * b + i, TF ? (v[i] - L[i] * ldv) / lscale : (v[i] - L[i] * ldv) * lscale);
+    for (int i = 0; i < 3; ++i) {
+      const float dli = TF ? (v[i] - L[i] * ldv) / lscale : (v[i] - L[i] * ldv) * lscale;
+      if constexpr (FX) slots[(static_cast<size_t>(b) * gridDim.x + blockIdx.x) * 3 + i] = dli;
+      else atomicAdd(d_light + 3 * b + i, dli);
+    }
   }
 }
 
@@ -718,8 +858,14 @@ extern "C" int rn_resample_backward_f32(const float* vox, const float* minv, con
   const long long rows = static_cast<long long>(B) * new_size * new_size;
   const int grid = static_cast<int>((rows * 32 + 255) / 256);
   switch (C) {
-    case 1: resample_backward_kernel<1><<<grid, 256, 0, st>>>(vox, minv, gout, dvox, dminv, B, size, new_size, transform); break;
-    case 4: resample_backward_kernel<4><<<grid, 256, 0, st>>>(vox, minv, gout, dvox, dminv, B, size, new_size, transform); break;
+    case 1:
+      resample_backward_kernel<1, false><<<grid, 256, 0, st>>>(vox, minv, gout, dvox, dminv, B, size, new_size, transform, nullptr,
+                                                               nullptr, 0, nullptr);
+      break;
+    case 4:
+      resample_backward_kernel<4, false><<<grid, 256, 0, st>>>(vox, minv, gout, dvox, dminv, B, size, new_size, transform, nullptr,
+                                                               nullptr, 0, nullptr);
+      break;
     default: return -3;
   }
   RN_COUNT_LAUNCH();
@@ -731,8 +877,8 @@ static int resample5_backward_launch(const float* vox, const float* tex, const f
                                      void* stream) {
   if ((reinterpret_cast<uintptr_t>(tex) & 15) != 0 || (reinterpret_cast<uintptr_t>(dtex) & 15) != 0) return -3;
   const long long rows = static_cast<long long>(B) * ph * pw;
-  resample5_backward_kernel<<<static_cast<int>((rows * 32 + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      vox, tex, minv, gout, dvox, dtex, dminv, B, size, new_size, y0, x0, ph, pw);
+  resample5_backward_kernel<false><<<static_cast<int>((rows * 32 + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      vox, tex, minv, gout, dvox, dtex, dminv, B, size, new_size, y0, x0, ph, pw, nullptr, nullptr, nullptr, 0, nullptr);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }
@@ -797,9 +943,9 @@ extern "C" int rn_phong_recon_loss_grad(const float* albedo, const float* normal
     return -1;
   const int HW = H * W;
   const dim3 grid((HW + 255) / 256, B);
-  phong_recon_loss_grad_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  phong_recon_loss_grad_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       albedo, normal, target, light_dir, light_col, ambient, k_diffuse, black_background, with_mask, loss, d_albedo, d_normal,
-      d_light_dir, HW);
+      d_light_dir, HW, nullptr);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }
@@ -811,8 +957,8 @@ extern "C" int rn_phong_composite_loss_grad(const float* img, const float* targe
   if (static_cast<long long>(H) * W > 0x7fffffffLL - 256 || B > 65535) return -2;
   const int HW = H * W;
   const dim3 grid((HW + 255) / 256, B);
-  phong_composite_loss_grad_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      img, target, light_dir, light_col, ambient, k_diffuse, background_white, with_mask, loss, d_img, d_light_dir, HW);
+  phong_composite_loss_grad_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      img, target, light_dir, light_col, ambient, k_diffuse, background_white, with_mask, loss, d_img, d_light_dir, HW, nullptr);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }
@@ -828,11 +974,209 @@ extern "C" int rn_phong_shade_backward(const float* normal, const float* albedo,
   const dim3 grid((HW + 255) / 256, B);
   const int white = background_white != 0, mask = with_mask != 0;
   if (composite == RN_PHONG_TF)
-    phong_shade_backward_kernel<true><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, g_compos, d_normal, d_albedo, d_light_dir, HW);
+    phong_shade_backward_kernel<true, false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, g_compos, d_normal, d_albedo, d_light_dir, HW,
+        nullptr);
   else
-    phong_shade_backward_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, g_compos, d_normal, d_albedo, d_light_dir, HW);
+    phong_shade_backward_kernel<false, false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, g_compos, d_normal, d_albedo, d_light_dir, HW,
+        nullptr);
   RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+// ------------------------------------------------------------------------------------------ fixed-order twins (entry points)
+namespace rn {
+// the second stage of every twin (also launched by rn_train.cu's rn_image_loss_grad_items_fixed)
+int launch_slot_sum(const double* part, int B, int nblk, int width, int nd, double* out_d, float* out_f, const unsigned* amax,
+                    int namax, cudaStream_t st) {
+  const long long threads = static_cast<long long>(B) * width * 32;
+  slot_sum_kernel<<<static_cast<int>((threads + 255) / 256), 256, 0, st>>>(part, B, nblk, width, nd, out_d, out_f, amax, namax);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+}  // namespace rn
+
+namespace {
+int lg_points(int new_size) {                                          // smallest L with 2^L >= new_size^3
+  const long long n = static_cast<long long>(new_size) * new_size * new_size;
+  int L = 0;
+  while ((1LL << L) < n) ++L;
+  return L;
+}
+long long up8(long long bytes) { return (bytes + 7) / 8 * 8; }
+// workspace of the resampler twins: [acc int64 B*size^3*nacc][slots double B*(new^2/8)*12][amax uint32 B*C]
+long long resample_fixed_bytes(int B, int C, int size, int new_size, int nacc) {
+  const long long vol = static_cast<long long>(size) * size * size;
+  return 8LL * B * vol * nacc + 8LL * B * (static_cast<long long>(new_size) * new_size / 8) * 12 + up8(4LL * B * C);
+}
+int resample_fixed_check(const float* vox, const float* minv, const float* gout, int B, int size, int new_size) {
+  if (!vox || !minv || !gout || B < 1 || size < 2 || new_size < 1) return -1;
+  if ((new_size * new_size) % 8 != 0) return -2;                       // a block's 8 rows must belong to one batch item
+  if (new_size > 1024 || size > 1024) return -2;                       // new_size^3 < 2^31 sample points, 2^L fits int64
+  return 0;
+}
+int grid_items(long long per_item) {                                   // blocks per item of the twins' elementwise stages
+  return grid_for(per_item, 256 * 4, 132 * 4);
+}
+}  // namespace
+
+extern "C" int rn_fixed_point_exponent(float max_abs, int new_size) {
+  if (new_size < 1 || new_size > 1024) return -1000;
+  return fx_exponent(max_abs, lg_points(new_size));
+}
+
+extern "C" long long rn_resample_backward_fixed_workspace(int B, int C, int size, int new_size, int want_dvox) {
+  if (B < 1 || (C != 1 && C != 4) || size < 2 || new_size < 1) return -1;
+  return resample_fixed_bytes(B, C, size, new_size, want_dvox ? C : 0);
+}
+
+extern "C" int rn_resample_backward_fixed_f32(const float* vox, const float* minv, const float* gout, float* dvox, float* dminv,
+                                              int B, int C, int size, int new_size, int transform, void* work, long long work_bytes,
+                                              void* stream) {
+  if (int rc = resample_fixed_check(vox, minv, gout, B, size, new_size)) return rc;
+  if (!dvox && !dminv) return -1;
+  if (C != 1 && C != 4) return -3;
+  if (!work || work_bytes < resample_fixed_bytes(B, C, size, new_size, dvox ? C : 0)) return -4;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long vol = static_cast<long long>(size) * size * size, nbpi = static_cast<long long>(new_size) * new_size / 8;
+  unsigned long long* acc = dvox ? static_cast<unsigned long long*>(work) : nullptr;
+  double* slots = reinterpret_cast<double*>(static_cast<char*>(work) + 8LL * B * vol * (dvox ? C : 0));
+  unsigned* amax = reinterpret_cast<unsigned*>(slots + B * nbpi * 12);
+  const int L = lg_points(new_size);
+  cudaError_t e = cudaMemsetAsync(amax, 0, 4ULL * B * C, st);
+  if (e == cudaSuccess && acc) e = cudaMemsetAsync(acc, 0, 8ULL * B * vol * C, st);
+  if (e != cudaSuccess) return static_cast<int>(e);
+  const long long points = static_cast<long long>(new_size) * new_size * new_size;
+  const dim3 mgrid(grid_items(points), B);
+  const int grid = static_cast<int>(B * nbpi);
+  double* sl = dminv ? slots : nullptr;
+  if (C == 1) {
+    absmax_bits_kernel<1><<<mgrid, 256, 0, st>>>(gout, amax, points);
+    resample_backward_kernel<1, true><<<grid, 256, 0, st>>>(vox, minv, gout, nullptr, nullptr, B, size, new_size, transform, acc,
+                                                            amax, L, sl);
+  } else {
+    absmax_bits_kernel<4><<<mgrid, 256, 0, st>>>(gout, amax, points);
+    resample_backward_kernel<4, true><<<grid, 256, 0, st>>>(vox, minv, gout, nullptr, nullptr, B, size, new_size, transform, acc,
+                                                            amax, L, sl);
+  }
+  RN_COUNT_LAUNCH();
+  RN_COUNT_LAUNCH();
+  if (dvox) {
+    fx_finalize_kernel<<<dim3(grid_items(vol * C), B), 256, 0, st>>>(acc, amax, C, 0, L, dvox, vol * C, C);
+    RN_COUNT_LAUNCH();
+  }
+  if (dminv) return launch_slot_sum(slots, B, static_cast<int>(nbpi), 12, 0, nullptr, dminv, amax, C, st);
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" long long rn_resample5_backward_fixed_workspace(int B, int size, int new_size, int want_dvox, int want_dtex) {
+  if (B < 1 || size < 2 || new_size < 1) return -1;
+  return resample_fixed_bytes(B, 5, size, new_size, (want_dvox ? 1 : 0) + (want_dtex ? 4 : 0));
+}
+
+extern "C" int rn_resample5_backward_fixed_f32(const float* vox, const float* tex, const float* minv, const float* gout, float* dvox,
+                                               float* dtex, float* dminv, int B, int size, int new_size, void* work,
+                                               long long work_bytes, void* stream) {
+  if (int rc = resample_fixed_check(vox, minv, gout, B, size, new_size)) return rc;
+  if (!tex || (!dvox && !dtex && !dminv)) return -1;
+  if ((reinterpret_cast<uintptr_t>(tex) & 15) != 0) return -3;
+  const int nacc = (dvox ? 1 : 0) + (dtex ? 4 : 0);
+  if (!work || work_bytes < resample_fixed_bytes(B, 5, size, new_size, nacc)) return -4;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long vol = static_cast<long long>(size) * size * size, nbpi = static_cast<long long>(new_size) * new_size / 8;
+  unsigned long long* acc_vox = dvox ? static_cast<unsigned long long*>(work) : nullptr;
+  unsigned long long* acc_tex = dtex ? static_cast<unsigned long long*>(work) + (dvox ? B * vol : 0) : nullptr;
+  double* slots = reinterpret_cast<double*>(static_cast<char*>(work) + 8LL * B * vol * nacc);
+  unsigned* amax = reinterpret_cast<unsigned*>(slots + B * nbpi * 12);
+  const int L = lg_points(new_size);
+  cudaError_t e = cudaMemsetAsync(amax, 0, 4ULL * B * 5, st);
+  if (e == cudaSuccess && nacc) e = cudaMemsetAsync(work, 0, 8ULL * B * vol * nacc, st);
+  if (e != cudaSuccess) return static_cast<int>(e);
+  const long long points = static_cast<long long>(new_size) * new_size * new_size;
+  absmax_bits_kernel<5><<<dim3(grid_items(points), B), 256, 0, st>>>(gout, amax, points);
+  RN_COUNT_LAUNCH();
+  resample5_backward_kernel<true><<<static_cast<int>(B * nbpi), 256, 0, st>>>(
+      vox, tex, minv, gout, nullptr, nullptr, nullptr, B, size, new_size, 0, 0, new_size, new_size, acc_vox, acc_tex, amax, L,
+      dminv ? slots : nullptr);
+  RN_COUNT_LAUNCH();
+  if (dvox) {
+    fx_finalize_kernel<<<dim3(grid_items(vol), B), 256, 0, st>>>(acc_vox, amax, 5, 0, L, dvox, vol, 1);
+    RN_COUNT_LAUNCH();
+  }
+  if (dtex) {
+    fx_finalize_kernel<<<dim3(grid_items(vol * 4), B), 256, 0, st>>>(acc_tex, amax, 5, 1, L, dtex, vol * 4, 4);
+    RN_COUNT_LAUNCH();
+  }
+  if (dminv) return launch_slot_sum(slots, B, static_cast<int>(nbpi), 12, 0, nullptr, dminv, amax, 5, st);
+  return static_cast<int>(cudaGetLastError());
+}
+
+// the three Phong twins: one slot row of 4 doubles per (item, 256-pixel block)
+extern "C" long long rn_phong_recon_loss_grad_fixed_workspace(int B, int H, int W) {
+  if (B < 1 || H < 1 || W < 1) return -1;
+  return 8LL * B * ((static_cast<long long>(H) * W + 255) / 256) * 4;
+}
+extern "C" long long rn_phong_composite_loss_grad_fixed_workspace(int B, int H, int W) {
+  return rn_phong_recon_loss_grad_fixed_workspace(B, H, W);
+}
+extern "C" long long rn_phong_shade_backward_fixed_workspace(int B, int H, int W) {
+  return rn_phong_recon_loss_grad_fixed_workspace(B, H, W);
+}
+
+extern "C" int rn_phong_recon_loss_grad_fixed(const float* albedo, const float* normal, const float* target, const float* light_dir,
+                                              const float* light_col, float ambient, float k_diffuse, int black_background,
+                                              int with_mask, double* loss, float* d_albedo, float* d_normal, float* d_light_dir,
+                                              int B, int H, int W, void* work, long long work_bytes, void* stream) {
+  if (!albedo || !normal || !target || !light_dir || !light_col || !loss || !d_albedo || !d_normal || B < 1 || H < 1 || W < 1)
+    return -1;
+  if (static_cast<long long>(H) * W > 0x7fffffffLL - 255 || B > 65535) return -2;
+  if (!work || work_bytes < rn_phong_recon_loss_grad_fixed_workspace(B, H, W)) return -4;
+  const int HW = H * W, nblk = (HW + 255) / 256;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  phong_recon_loss_grad_kernel<true><<<dim3(nblk, B), 256, 0, st>>>(albedo, normal, target, light_dir, light_col, ambient, k_diffuse,
+                                                                      black_background, with_mask, nullptr, d_albedo, d_normal,
+                                                                      nullptr, HW, static_cast<double*>(work));
+  RN_COUNT_LAUNCH();
+  return launch_slot_sum(static_cast<double*>(work), B, nblk, 4, 1, loss, d_light_dir, nullptr, 0, st);
+}
+
+extern "C" int rn_phong_composite_loss_grad_fixed(const float* img, const float* target, const float* light_dir,
+                                                  const float* light_col, float ambient, float k_diffuse, int background_white,
+                                                  int with_mask, double* loss, float* d_img, float* d_light_dir, int B, int H, int W,
+                                                  void* work, long long work_bytes, void* stream) {
+  if (!img || !target || !light_dir || !light_col || !loss || !d_img || B < 1 || H < 1 || W < 1) return -1;
+  if (static_cast<long long>(H) * W > 0x7fffffffLL - 256 || B > 65535) return -2;
+  if (!work || work_bytes < rn_phong_composite_loss_grad_fixed_workspace(B, H, W)) return -4;
+  const int HW = H * W, nblk = (HW + 255) / 256;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  phong_composite_loss_grad_kernel<true><<<dim3(nblk, B), 256, 0, st>>>(img, target, light_dir, light_col, ambient, k_diffuse,
+                                                                          background_white, with_mask, nullptr, d_img, nullptr, HW,
+                                                                          static_cast<double*>(work));
+  RN_COUNT_LAUNCH();
+  return launch_slot_sum(static_cast<double*>(work), B, nblk, 4, 1, loss, d_light_dir, nullptr, 0, st);
+}
+
+extern "C" int rn_phong_shade_backward_fixed(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
+                                             float ambient, float k_diffuse, int composite, int background_white, int with_mask,
+                                             const float* g_compos, float* d_normal, float* d_albedo, float* d_light_dir, int B,
+                                             int H, int W, void* work, long long work_bytes, void* stream) {
+  if (!normal || !light_dir || !light_col || !g_compos || !d_normal || B < 1 || H < 1 || W < 1) return -1;
+  if (composite != RN_PHONG_NUMPY && composite != RN_PHONG_TF) return -1;
+  if (B > 65535 || static_cast<long long>(H) * W > 0x7fffffffLL - 255) return -2;
+  if (d_light_dir && (!work || work_bytes < rn_phong_shade_backward_fixed_workspace(B, H, W))) return -4;
+  const int HW = H * W, nblk = (HW + 255) / 256;
+  const dim3 grid(nblk, B);
+  const int white = background_white != 0, mask = with_mask != 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* slots = d_light_dir ? static_cast<double*>(work) : nullptr;
+  if (composite == RN_PHONG_TF)
+    phong_shade_backward_kernel<true, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, ambient, k_diffuse, white,
+                                                                  mask, g_compos, d_normal, d_albedo, nullptr, HW, slots);
+  else
+    phong_shade_backward_kernel<false, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, ambient, k_diffuse, white,
+                                                                   mask, g_compos, d_normal, d_albedo, nullptr, HW, slots);
+  RN_COUNT_LAUNCH();
+  if (d_light_dir) return launch_slot_sum(slots, B, nblk, 3, 0, nullptr, d_light_dir, nullptr, 0, st);
   return static_cast<int>(cudaGetLastError());
 }

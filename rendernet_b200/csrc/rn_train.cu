@@ -26,6 +26,8 @@
 
 namespace rn {
 extern std::atomic<long long> g_launch_count;
+int launch_slot_sum(const double* part, int B, int nblk, int width, int nd, double* out_d, float* out_f, const unsigned* amax,
+                    int namax, cudaStream_t st);                        // rn_backward.cu
 }
 #define RN_COUNT_LAUNCH() rn::g_launch_count.fetch_add(1, std::memory_order_relaxed)
 
@@ -348,10 +350,12 @@ __global__ void __launch_bounds__(256) image_loss_grad_kernel(const float* __res
 
 // Per item (rn_image_loss_grad_items): blockIdx.y = item b of m elements.  kind 0: loss[b] = mean (p - t)^2, dL/dp = 2 (p - t) / m;
 // kind 1: loss[b] = -sum [t log(1e-6 + p) + (1 - t) log(1e-6 + 1 - p)], dL/dp = -(t / (1e-6 + p) - (1 - t) / (1e-6 + 1 - p)).
-// dimg is the gradient of sum_b loss[b].  One double atomic per block.
+// dimg is the gradient of sum_b loss[b].  One double atomic per block; FX (the fixed-order twin): the block's term goes to
+// slots[b][blockIdx.x] instead, summed in block order by rn::launch_slot_sum.
+template <bool FX>
 __global__ void __launch_bounds__(256) image_loss_grad_items_kernel(const float* __restrict__ img, const float* __restrict__ target,
                                                                     float* __restrict__ dimg, double* __restrict__ loss, long long m,
-                                                                    int kind) {
+                                                                    int kind, double* __restrict__ slots) {
   __shared__ double red[256];
   const long long base = static_cast<long long>(blockIdx.y) * m;
   double s = 0.0;
@@ -376,7 +380,11 @@ __global__ void __launch_bounds__(256) image_loss_grad_items_kernel(const float*
     if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
     __syncthreads();
   }
-  if (threadIdx.x == 0) atomicAdd(loss + blockIdx.y, kind == 0 ? red[0] / static_cast<double>(m) : red[0]);
+  if (threadIdx.x == 0) {
+    const double v = kind == 0 ? red[0] / static_cast<double>(m) : red[0];
+    if constexpr (FX) slots[static_cast<size_t>(blockIdx.y) * gridDim.x + blockIdx.x] = v;
+    else atomicAdd(loss + blockIdx.y, v);
+  }
 }
 
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
@@ -623,9 +631,31 @@ extern "C" int rn_image_loss_grad_items(const float* img, const float* target, f
   const long long m = npix * C;
   const int per_item = (132 * 4 + batch - 1) / batch;
   const dim3 grid(static_cast<unsigned>(grid_for(m, 256 * 8, per_item)), static_cast<unsigned>(batch));
-  image_loss_grad_items_kernel<<<grid, 256, 0, st>>>(img, target, dimg, loss, m, kind);
+  image_loss_grad_items_kernel<false><<<grid, 256, 0, st>>>(img, target, dimg, loss, m, kind, nullptr);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
+}
+
+// the fixed-order twin: the block count per item depends on the item's size alone, so an item's loss does not depend on the batch
+static int image_loss_items_blocks(long long m) { return grid_for(m, 256 * 8, 132 * 4); }
+
+extern "C" long long rn_image_loss_grad_items_fixed_workspace(long long npix, int C, int batch) {
+  if (npix < 1 || (C != 1 && C != 3) || batch < 1) return -1;
+  return 8LL * batch * image_loss_items_blocks(npix * C);
+}
+
+extern "C" int rn_image_loss_grad_items_fixed(const float* img, const float* target, float* dimg, double* loss, long long npix, int C,
+                                              int batch, int kind, void* work, long long work_bytes, void* stream) {
+  if (!img || !target || !loss || npix < 1 || (C != 1 && C != 3) || batch < 1 || batch > 65535 || (kind != 0 && kind != 1))
+    return -1;
+  if (!work || work_bytes < rn_image_loss_grad_items_fixed_workspace(npix, C, batch)) return -4;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long m = npix * C;
+  const int nblk = image_loss_items_blocks(m);
+  image_loss_grad_items_kernel<true><<<dim3(nblk, batch), 256, 0, st>>>(img, target, dimg, nullptr, m, kind,
+                                                                          static_cast<double*>(work));
+  RN_COUNT_LAUNCH();
+  return rn::launch_slot_sum(static_cast<double*>(work), batch, nblk, 1, 1, loss, nullptr, nullptr, 0, st);
 }
 
 extern "C" int rn_adam_step(float* param, const float* grad, float* m, float* v, long long n, float lr_t, float beta1, float beta2,

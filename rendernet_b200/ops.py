@@ -6,6 +6,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import warnings
 from dataclasses import dataclass
 from typing import Optional, Sequence
 
@@ -23,6 +24,29 @@ def _stream() -> int:
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
+
+
+# --------------------------------------------------------------------------- torch.use_deterministic_algorithms (DESIGN §8b)
+# Under PyTorch's flag the input-gradient ops that sum with float atomics call their fixed-order twins (rn_*_fixed: the same
+# bits on every run, whatever the batch); the ops without a twin follow PyTorch's rule: raise, or warn under warn_only.
+def _fixed_order() -> bool:
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def _alert_no_fixed_order(op: str) -> None:
+    if not torch.are_deterministic_algorithms_enabled():
+        return
+    msg = (f"{op} sums with float atomics and has no deterministic implementation, but torch.use_deterministic_algorithms(True) "
+           "is set (rendernet_b200 reproduces input gradients and the fits, not the Shader / Texture+Normal training step)")
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg, UserWarning, stacklevel=3)
+    else:
+        raise RuntimeError(msg)
+
+
+def _workspace(nbytes: int, device) -> torch.Tensor:
+    """Caller-owned workspace of a fixed-order twin (a failed size query, < 0, leaves the twin to reject its arguments)."""
+    return torch.empty(max(int(nbytes), 8), device=device, dtype=torch.uint8)
 
 
 class Split16:
@@ -903,6 +927,15 @@ def phong_shade_backward(normal: torch.Tensor, g_compos: torch.Tensor, light_dir
     albedo = None if albedo is None else _cuda(albedo, torch.float32)
     d_normal = torch.empty_like(normal)
     d_albedo = None if albedo is None else torch.empty_like(normal)
+    if _fixed_order():
+        d_light = torch.empty((B, 3), device=normal.device, dtype=torch.float32) if want_light_grad else None
+        work = _workspace(lib.rn_phong_shade_backward_fixed_workspace(B, H, W), normal.device) if want_light_grad else None
+        check(lib.rn_phong_shade_backward_fixed(normal.data_ptr(), _ptr(albedo), ld.data_ptr(), lc.data_ptr(), float(ambient),
+                                                float(k_diffuse), PHONG_COMPOSITES[composite], 1 if background_white else 0,
+                                                1 if with_mask else 0, g_compos.data_ptr(), d_normal.data_ptr(), _ptr(d_albedo),
+                                                _ptr(d_light), B, H, W, _ptr(work), 0 if work is None else work.numel(), _stream()),
+              "rn_phong_shade_backward_fixed")
+        return d_normal, d_albedo, d_light
     d_light = torch.zeros((B, 3), device=normal.device, dtype=torch.float32) if want_light_grad else None
     check(lib.rn_phong_shade_backward(normal.data_ptr(), _ptr(albedo), ld.data_ptr(), lc.data_ptr(), float(ambient),
                                       float(k_diffuse), PHONG_COMPOSITES[composite], 1 if background_white else 0,
@@ -1149,6 +1182,14 @@ def resample_backward(vox: torch.Tensor, minv: torch.Tensor, gout: torch.Tensor,
     vox, minv, gout = _cuda(vox, torch.float32), _cuda(minv, torch.float32), _cuda(gout, torch.float32)
     B, S, _, _, Cc = vox.shape
     N = gout.shape[1]
+    if _fixed_order():
+        dvox = torch.empty_like(vox) if want_dvox else None
+        dminv = torch.empty_like(minv) if want_dminv else None
+        work = _workspace(lib.rn_resample_backward_fixed_workspace(B, Cc, S, N, 1 if want_dvox else 0), vox.device)
+        check(lib.rn_resample_backward_fixed_f32(vox.data_ptr(), minv.data_ptr(), gout.data_ptr(), _ptr(dvox), _ptr(dminv), B, Cc, S,
+                                                 N, 1 if transform else 0, work.data_ptr(), work.numel(), _stream()),
+              "rn_resample_backward_fixed_f32")
+        return dvox, dminv
     dvox = torch.zeros_like(vox) if want_dvox else None
     dminv = torch.zeros_like(minv) if want_dminv else None
     check(lib.rn_resample_backward_f32(vox.data_ptr(), minv.data_ptr(), gout.data_ptr(), _ptr(dvox), _ptr(dminv), B, Cc, S, N,
@@ -1173,6 +1214,18 @@ def resample5_backward(vox: torch.Tensor, tex: torch.Tensor, minv: torch.Tensor,
     if (tuple(vox.shape) != (B, S, S, S, 1) or tuple(tex.shape) != (B, S, S, S, 4) or tuple(minv.shape) != (B, 3, 4)
             or tuple(gout.shape) != (B, ph, pw, N, 5)):
         raise ValueError(f"resample5_backward: unsupported shapes {tuple(vox.shape)}, {tuple(tex.shape)}, {tuple(gout.shape)}")
+    if window is None and _fixed_order():
+        dvox = torch.empty_like(vox) if want_dvox else None
+        dtex = torch.empty_like(tex) if want_dtex else None
+        dminv = torch.empty_like(minv) if want_dminv else None
+        work = _workspace(lib.rn_resample5_backward_fixed_workspace(B, S, N, 1 if want_dvox else 0, 1 if want_dtex else 0),
+                          vox.device)
+        check(lib.rn_resample5_backward_fixed_f32(vox.data_ptr(), tex.data_ptr(), minv.data_ptr(), gout.data_ptr(), _ptr(dvox),
+                                                  _ptr(dtex), _ptr(dminv), B, S, N, work.data_ptr(), work.numel(), _stream()),
+              "rn_resample5_backward_fixed_f32")
+        return dvox, dtex, dminv
+    if window is not None:
+        _alert_no_fixed_order("rn_resample5_backward_window_f32")
     dvox = torch.zeros_like(vox) if want_dvox else None
     dtex = torch.zeros_like(tex) if want_dtex else None
     dminv = torch.zeros_like(minv) if want_dminv else None
@@ -1228,8 +1281,18 @@ def phong_recon_loss_grad(albedo: torch.Tensor, normal: torch.Tensor, target: to
         raise ValueError(f"phong_recon_loss_grad: shapes {tuple(albedo.shape)}, {tuple(normal.shape)}, {tuple(target.shape)}")
     ld, lc = (_cuda(t.to(device=albedo.device, dtype=torch.float32).reshape(-1, 3).expand(B, 3).contiguous(), torch.float32)
               for t in (light_dir, light_col))
-    loss = torch.zeros(B, device=albedo.device, dtype=torch.float64)
     d_albedo, d_normal = torch.empty_like(albedo), torch.empty_like(albedo)
+    if _fixed_order():
+        loss = torch.empty(B, device=albedo.device, dtype=torch.float64)
+        d_light = torch.empty((B, 3), device=albedo.device, dtype=torch.float32)
+        work = _workspace(lib.rn_phong_recon_loss_grad_fixed_workspace(B, H, W), albedo.device)
+        check(lib.rn_phong_recon_loss_grad_fixed(albedo.data_ptr(), normal.data_ptr(), target.data_ptr(), ld.data_ptr(), lc.data_ptr(),
+                                                 float(ambient), float(k_diffuse), 1 if black_background else 0,
+                                                 1 if with_mask else 0, loss.data_ptr(), d_albedo.data_ptr(), d_normal.data_ptr(),
+                                                 d_light.data_ptr(), B, H, W, work.data_ptr(), work.numel(), _stream()),
+              "rn_phong_recon_loss_grad_fixed")
+        return loss, d_albedo, d_normal, d_light
+    loss = torch.zeros(B, device=albedo.device, dtype=torch.float64)
     d_light = torch.zeros((B, 3), device=albedo.device, dtype=torch.float32)
     check(lib.rn_phong_recon_loss_grad(albedo.data_ptr(), normal.data_ptr(), target.data_ptr(), ld.data_ptr(), lc.data_ptr(),
                                        float(ambient), float(k_diffuse), 1 if black_background else 0, 1 if with_mask else 0,
@@ -1254,8 +1317,17 @@ def phong_composite_loss_grad(img: torch.Tensor, target: torch.Tensor, light_dir
     ld = _light_rows(light_dir, B, img.device, "light_dir")
     lc = _light_rows(light_col, B, img.device, "light_col")
     img, target = _cuda(img, torch.float32), _cuda(target, torch.float32)
-    loss = torch.zeros(B, device=img.device, dtype=torch.float64)
     d_img = torch.empty_like(img)
+    if _fixed_order():
+        loss = torch.empty(B, device=img.device, dtype=torch.float64)
+        d_light = torch.empty((B, 3), device=img.device, dtype=torch.float32) if want_light_grad else None
+        work = _workspace(lib.rn_phong_composite_loss_grad_fixed_workspace(B, H, W), img.device)
+        check(lib.rn_phong_composite_loss_grad_fixed(img.data_ptr(), target.data_ptr(), ld.data_ptr(), lc.data_ptr(), float(ambient),
+                                                     float(k_diffuse), 1 if background_white else 0, 1 if with_mask else 0,
+                                                     loss.data_ptr(), d_img.data_ptr(), _ptr(d_light), B, H, W, work.data_ptr(),
+                                                     work.numel(), _stream()), "rn_phong_composite_loss_grad_fixed")
+        return loss, d_img, d_light
+    loss = torch.zeros(B, device=img.device, dtype=torch.float64)
     d_light = torch.zeros((B, 3), device=img.device, dtype=torch.float32) if want_light_grad else None
     check(lib.rn_phong_composite_loss_grad(img.data_ptr(), target.data_ptr(), ld.data_ptr(), lc.data_ptr(), float(ambient),
                                            float(k_diffuse), 1 if background_white else 0, 1 if with_mask else 0, loss.data_ptr(),
@@ -1273,6 +1345,7 @@ def conv2d_weight_grad(x, g, kh: int, kw: int) -> torch.Tensor:
     B, H, W, Cin = x.shape
     Cout = g.shape[-1]
     assert tuple(g.shape[:3]) == (B, H, W)
+    _alert_no_fixed_order("rn_conv2d_weight_grad")
     dw = torch.empty((kh, kw, Cin, Cout), device=x.device, dtype=torch.float32)
     check(lib.rn_conv2d_weight_grad(x.data_ptr(), g.data_ptr(), dw.data_ptr(), B, H, W, Cin, Cout, kh, kw, fmt, _stream()),
           "rn_conv2d_weight_grad")
@@ -1284,6 +1357,7 @@ def bias_grad(g) -> torch.Tensor:
     g = _cuda(g)
     fmt = 2 if isinstance(g, Split16) else fmt_of(g.dtype)
     Cc = g.shape[-1]
+    _alert_no_fixed_order("rn_bias_grad_16")
     db = torch.empty(Cc, device=g.device, dtype=torch.float32)
     check(lib.rn_bias_grad_16(g.data_ptr(), db.data_ptr(), g.numel() // Cc, Cc, fmt, _stream()), "rn_bias_grad_16")
     return db
@@ -1317,6 +1391,7 @@ def conv_weight_grad_direct(P, Q, ksize: Sequence[int], stride: Sequence[int], p
     _, Dq, Hq, Wq, Cbp = (int(v) for v in Q5)
     assert int(Q5[0]) == B
     Ca, Cb = int(Ca or Cap), int(Cb or Cbp)
+    _alert_no_fixed_order("rn_conv_weight_grad_direct")
     dW = torch.empty(tuple(int(k) for k in ksize) + (Ca, Cb), device=P.device, dtype=torch.float32)
     check(lib.rn_conv_weight_grad_direct(P.data_ptr(), Q.data_ptr(), dW.data_ptr(), B, Dp, Hp, Wp, Ca, Cap, Dq, Hq, Wq, Cb, Cbp,
                                          int(ks[0]), int(ks[1]), int(ks[2]), int(st[0]), int(st[1]), int(st[2]),
@@ -1332,6 +1407,7 @@ def prelu_alpha_grad(g, z, scale: float = 1.0) -> torch.Tensor:
     if isinstance(z, Split16) != (fmt == 2) or tuple(z.shape) != tuple(g.shape):
         raise TypeError("prelu_alpha_grad: g and z must share shape and 16-bit format")
     Cc = int(g.shape[-1])
+    _alert_no_fixed_order("rn_prelu_alpha_grad")
     da = torch.empty(Cc, device=g.device, dtype=torch.float32)
     check(lib.rn_prelu_alpha_grad(g.data_ptr(), z.data_ptr(), da.data_ptr(), g.numel(), Cc, fmt, float(scale), _stream()),
           "rn_prelu_alpha_grad")
@@ -1375,6 +1451,7 @@ def prelu_grad_f32(gy: torch.Tensor, z: torch.Tensor, alpha: torch.Tensor):
     alpha = _cuda(alpha.to(device=gy.device, dtype=torch.float32))
     if alpha.numel() != Cc:
         raise ValueError(f"prelu_grad_f32: {alpha.numel()} slopes for {Cc} channels")
+    _alert_no_fixed_order("rn_prelu_grad_f32")
     gz = torch.empty_like(gy)
     db = torch.empty(Cc, device=gy.device, dtype=torch.float32)
     da = torch.empty(Cc, device=gy.device, dtype=torch.float32)
@@ -1408,6 +1485,7 @@ def image_loss_grad(img: torch.Tensor, target: torch.Tensor, kind: str = "mse", 
     -> (loss: 0-d float64 device tensor, dimg fp32 like img or None)."""
     img, target = _cuda(img, torch.float32), _cuda(target, torch.float32)
     assert tuple(img.shape) == tuple(target.shape) and img.is_contiguous() and target.is_contiguous()
+    _alert_no_fixed_order("rn_image_loss_grad")
     loss = torch.empty((), device=img.device, dtype=torch.float64)
     dimg = torch.empty_like(img) if want_grad else None
     check(lib.rn_image_loss_grad(img.data_ptr(), target.data_ptr(), _ptr(dimg), loss.data_ptr(), img.numel(), int(img.shape[0]),
@@ -1432,6 +1510,12 @@ def image_loss_grad_items(img: torch.Tensor, target: torch.Tensor, kind: str = "
     B, H, W, C_ = img.shape
     loss = torch.empty(B, device=img.device, dtype=torch.float64)
     dimg = torch.empty_like(img) if want_grad else None
+    if _fixed_order():
+        work = _workspace(lib.rn_image_loss_grad_items_fixed_workspace(H * W, C_, B), img.device)
+        check(lib.rn_image_loss_grad_items_fixed(img.data_ptr(), target.data_ptr(), _ptr(dimg), loss.data_ptr(), H * W, C_, B,
+                                                 IMAGE_LOSSES[kind], work.data_ptr(), work.numel(), _stream()),
+              "rn_image_loss_grad_items_fixed")
+        return loss, dimg
     check(lib.rn_image_loss_grad_items(img.data_ptr(), target.data_ptr(), _ptr(dimg), loss.data_ptr(), H * W, C_, B,
                                        IMAGE_LOSSES[kind], _stream()), "rn_image_loss_grad_items")
     return loss, dimg
