@@ -111,8 +111,9 @@ typedef struct rn_conv_desc {
   const void* x;            /* 16-bit [B,H,W,(D),Cin] */
   const void* w_packed;     /* 16-bit [ntaps][cout_pad][Cin] */
   const float* bias;        /* fp32 [cout_pad], or NULL: the raw fp32 sums, stored straight from the accumulators (out32
-                             * only, act none, no residual, Cout = cout_pad, 8-byte aligned rows; a kernel variant built for
-                             * it, today the exact-mode N = 256 one of rn_winograd_gemm, else an error) */
+                             * only, act none, no residual, Cout = cout_pad, 8-byte aligned rows).  The only kernel built for
+                             * it is the exact-mode (fmt 2) one with N tile 256 and no banded filter (rn_winograd_gemm);
+                             * any other raw plan is rejected with -25 */
   const float* alpha;       /* fp32 [cout_pad] or NULL */
   int act;                  /* RN_ACT_* */
   const void* residual;     /* NULL, or same indexing as the output */
@@ -142,7 +143,8 @@ typedef struct rn_conv_desc {
   int o_nsplit;
   long long o_nhi;
   /* fmt == RN_FMT_F16X2: element offsets of the LO plane of x, of w_packed and of out16 / a 16-bit residual (multiples
-   * of 8).  The reference-shaped wrappers below derive them from the tensor shapes ([2][numel] pairs). */
+   * of 8; o_plane > 0 whenever out16 or a 16-bit residual is given, else -18).  The reference-shaped wrappers below
+   * derive them from the tensor shapes ([2][numel] pairs). */
   long long x_plane, w_plane, o_plane;
   /* accepted and ignored (kept so that the struct layout stays stable): the sm_90 kernel has a single epilogue form, two
    * consumer warpgroups storing their own rows directly */
@@ -152,6 +154,8 @@ typedef struct rn_conv_desc {
    * 16 per-position GEMMs of a Winograd convolution as one launch.  0 = off. */
   int b_tap_div;
 } rn_conv_desc;
+/* Besides the argument codes of the source, -25 = no kernel variant is built for the plan (N tile, cluster, M sub-tiles,
+ * exact mode, banded half blocks, raw output) that the descriptor leads to; rn_conv_plan reports it as well. */
 int rn_conv_igemm(const rn_conv_desc* d, void* stream);
 /* Per-call overrides of the launch heuristics for the reference-shaped wrappers below (their last argument before
  * `stream`; NULL = library defaults).  0 = default for every field; cluster 1/2/4; cta_group 1; kps = k-groups per

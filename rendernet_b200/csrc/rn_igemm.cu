@@ -28,31 +28,19 @@
 
 namespace rn {
 
-// launch_ms<BN, CL, MS, SPLIT, HALF, RAW> is defined in rn_igemm_kernel.cuh and explicitly instantiated once per variant
-// (rn_igemm_inst.cu x the Makefile's VARIANTS list); this table must list exactly those variants.
+// launch_ms<BN, CL, MS, SPLIT, HALF, RAW> is defined in rn_igemm_kernel.cuh and explicitly instantiated once per row of
+// RN_IGEMM_VARIANTS (rn_igemm.cuh; rn_igemm_inst.cu x the Makefile's VARIANTS list).
 template <int BN, int CL, int MS, bool SPLIT, bool HALF, bool RAW>
 cudaError_t launch_ms(const IgemmParams& p, int grid, size_t smem, cudaStream_t stream);
 
 static cudaError_t launch_variant(int BN, int CL, int MS, int SP, int HF, int RW, const IgemmParams& p, int grid, size_t smem,
                                   cudaStream_t stream) {
-#define RN_V(bn, cl, ms, sp, hf) RN_VR(bn, cl, ms, sp, hf, 0)
-#define RN_VR(bn, cl, ms, sp, hf, rw) \
+#define RN_V(bn, cl, ms, sp, hf, rw) \
   if (BN == bn && CL == cl && MS == ms && SP == sp && HF == hf && RW == rw) \
     return launch_ms<bn, cl, ms, (sp != 0), (hf != 0), (rw != 0)>(p, grid, smem, stream);
-  RN_V(256, 1, 1, 0, 0) RN_V(256, 2, 1, 0, 0) RN_V(256, 4, 1, 0, 0)
-  RN_V(128, 1, 1, 0, 0) RN_V(128, 2, 1, 0, 0) RN_V(128, 4, 1, 0, 0) RN_V(128, 1, 2, 0, 0) RN_V(128, 2, 2, 0, 0) RN_V(128, 4, 2, 0, 0)
-  RN_V(64, 1, 1, 0, 0) RN_V(64, 1, 2, 0, 0) RN_V(32, 1, 1, 0, 0) RN_V(32, 1, 2, 0, 0) RN_V(16, 1, 1, 0, 0) RN_V(16, 1, 2, 0, 0)
-  // operand-split "exact" mode (fmt 2): single CTAs
-  RN_V(256, 1, 1, 1, 0) RN_V(128, 1, 1, 1, 0) RN_V(128, 1, 2, 1, 0) RN_V(64, 1, 1, 1, 0) RN_V(64, 1, 2, 1, 0)
-  RN_V(32, 1, 1, 1, 0) RN_V(32, 1, 2, 1, 0) RN_V(16, 1, 1, 1, 0) RN_V(16, 1, 2, 1, 0)
-  // banded filters (N tile 128) with half-tile K blocks
-  RN_V(128, 1, 1, 0, 1) RN_V(128, 2, 1, 0, 1) RN_V(128, 4, 1, 0, 1) RN_V(128, 1, 2, 0, 1) RN_V(128, 2, 2, 0, 1)
-  RN_V(128, 4, 2, 0, 1) RN_V(128, 1, 1, 1, 1) RN_V(128, 1, 2, 1, 1)
-  // raw fp32 output (no bias): the exact-mode Winograd per-position GEMM
-  RN_VR(256, 1, 1, 1, 0, 1)
+  RN_IGEMM_VARIANTS(RN_V)
 #undef RN_V
-#undef RN_VR
-  return cudaErrorInvalidDeviceFunction;   // plan_conv chose a variant that is not built
+  return cudaErrorInvalidDeviceFunction;   // unreachable: plan_conv rejects a plan without a built variant (-25)
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -151,7 +139,8 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
   if (d->ndim != 2 && d->ndim != 3) return -2;
   if (d->ntaps < 1 || d->ntaps * (d->fmt == 2 ? 3 : 1) > kMaxTaps) return -3;
   if (d->fmt < 0 || d->fmt > 2) return -17;
-  if (d->fmt == 2 && (d->x_plane <= 0 || d->w_plane <= 0 || (d->out16 != nullptr && d->o_plane <= 0) ||
+  const bool res16 = d->residual != nullptr && !d->residual_is_f32;
+  if (d->fmt == 2 && (d->x_plane <= 0 || d->w_plane <= 0 || ((d->out16 != nullptr || res16) && d->o_plane <= 0) ||
                       d->x_plane % 8 != 0 || d->w_plane % 8 != 0 || d->o_plane % 8 != 0))
     return -18;   // fp16 hi/lo pairs: the LO plane of every 16-bit tensor must be given (16-byte aligned offsets)
   if (d->Cin % 16 != 0 || d->cout_pad % 16 != 0 || d->Cout > d->cout_pad || d->Cout < 1) return -4;
@@ -274,6 +263,7 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
     else p.ny = 1;                          // then without halo sharing
   }
   if (p.stages < 2) return -10;
+  if (!igemm_variant_built(BN, CL, p.ms, p.split, p.band_half, raw ? 1 : 0)) return -25;
   if (!split) {
     for (int t = 0; t < d->ntaps; ++t) {
       p.tap[t][0] = d->taps[3 * t + 0];

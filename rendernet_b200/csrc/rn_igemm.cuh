@@ -12,6 +12,33 @@ constexpr int kTileM = 128;  // rows (pixels / voxels) per CTA (sub-)tile: 64 pe
 
 enum Act : int { ACT_NONE = 0, ACT_PRELU = 1, ACT_SIGMOID = 2 };
 
+// Every built igemm_kernel variant X(BN, CL, MS, SPLIT, HALF, RAW): N tile, cluster size, M sub-tiles, operand-split exact
+// mode, half-tile K blocks of banded filters, raw fp32 output.  rn_igemm_inst.cu is compiled once per row (the Makefile's
+// VARIANTS list, which tests/test_igemm_variants_host.py pins equal to this table); launch_variant dispatches over it and
+// plan_conv rejects a plan that names no row of it.
+#define RN_IGEMM_VARIANTS(X)                                                                                              \
+  X(256, 1, 1, 0, 0, 0) X(256, 2, 1, 0, 0, 0) X(256, 4, 1, 0, 0, 0)                                                        \
+  X(128, 1, 1, 0, 0, 0) X(128, 2, 1, 0, 0, 0) X(128, 4, 1, 0, 0, 0) X(128, 1, 2, 0, 0, 0) X(128, 2, 2, 0, 0, 0)            \
+  X(128, 4, 2, 0, 0, 0)                                                                                                    \
+  X(64, 1, 1, 0, 0, 0) X(64, 1, 2, 0, 0, 0) X(32, 1, 1, 0, 0, 0) X(32, 1, 2, 0, 0, 0) X(16, 1, 1, 0, 0, 0)                 \
+  X(16, 1, 2, 0, 0, 0)                                                                                                     \
+  /* operand-split "exact" mode (fmt 2): single CTAs */                                                                    \
+  X(256, 1, 1, 1, 0, 0) X(128, 1, 1, 1, 0, 0) X(128, 1, 2, 1, 0, 0) X(64, 1, 1, 1, 0, 0) X(64, 1, 2, 1, 0, 0)              \
+  X(32, 1, 1, 1, 0, 0) X(32, 1, 2, 1, 0, 0) X(16, 1, 1, 1, 0, 0) X(16, 1, 2, 1, 0, 0)                                      \
+  /* banded filters (N tile 128) with half-tile K blocks */                                                                \
+  X(128, 1, 1, 0, 1, 0) X(128, 2, 1, 0, 1, 0) X(128, 4, 1, 0, 1, 0) X(128, 1, 2, 0, 1, 0) X(128, 2, 2, 0, 1, 0)            \
+  X(128, 4, 2, 0, 1, 0) X(128, 1, 1, 1, 1, 0) X(128, 1, 2, 1, 1, 0)                                                        \
+  /* raw fp32 output (no bias): the exact-mode Winograd per-position GEMM */                                               \
+  X(256, 1, 1, 1, 0, 1)
+
+inline bool igemm_variant_built(int BN, int CL, int MS, int SP, int HF, int RW) {
+#define RN_IGEMM_IS(bn, cl, ms, sp, hf, rw) \
+  if (BN == bn && CL == cl && MS == ms && SP == sp && HF == hf && RW == rw) return true;
+  RN_IGEMM_VARIANTS(RN_IGEMM_IS)
+#undef RN_IGEMM_IS
+  return false;
+}
+
 struct alignas(64) IgemmParams {
   CUtensorMap tmA;  // activations, channel-last: rank 4 {C,W,H,B} or rank 5 {C,D,W,H,B}; box {KB,[BD],BW,BH,1}
   CUtensorMap tmB;  // weights [tap][CoutPad][Cin]: rank 3 {Cin,CoutPad,taps}; box {KB,BN,1}

@@ -689,7 +689,7 @@ def conv_igemm_raw(x, w_packed, bias, taps, ndim, B, H, W, D, Cin, Cout, cout_pa
                    alpha=None, act=ACT_NONE, residual=None, o=None, fmt=0, force_bn=0, force_kps=0, max_ctas=0,
                    cluster=0, cta_group=0, ny=0, tile_w=0, msub=0, epi_groups=0, res_prefetch=0, tma_store=0):
     """Direct access to rn_conv_igemm for tests / tuning.  taps: list of (dx,dy,dz).  fmt 2: x, w_packed, out16 and a
-    16-bit residual are [2, ...] hi/lo plane tensors (or Split16)."""
+    16-bit residual are [2, ...] hi/lo plane tensors (or Split16).  bias None: the raw fp32 sums (out32 only)."""
     n = len(taps)
     arr = (C.c_int8 * (3 * n))(*[v for t in taps for v in t])
     x, w_packed, out16, residual = _unwrap(x), _unwrap(w_packed), _unwrap(out16), _unwrap(residual)
@@ -697,7 +697,7 @@ def conv_igemm_raw(x, w_packed, bias, taps, ndim, B, H, W, D, Cin, Cout, cout_pa
     d.ndim, d.B, d.H, d.W, d.D = ndim, B, H, W, D
     d.Cin, d.Cout, d.cout_pad, d.ntaps = Cin, Cout, cout_pad, n
     d.taps = C.cast(arr, C.c_void_p)
-    d.x, d.w_packed, d.bias, d.alpha = x.data_ptr(), w_packed.data_ptr(), bias.data_ptr(), _ptr(alpha)
+    d.x, d.w_packed, d.bias, d.alpha = x.data_ptr(), w_packed.data_ptr(), _ptr(bias), _ptr(alpha)
     d.act = act
     d.residual = _ptr(residual)
     d.residual_is_f32 = 1 if (residual is not None and residual.dtype == torch.float32) else 0
@@ -716,7 +716,8 @@ def conv_igemm_raw(x, w_packed, bias, taps, ndim, B, H, W, D, Cin, Cout, cout_pa
     if fmt == 2:
         d.x_plane = x.numel() // 2
         d.w_plane = w_packed.numel() // 2
-        d.o_plane = (out16.numel() // 2) if out16 is not None else 0
+        planes16 = out16 if out16 is not None else (residual if d.residual and not d.residual_is_f32 else None)
+        d.o_plane = (planes16.numel() // 2) if planes16 is not None else 0     # LO plane of out16 and a 16-bit residual
     check(lib.rn_conv_igemm(C.byref(d), _stream()), "rn_conv_igemm")
 
 
