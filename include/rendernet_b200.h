@@ -16,9 +16,12 @@
  *     exactly the reference's layouts (tools/layer_util.py:228,147; SURVEY.md §8b).
  *   - "16-bit" tensors (`fmt`): RN_FMT_F16 = IEEE fp16, RN_FMT_BF16 = bfloat16, RN_FMT_F16X2 = "exact" mode: a PAIR of
  *     fp16 planes stored back to back, [2][numel]: plane 0 = hi = fp16(v), plane 1 = lo = fp16(v - hi), together ~22
- *     significant bits.  In that mode every convolution evaluates x_hi.w_hi + x_lo.w_hi + x_hi.w_lo on the tensor cores
- *     (3x the MMAs) and matches the reference's fp32 convolutions (tools/layer_util.py:171,212,253) to ~1e-6 relative;
- *     packed filters, 16-bit activations, residuals and outputs are all such pairs (buffers twice the size).
+ *     significant bits while |v| >= 2^-3 (below, lo is an fp16 subnormal: an absolute step of 2^-25).  In that mode every
+ *     convolution evaluates x_hi.w_hi + x_lo.w_hi + x_hi.w_lo on the tensor cores (3x the MMAs) and matches the reference's
+ *     fp32 convolutions (tools/layer_util.py:171,212,253) to ~1e-6 relative; packed filters, 16-bit activations, residuals
+ *     and outputs are all such pairs (buffers twice the size).  The networks' packed filters carry a per-layer power-of-two
+ *     exponent (2^s w, rn_conv_desc::w_unscale), so any filter scale packs to the same bits; activations are not rescaled and hold
+ *     the bars for x ~ N(0,1) 2^k from k = -9 (F(4x4): k = -5) up to the range limits (DESIGN.md §4).
  *     Accumulation is always fp32.
  *   - Return value: 0 = ok; <0 = invalid argument (see source for the code); >0 = CUDA / driver error.
  */
@@ -153,9 +156,15 @@ typedef struct rn_conv_desc {
   /* > 0 (ntaps == 1 only): image b reads filter tap b / b_tap_div of w_packed, which then holds B / b_tap_div taps -- the
    * 16 per-position GEMMs of a Winograd convolution as one launch.  0 = off. */
   int b_tap_div;
+  /* RN_FMT_F16X2 only: DEVICE pointer to one fp32 2^-s, where w_packed holds 2^s w (the filter exponent, DESIGN.md §4: s puts
+   * max |2^s w| in (2^11, 2^12], so that the LO halves of small filters stay fp16 normals).  The epilogue multiplies the
+   * accumulator by it before the bias, which is exact in fp32.  NULL = s = 0, today's bits.  Read on the device, so a re-pack
+   * chooses s without a host synchronisation. */
+  const float* w_unscale;
 } rn_conv_desc;
 /* Besides the argument codes of the source, -25 = no kernel variant is built for the plan (N tile, cluster, M sub-tiles,
- * exact mode, banded half blocks, raw output) that the descriptor leads to; rn_conv_plan reports it as well. */
+ * exact mode, banded half blocks, raw output) that the descriptor leads to; rn_conv_plan reports it as well.  -26 = a
+ * w_unscale with fmt != RN_FMT_F16X2 or with a raw (bias NULL) plan. */
 int rn_conv_igemm(const rn_conv_desc* d, void* stream);
 /* Per-call overrides of the launch heuristics for the reference-shaped wrappers below (their last argument before
  * `stream`; NULL = library defaults).  0 = default for every field; cluster 1/2/4; cta_group 1; kps = k-groups per
@@ -183,6 +192,16 @@ int rn_conv2d_same(const void* x, const void* w_packed, const float* bias, const
 int rn_conv3d_same(const void* x, const void* w_packed, const float* bias, const float* alpha, int act,
                    const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W,
                    int D, int Cin, int Cout, int cout_pad, int k, int fmt, const rn_tuning* tune, void* stream);
+/* Every exact-mode wrapper has a companion rn_*_scaled that takes one more argument right after the packed filter:
+ * w_unscale, a DEVICE pointer to the fp32 2^-s of a filter packed as 2^s w (rn_conv_desc::w_unscale; NULL or fmt != 2 with
+ * NULL = the plain entry point, bit for bit; non-NULL with fmt != RN_FMT_F16X2 = -26).  The pack functions take the filter as
+ * given, so the caller scales it by 2^s first (ops.exact_filter). */
+int rn_conv2d_same_scaled(const void* x, const void* w_packed, const float* w_unscale, const float* bias, const float* alpha,
+                          int act, const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W,
+                          int Cin, int Cout, int cout_pad, int kh, int kw, int fmt, const rn_tuning* tune, void* stream);
+int rn_conv3d_same_scaled(const void* x, const void* w_packed, const float* w_unscale, const float* bias, const float* alpha,
+                          int act, const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W,
+                          int D, int Cin, int Cout, int cout_pad, int k, int fmt, const rn_tuning* tune, void* stream);
 /* layer_util.conv3d 3^3 SAME stride 1 (res_block_3d, tools/layer_util.py:60-88; RenderNet_Shader.py:45-64) as a
  * depth-folded 2-D convolution: the D axis is part of the GEMM's N (128 = (128/Cout) output depths x Cout) and K
  * ((128/Cout + 2) input depths x Cin, padded to 64-element blocks), so TMA moves full 128-byte rows and each
@@ -198,6 +217,10 @@ int rn_expand_channels(const float* v, float* v_full, int C, int D, void* stream
 int rn_conv3d_banded_same(const void* x, const void* w_banded, const float* bias_full, const float* alpha_full,
                           int act, const void* residual, int residual_is_f32, void* out16, float* out32, int B,
                           int H, int W, int D, int Cin, int Cout, int sz, int fmt, const rn_tuning* tune, void* stream);
+int rn_conv3d_banded_same_scaled(const void* x, const void* w_banded, const float* w_unscale, const float* bias_full,
+                                 const float* alpha_full, int act, const void* residual, int residual_is_f32, void* out16,
+                                 float* out32, int B, int H, int W, int D, int Cin, int Cout, int sz, int fmt,
+                                 const rn_tuning* tune, void* stream);
 
 /* The same 3^3 SAME stride-1 conv3d for Cin = Cout = 32 (res1, res_block_3d at RenderNet_Shader.py:45-64; tools/layer_util.py:60-88)
  * as a depth-sliced kernel (rn_conv3d_sliced.cu): tiles of 8 x 8 pixels x 8 output depths, each input depth issued as
@@ -211,6 +234,9 @@ int rn_pack_conv3d_sliced(const float* w, void* packed, int fmt, void* stream);
 int rn_conv3d_sliced_same(const void* x, const void* w_sliced, const float* bias_full, const float* alpha_full, int act,
                           const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W, int D,
                           int Cin, int Cout, int fmt, void* stream);
+int rn_conv3d_sliced_same_scaled(const void* x, const void* w_sliced, const float* w_unscale, const float* bias_full,
+                                 const float* alpha_full, int act, const void* residual, int residual_is_f32, void* out16,
+                                 float* out32, int B, int H, int W, int D, int Cin, int Cout, int fmt, void* stream);
 int rn_conv3d_sliced_plan(int B, int H, int W, int D, int fmt, int* out, int n_out);
 
 /* 3x3 SAME stride-1 conv2d, C -> C channels, RN_FMT_F16X2 only, as Winograd F(2x2, 3x3) (rn_winograd.cu): 16 products per
@@ -235,6 +261,13 @@ int rn_winograd_out(const float* m, const float* bias, const float* alpha, int a
 int rn_conv2d_winograd(const void* x, const void* u, const float* bias, const float* alpha, int act, const void* residual,
                        int residual_is_f32, void* out16, float* out32, int B, int H, int W, int C, void* workspace,
                        long long workspace_bytes, const rn_tuning* tune, void* stream);
+/* F(2x2) of a filter packed with an exponent: u = G (2^s g) G^T, and the epilogue multiplies A^T M A by w_unscale = 2^-s. */
+int rn_winograd_out_scaled(const float* m, const float* w_unscale, const float* bias, const float* alpha, int act,
+                           const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W, int C,
+                           void* stream);
+int rn_conv2d_winograd_scaled(const void* x, const void* u, const float* w_unscale, const float* bias, const float* alpha,
+                              int act, const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H,
+                              int W, int C, void* workspace, long long workspace_bytes, const rn_tuning* tune, void* stream);
 
 /* The same convolution as Winograd F(4x4, 3x3): 36 products per 4x4 output block (2.25 per pixel instead of 4), V and M
  * 2.25x the activation instead of 4x.  Interpolation points 0, +-1, +-1/2, infinity; powers of two keep V and U in range
@@ -264,6 +297,10 @@ int rn_pack_conv2d_transpose_weights(const float* w, void* packed, int kh, int k
 int rn_conv2d_transpose_same(const void* x, const void* w_packed, const float* bias, const float* alpha, int act,
                              void* out16, float* out32, int B, int H, int W, int Cin, int Cout, int cout_pad,
                              int kh, int kw, int stride, int fmt, const rn_tuning* tune, void* stream);
+int rn_conv2d_transpose_same_scaled(const void* x, const void* w_packed, const float* w_unscale, const float* bias,
+                                    const float* alpha, int act, void* out16, float* out32, int B, int H, int W, int Cin,
+                                    int Cout, int cout_pad, int kh, int kw, int stride, int fmt, const rn_tuning* tune,
+                                    void* stream);
 
 /* Stride-2, k = 4 SAME transposed conv (e_conv7/8/9, RenderNet_Shader.py:106-119) as ONE launch: rows = input pixels,
  * N = (ay, ax, co) = 4*Cout, 9 taps (dy,dx in {-1,0,1}) with the unused phase/tap combinations zero in the packed
@@ -273,6 +310,9 @@ int rn_pack_conv2d_transpose_s2_merged(const float* w, void* packed, int Cin, in
 int rn_conv2d_transpose_s2_merged(const void* x, const void* w_merged, const float* bias4, const float* alpha4, int act,
                                   void* out16, float* out32, int B, int H, int W, int Cin, int Cout, int fmt,
                                   const rn_tuning* tune, void* stream);
+int rn_conv2d_transpose_s2_merged_scaled(const void* x, const void* w_merged, const float* w_unscale, const float* bias4,
+                                         const float* alpha4, int act, void* out16, float* out32, int B, int H, int W,
+                                         int Cin, int Cout, int fmt, const rn_tuning* tune, void* stream);
 
 /* Thin-channel stride-1 transposed conv (e_conv10 32->16, e_conv11 16->3 at 512^2; RenderNet_Shader.py:122-129) with
  * F = 64/Cin adjacent x-pixels folded into the channel axis: rows of the implicit GEMM are pixel groups, K = F*Cin
@@ -284,6 +324,10 @@ int rn_pack_conv2d_transpose_xfold(const float* w, void* packed, int kh, int kw,
 int rn_conv2d_transpose_s1_xfold(const void* x, const void* w_xfold, const float* bias_x, const float* alpha_x, int act,
                                  void* out16, float* out32, int B, int H, int W, int Cin, int Cout, int kh, int kw, int F,
                                  int cout_pad, int fmt, const rn_phong* phong, const rn_tuning* tune, void* stream);
+int rn_conv2d_transpose_s1_xfold_scaled(const void* x, const void* w_xfold, const float* w_unscale, const float* bias_x,
+                                        const float* alpha_x, int act, void* out16, float* out32, int B, int H, int W,
+                                        int Cin, int Cout, int kh, int kw, int F, int cout_pad, int fmt,
+                                        const rn_phong* phong, const rn_tuning* tune, void* stream);
 
 /* ---- thin 3-D convolutions on CUDA cores (too few channels for the tensor pipe) ---------------------
  * tf.nn.conv3d SAME + bias + PReLU (layer_util.py:228-265, RenderNet_Shader.py:36-43): e_conv1 (Cin=1,

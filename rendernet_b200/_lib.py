@@ -29,7 +29,7 @@ class rn_conv_desc(C.Structure):
         ("o_nsplit", C.c_int), ("o_nhi", C.c_longlong),
         ("x_plane", C.c_longlong), ("w_plane", C.c_longlong), ("o_plane", C.c_longlong),
         ("epi_groups", C.c_int), ("res_prefetch", C.c_int), ("tma_store", C.c_int),
-        ("phong", C.c_void_p), ("b_tap_div", C.c_int),
+        ("phong", C.c_void_p), ("b_tap_div", C.c_int), ("w_unscale", C.c_void_p),
     ]
 
 
@@ -145,6 +145,12 @@ SIGNATURES = {
     "rn_image_loss_grad_items_fixed_workspace": (_ll, [_ll, _i, _i]),
     "rn_image_loss_grad_items_fixed": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _i, _vp, _ll, _vp]),
 }
+# the exact-mode companions rn_*_scaled: the same arguments plus w_unscale (a device pointer) after the packed filter
+for _name, _at in (("rn_conv2d_same", 2), ("rn_conv3d_same", 2), ("rn_conv3d_banded_same", 2), ("rn_conv3d_sliced_same", 2),
+                   ("rn_winograd_out", 1), ("rn_conv2d_winograd", 2), ("rn_conv2d_transpose_same", 2),
+                   ("rn_conv2d_transpose_s2_merged", 2), ("rn_conv2d_transpose_s1_xfold", 2)):
+    _res, _args = SIGNATURES[_name]
+    SIGNATURES[_name + "_scaled"] = (_res, _args[:_at] + [_vp] + _args[_at:])
 RN_PHONG_NUMPY, RN_PHONG_TF = 0, 1
 
 

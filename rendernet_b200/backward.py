@@ -196,12 +196,12 @@ class _InputGradients:
         if kind == "conv2d":                       # [kh,kw,Ci,Co] -> mirrored, channel roles swapped: [kh,kw,Co,Ci]
             k = int(w.shape[0])
             wd = torch.flip(wt, dims=(0, 1)).permute(0, 1, 3, 2).contiguous()
-            L = ops.pack_conv("conv2d", wd, None, None, device=dev, fmt=fmt, winograd=False)
+            L = ops.pack_conv("conv2d", wd, None, None, device=dev, fmt=fmt, winograd=False, exponent=True)
             pb = (k - 1) // 2
             L.taps = [(kx - (k - 1 - pb), ky - (k - 1 - pb)) for ky in range(k) for kx in range(k)]   # offset of mirrored tap
         elif kind == "conv3d":                     # 3^3, stride 1: depth-folded gradient conv
             wd = torch.flip(wt, dims=(0, 1, 2)).permute(0, 1, 2, 4, 3).contiguous()
-            L = ops.BandedConv3d(wd, None, device=dev, sz=1, fmt=fmt)
+            L = ops.BandedConv3d(wd, None, device=dev, sz=1, fmt=fmt, exponent=True)
         elif kind == "conv2d_transpose" and stride == 1:
             # y[o] = sum_k x[o - k + pb] w[k][co][ci]  =>  dx[i] = sum_k g[i + k - pb] w[k][co][ci]: a forward SAME conv whose TF filter
             # [kh,kw,Cin'=Co,Cout'=Ci] IS the transposed-conv filter array; Co is zero padded to a multiple of 16 (e_conv11: 3)
@@ -209,7 +209,7 @@ class _InputGradients:
             cp = ops.round_up(co, 16)
             wd = torch.zeros((w.shape[0], w.shape[1], cp, w.shape[3]), device=dev, dtype=torch.float32)
             wd[:, :, :co] = wt
-            L = ops.pack_conv("conv2d", wd, None, None, device=dev, fmt=fmt, winograd=False)
+            L = ops.pack_conv("conv2d", wd, None, None, device=dev, fmt=fmt, winograd=False, exponent=True)
             L.taps = None
         elif kind == "conv2d_transpose" and stride == 2:
             # o = 2i + k - 1.  With g2[i,j,(ay,ax,co)] = g[2i+ay, 2j+ax, co]:  dx[i] = sum_{dy,dx in -1..1} g2[i+dy, j+dx] . Wd[dy+1][dx+1]
@@ -227,7 +227,7 @@ class _InputGradients:
                             kx = 2 * dx + ax + 1
                             if 0 <= kx < 4:
                                 wd[dy + 1, dx + 1, ay, ax] = wt[ky, kx]
-            L = ops.pack_conv("conv2d", wd.reshape(3, 3, 4 * co, ci), None, None, device=dev, fmt=fmt, winograd=False)
+            L = ops.pack_conv("conv2d", wd.reshape(3, 3, 4 * co, ci), None, None, device=dev, fmt=fmt, winograd=False, exponent=True)
             L.taps = None
         else:
             raise NotImplementedError(f"no data-gradient path for {kind} stride {stride}")
@@ -477,7 +477,7 @@ class _InputGradients:
             if k % 2 == 1:
                 return ops.conv2d(g, L, residual=acc)
             return ops.conv2d_taps(g, L.w, L.bias, L.taps, L.cout, L.cout_pad, self.store.fmt, residual=acc,
-                                   ny=k if L.cin % 64 == 0 else 0)
+                                   ny=k if L.cin % 64 == 0 else 0, w_unscale=L.w_unscale)
         if stride == 1:                                # transposed conv, stride 1
             return ops.conv2d(g, L, residual=acc)
         return ops.conv2d(self._space_to_depth(g), L, residual=acc)      # transposed conv, stride 2

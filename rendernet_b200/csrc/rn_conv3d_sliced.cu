@@ -228,6 +228,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv3d_sliced_kernel(const __g
       const int x = x0 + (er & 7), y = y0 + (er >> 3);
       const bool row_valid = x < p.W && y < p.H;
       const long long off = p.o_base + b * p.o_b + y * p.o_y + x * p.o_x;
+      const float wsc = SPLIT ? w_unscale_of(p) : 1.f;
 #pragma unroll
       for (int c0 = 0; c0 < kSlDepths * kSlCh; c0 += kStgCols) {
         named_bar_sync(bar_id, 128);                          // the previous pass has read the staging panel
@@ -246,7 +247,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) conv3d_sliced_kernel(const __g
             const float4 q = sp[i];
             a[4 * i] = q.x; a[4 * i + 1] = q.y; a[4 * i + 2] = q.z; a[4 * i + 3] = q.w;
           }
-          epilogue_chunk<16, SPLIT>(p, a, z0 * kSlCh + c0 + ec, off, true, b);
+          epilogue_chunk<16, SPLIT>(p, a, z0 * kSlCh + c0 + ec, off, true, b, wsc);
         }
       }
     }
@@ -296,11 +297,13 @@ extern "C" int rn_conv3d_sliced_plan(int B, int H, int W, int D, int fmt, int* o
   return 0;
 }
 
-extern "C" int rn_conv3d_sliced_same(const void* x, const void* w_sliced, const float* bias_full, const float* alpha_full,
-                                     int act, const void* residual, int residual_is_f32, void* out16, float* out32, int B,
-                                     int H, int W, int D, int Cin, int Cout, int fmt, void* stream) {
+extern "C" int rn_conv3d_sliced_same_scaled(const void* x, const void* w_sliced, const float* w_unscale,
+                                            const float* bias_full, const float* alpha_full, int act, const void* residual,
+                                            int residual_is_f32, void* out16, float* out32, int B, int H, int W, int D,
+                                            int Cin, int Cout, int fmt, void* stream) {
   using namespace rn;
   if (x == nullptr || w_sliced == nullptr || bias_full == nullptr) return -1;
+  if (w_unscale != nullptr && fmt != 2) return -26;
   if (Cin != kSlCh || Cout != kSlCh) return -4;
   if (act != ACT_NONE && act != ACT_PRELU) return -5;
   if (act == ACT_PRELU && alpha_full == nullptr) return -5;
@@ -347,6 +350,7 @@ extern "C" int rn_conv3d_sliced_same(const void* x, const void* w_sliced, const 
   p.out16 = out16; p.out32 = out32; p.res = residual; p.res_is_f32 = residual_is_f32;
   p.bias = bias_full; p.alpha = alpha_full; p.act = act; p.n_valid = static_cast<int>(F);
   p.o_base = 0; p.o_x = F; p.o_y = static_cast<long long>(W) * F; p.o_b = static_cast<long long>(H) * W * F;
+  p.w_unscale = w_unscale;
   auto al16 = [](const void* q) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   p.vec_ok = al16(out16) && al16(out32) && al16(residual) ? 1 : 0;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -354,4 +358,11 @@ extern "C" int rn_conv3d_sliced_same(const void* x, const void* w_sliced, const 
                         : fmt == 1 ? launch_sliced<false, 1>(p, pl.grid, pl.smem, st)
                                    : launch_sliced<false, 0>(p, pl.grid, pl.smem, st);
   return e == cudaSuccess ? 0 : static_cast<int>(e);
+}
+
+extern "C" int rn_conv3d_sliced_same(const void* x, const void* w_sliced, const float* bias_full, const float* alpha_full,
+                                     int act, const void* residual, int residual_is_f32, void* out16, float* out32, int B,
+                                     int H, int W, int D, int Cin, int Cout, int fmt, void* stream) {
+  return rn_conv3d_sliced_same_scaled(x, w_sliced, nullptr, bias_full, alpha_full, act, residual, residual_is_f32, out16,
+                                      out32, B, H, W, D, Cin, Cout, fmt, stream);
 }

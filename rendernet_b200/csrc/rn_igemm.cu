@@ -150,10 +150,12 @@ static int plan_conv(const rn_conv_desc* d, IgemmParams& p, ConvPlan& pl) {
   const int D = d->ndim == 3 ? d->D : 1;
   if (d->B < 1 || d->H < 1 || d->W < 1 || D < 1) return -7;
   if (d->b_tap_div < 0 || (d->b_tap_div > 0 && (d->ntaps != 1 || d->w_banded || d->B % d->b_tap_div != 0))) return -23;
+  if (d->w_unscale != nullptr && (d->fmt != 2 || raw)) return -26;   // only the exact-mode epilogue applies it
 
   const Tuning& tn = tuning();
   const bool split = d->fmt == 2;
   memset(&p, 0, sizeof(p));
+  p.w_unscale = d->w_unscale;
   // K block: as many input channels as fit one 128/64/32-byte swizzle row
   p.row_bytes = (d->Cin % 64 == 0) ? 128 : ((d->Cin % 32 == 0) ? 64 : 32);
   const int KB = p.row_bytes / 2;

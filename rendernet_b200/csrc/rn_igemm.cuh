@@ -100,6 +100,8 @@ struct alignas(64) IgemmParams {
   long long o_nhi;                //      phases of a stride-2 transposed conv: n = (ay, ax, co))
   int b_tap_div;                  // > 0 (one-tap convs only): image b of the tile reads filter tap b / b_tap_div -- the 16
                                   // per-position GEMMs of a Winograd conv as one launch over [16*B, H/2, W/2, C]
+  const float* w_unscale;         // split mode: device fp32 2^-s of a filter packed as 2^s w (the epilogue's acc * 2^-s, exact
+                                  // in fp32, comes before the bias), or nullptr (s = 0)
 };
 
 // Band structure of the depth-folded 3^3 conv3d (rn_conv3d_banded_same): N tile = 128/Cout output depths x Cout, K per tap =

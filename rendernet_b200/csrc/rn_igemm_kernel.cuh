@@ -62,20 +62,26 @@ __device__ __forceinline__ TileCoord decode_tile(const IgemmParams& p, int tile,
   return t;
 }
 
+// 2^-s of an exact-mode filter packed as 2^s w (DESIGN.md §4, the filter exponent): read once per tile, not per chunk
+__device__ __forceinline__ float w_unscale_of(const IgemmParams& p) {
+  return p.w_unscale != nullptr ? __ldg(p.w_unscale) : 1.f;
+}
+
 // Epilogue of CW consecutive accumulator columns n0.. of one output row (element offset `off`): bias, activation, residual,
-// 16-bit and/or fp32 stores.
+// 16-bit and/or fp32 stores.  sc = w_unscale_of(p) in split mode: acc * sc is exact, and sc = 1 gives the bits of acc + bias.
 template <int CW, bool SPLIT = false>
 __device__ __forceinline__ void epilogue_chunk(const IgemmParams& p, const float* __restrict__ a, int n0, long long off,
-                                               bool row_valid, int bidx) {
+                                               bool row_valid, int bidx, float sc = 1.f) {
   if (!row_valid) return;
+  if constexpr (!SPLIT) sc = 1.f;
   float v[CW];
 #pragma unroll
   for (int i = 0; i < CW; i += 4) {
     const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + i));
-    v[i + 0] = a[i + 0] + b4.x;
-    v[i + 1] = a[i + 1] + b4.y;
-    v[i + 2] = a[i + 2] + b4.z;
-    v[i + 3] = a[i + 3] + b4.w;
+    v[i + 0] = fmaf(a[i + 0], sc, b4.x);
+    v[i + 1] = fmaf(a[i + 1], sc, b4.y);
+    v[i + 2] = fmaf(a[i + 2], sc, b4.z);
+    v[i + 3] = fmaf(a[i + 3], sc, b4.w);
   }
   if (p.act == ACT_PRELU) {
 #pragma unroll
@@ -477,6 +483,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
       }
       // epilogue: accumulator fragments -> staging panel (SC columns at a time) -> one row per thread -> epilogue_chunk
       const int x = t.x0 + xl, z = t.z0 + zl;
+      const float wsc = SPLIT ? w_unscale_of(p) : 1.f;
 #pragma unroll
       for (int s = 0; s < MS; ++s) {
         const int y = t.y0 + s * p.BH + yl;
@@ -503,7 +510,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) igemm_kernel(const __grid_cons
             }
             const int nc = t.n0 + c0 + ec;
             const long long offc = p.o_nsplit > 0 ? off + (nc / p.o_nsplit) * p.o_nhi + (nc % p.o_nsplit) - nc : off;
-            epilogue_chunk<16, SPLIT>(p, a, nc, offc, true, t.b);
+            epilogue_chunk<16, SPLIT>(p, a, nc, offc, true, t.b, wsc);
           }
         }
       }

@@ -1169,10 +1169,10 @@ static void apply_tuning(rn_conv_desc& d, const rn_tuning* t) {
 }
 static bool want_yhalo(const rn_tuning* t) { return (t != nullptr && t->yhalo != 0) ? t->yhalo > 0 : tuning().yhalo != 0; }
 
-extern "C" int rn_conv2d_same(const void* x, const void* w_packed, const float* bias, const float* alpha, int act,
-                              const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H,
-                              int W, int Cin, int Cout, int cout_pad, int kh, int kw, int fmt, const rn_tuning* tune,
-                              void* stream) {
+extern "C" int rn_conv2d_same_scaled(const void* x, const void* w_packed, const float* w_unscale, const float* bias,
+                                     const float* alpha, int act, const void* residual, int residual_is_f32, void* out16,
+                                     float* out32, int B, int H, int W, int Cin, int Cout, int cout_pad, int kh, int kw,
+                                     int fmt, const rn_tuning* tune, void* stream) {
   if (kh * kw > kMaxTaps || kh < 1 || kw < 1) return -20;
   int8_t taps[kMaxTaps * 3];
   const int pby = (kh - 1) / 2, pbx = (kw - 1) / 2;  // SAME, stride 1: before = (k-1)//2
@@ -1193,15 +1193,24 @@ extern "C" int rn_conv2d_same(const void* x, const void* w_packed, const float* 
     d.w_plane = static_cast<long long>(kh) * kw * cout_pad * Cin;
     d.o_plane = static_cast<long long>(B) * H * W * Cout;
   }
+  d.w_unscale = w_unscale;
   apply_tuning(d, tune);
   if (kh == 3 && Cin % 64 == 0 && want_yhalo(tune)) d.ny = 3;   // taps are already ordered ky*kw + kx with dy = ky - 1
   return rn_conv_igemm(&d, stream);
 }
 
-extern "C" int rn_conv3d_same(const void* x, const void* w_packed, const float* bias, const float* alpha, int act,
+extern "C" int rn_conv2d_same(const void* x, const void* w_packed, const float* bias, const float* alpha, int act,
                               const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H,
-                              int W, int D, int Cin, int Cout, int cout_pad, int k, int fmt, const rn_tuning* tune,
+                              int W, int Cin, int Cout, int cout_pad, int kh, int kw, int fmt, const rn_tuning* tune,
                               void* stream) {
+  return rn_conv2d_same_scaled(x, w_packed, nullptr, bias, alpha, act, residual, residual_is_f32, out16, out32, B, H, W, Cin,
+                               Cout, cout_pad, kh, kw, fmt, tune, stream);
+}
+
+extern "C" int rn_conv3d_same_scaled(const void* x, const void* w_packed, const float* w_unscale, const float* bias,
+                                     const float* alpha, int act, const void* residual, int residual_is_f32, void* out16,
+                                     float* out32, int B, int H, int W, int D, int Cin, int Cout, int cout_pad, int k,
+                                     int fmt, const rn_tuning* tune, void* stream) {
   if (k * k * k > kMaxTaps || k < 1) return -20;
   int8_t taps[kMaxTaps * 3];
   const int pb = (k - 1) / 2;
@@ -1223,8 +1232,17 @@ extern "C" int rn_conv3d_same(const void* x, const void* w_packed, const float* 
     d.w_plane = static_cast<long long>(k) * k * k * cout_pad * Cin;
     d.o_plane = static_cast<long long>(B) * H * W * D * Cout;
   }
+  d.w_unscale = w_unscale;
   apply_tuning(d, tune);
   return rn_conv_igemm(&d, stream);
+}
+
+extern "C" int rn_conv3d_same(const void* x, const void* w_packed, const float* bias, const float* alpha, int act,
+                              const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H,
+                              int W, int D, int Cin, int Cout, int cout_pad, int k, int fmt, const rn_tuning* tune,
+                              void* stream) {
+  return rn_conv3d_same_scaled(x, w_packed, nullptr, bias, alpha, act, residual, residual_is_f32, out16, out32, B, H, W, D,
+                               Cin, Cout, cout_pad, k, fmt, tune, stream);
 }
 
 // Transposed SAME conv: o = i*s + kk - pb, pb = max(k-s,0)/2.  Output phase a (o = j*s + a) receives the
@@ -1269,10 +1287,10 @@ extern "C" int rn_pack_conv2d_transpose_weights(const float* w, void* packed, in
   return 0;
 }
 
-extern "C" int rn_conv2d_transpose_same(const void* x, const void* w_packed, const float* bias, const float* alpha,
-                                        int act, void* out16, float* out32, int B, int H, int W, int Cin, int Cout,
-                                        int cout_pad, int kh, int kw, int stride, int fmt, const rn_tuning* tune,
-                                        void* stream) {
+extern "C" int rn_conv2d_transpose_same_scaled(const void* x, const void* w_packed, const float* w_unscale,
+                                               const float* bias, const float* alpha, int act, void* out16, float* out32,
+                                               int B, int H, int W, int Cin, int Cout, int cout_pad, int kh, int kw,
+                                               int stride, int fmt, const rn_tuning* tune, void* stream) {
   if (kh * kw > kMaxTaps || stride < 1) return -20;
   const int Ho = H * stride, Wo = W * stride;
   size_t off = 0;
@@ -1297,12 +1315,21 @@ extern "C" int rn_conv2d_transpose_same(const void* x, const void* w_packed, con
         d.w_plane = static_cast<long long>(kh) * kw * cout_pad * Cin;   // LO plane follows ALL phases of the HI plane
         d.o_plane = static_cast<long long>(B) * Ho * Wo * Cout;
       }
+      d.w_unscale = w_unscale;
       apply_tuning(d, tune);
       int r = rn_conv_igemm(&d, stream);
       if (r != 0) return r;
       off += static_cast<size_t>(pt.n) * cout_pad * Cin;
     }
   return 0;
+}
+
+extern "C" int rn_conv2d_transpose_same(const void* x, const void* w_packed, const float* bias, const float* alpha,
+                                        int act, void* out16, float* out32, int B, int H, int W, int Cin, int Cout,
+                                        int cout_pad, int kh, int kw, int stride, int fmt, const rn_tuning* tune,
+                                        void* stream) {
+  return rn_conv2d_transpose_same_scaled(x, w_packed, nullptr, bias, alpha, act, out16, out32, B, H, W, Cin, Cout, cout_pad,
+                                         kh, kw, stride, fmt, tune, stream);
 }
 
 
@@ -1344,10 +1371,10 @@ extern "C" int rn_expand_channels(const float* v, float* v_full, int C, int D, v
   return static_cast<int>(cudaGetLastError());
 }
 
-extern "C" int rn_conv3d_banded_same(const void* x, const void* w_banded, const float* bias_full,
-                                     const float* alpha_full, int act, const void* residual, int residual_is_f32,
-                                     void* out16, float* out32, int B, int H, int W, int D, int Cin, int Cout,
-                                     int sz, int fmt, const rn_tuning* tune, void* stream) {
+extern "C" int rn_conv3d_banded_same_scaled(const void* x, const void* w_banded, const float* w_unscale,
+                                            const float* bias_full, const float* alpha_full, int act, const void* residual,
+                                            int residual_is_f32, void* out16, float* out32, int B, int H, int W, int D,
+                                            int Cin, int Cout, int sz, int fmt, const rn_tuning* tune, void* stream) {
   if (rn_conv3d_banded_bytes(Cin, Cout, sz) < 0) return -30;
   int Do, pz;
   same_pad(D, 3, sz, &Do, &pz);                     // TF SAME along z: out = ceil(D/sz), pad-before pz
@@ -1378,9 +1405,18 @@ extern "C" int rn_conv3d_banded_same(const void* x, const void* w_banded, const 
     d.w_plane = rn_conv3d_banded_bytes(Cin, Cout, sz) / 2;
     d.o_plane = static_cast<long long>(B) * H * W * Fo;
   }
+  d.w_unscale = w_unscale;
   apply_tuning(d, tune);
   if (want_yhalo(tune)) d.ny = 3;
   return rn_conv_igemm(&d, stream);
+}
+
+extern "C" int rn_conv3d_banded_same(const void* x, const void* w_banded, const float* bias_full,
+                                     const float* alpha_full, int act, const void* residual, int residual_is_f32,
+                                     void* out16, float* out32, int B, int H, int W, int D, int Cin, int Cout,
+                                     int sz, int fmt, const rn_tuning* tune, void* stream) {
+  return rn_conv3d_banded_same_scaled(x, w_banded, nullptr, bias_full, alpha_full, act, residual, residual_is_f32, out16,
+                                      out32, B, H, W, D, Cin, Cout, sz, fmt, tune, stream);
 }
 
 
@@ -1482,10 +1518,11 @@ extern "C" int rn_pack_conv2d_transpose_xfold(const float* w, void* packed, int 
 
 // x [B,H,W,Cin] 16-bit; w_xfold from rn_pack_conv2d_transpose_xfold ([kh*3][cout_pad][F*Cin]); bias_x / alpha_x are the
 // per-Cout vectors tiled F times and zero padded to cout_pad (rn_expand_channels + padding by the caller).
-extern "C" int rn_conv2d_transpose_s1_xfold(const void* x, const void* w_xfold, const float* bias_x, const float* alpha_x,
-                                            int act, void* out16, float* out32, int B, int H, int W, int Cin, int Cout,
-                                            int kh, int kw, int F, int cout_pad, int fmt, const rn_phong* phong,
-                                            const rn_tuning* tune, void* stream) {
+extern "C" int rn_conv2d_transpose_s1_xfold_scaled(const void* x, const void* w_xfold, const float* w_unscale,
+                                                   const float* bias_x, const float* alpha_x, int act, void* out16,
+                                                   float* out32, int B, int H, int W, int Cin, int Cout, int kh, int kw, int F,
+                                                   int cout_pad, int fmt, const rn_phong* phong, const rn_tuning* tune,
+                                                   void* stream) {
   if (F < 2 || W % F != 0 || kh * 3 > kMaxTaps) return -20;
   int8_t taps[kMaxTaps * 3];
   const int pby = (kh - 1) / 2;                     // SAME stride-1 transposed: dy = pb - ky
@@ -1508,9 +1545,18 @@ extern "C" int rn_conv2d_transpose_s1_xfold(const void* x, const void* w_xfold, 
   }
   if (phong != nullptr && (Cout != 3 || act != RN_ACT_SIGMOID || cout_pad != 16)) return -22;
   d.phong = phong;
+  d.w_unscale = w_unscale;
   apply_tuning(d, tune);
   if (want_yhalo(tune) && (F * Cin) % 64 == 0) d.ny = kh;    // tap = kyr*3 + j, dy consecutive in kyr: the kh taps share one halo load
   return rn_conv_igemm(&d, stream);
+}
+
+extern "C" int rn_conv2d_transpose_s1_xfold(const void* x, const void* w_xfold, const float* bias_x, const float* alpha_x,
+                                            int act, void* out16, float* out32, int B, int H, int W, int Cin, int Cout,
+                                            int kh, int kw, int F, int cout_pad, int fmt, const rn_phong* phong,
+                                            const rn_tuning* tune, void* stream) {
+  return rn_conv2d_transpose_s1_xfold_scaled(x, w_xfold, nullptr, bias_x, alpha_x, act, out16, out32, B, H, W, Cin, Cout, kh,
+                                             kw, F, cout_pad, fmt, phong, tune, stream);
 }
 
 
@@ -1524,9 +1570,10 @@ extern "C" int rn_pack_conv2d_transpose_s2_merged(const float* w, void* packed, 
   return static_cast<int>(cudaGetLastError());
 }
 
-extern "C" int rn_conv2d_transpose_s2_merged(const void* x, const void* w_merged, const float* bias4,
-                                             const float* alpha4, int act, void* out16, float* out32, int B, int H,
-                                             int W, int Cin, int Cout, int fmt, const rn_tuning* tune, void* stream) {
+extern "C" int rn_conv2d_transpose_s2_merged_scaled(const void* x, const void* w_merged, const float* w_unscale,
+                                                    const float* bias4, const float* alpha4, int act, void* out16,
+                                                    float* out32, int B, int H, int W, int Cin, int Cout, int fmt,
+                                                    const rn_tuning* tune, void* stream) {
   if (Cout % 16 != 0) return -20;
   int8_t taps[27];
   for (int ky = 0; ky < 3; ++ky)
@@ -1548,9 +1595,17 @@ extern "C" int rn_conv2d_transpose_s2_merged(const void* x, const void* w_merged
     d.w_plane = 9LL * 4 * Cout * Cin;
     d.o_plane = static_cast<long long>(B) * Ho * Wo * Cout;
   }
+  d.w_unscale = w_unscale;
   apply_tuning(d, tune);
   if (Cin % 64 == 0 && want_yhalo(tune)) d.ny = 3;
   return rn_conv_igemm(&d, stream);
+}
+
+extern "C" int rn_conv2d_transpose_s2_merged(const void* x, const void* w_merged, const float* bias4,
+                                             const float* alpha4, int act, void* out16, float* out32, int B, int H,
+                                             int W, int Cin, int Cout, int fmt, const rn_tuning* tune, void* stream) {
+  return rn_conv2d_transpose_s2_merged_scaled(x, w_merged, nullptr, bias4, alpha4, act, out16, out32, B, H, W, Cin, Cout, fmt,
+                                              tune, stream);
 }
 
 // ---------------------------------------------------------------------------------- thin conv3d

@@ -160,7 +160,7 @@ __global__ void __launch_bounds__(128) winograd_out_kernel(const __grid_constant
         for (int k = 0; k < 8; ++k)
           acc[k] = e == 0 ? s[a][0][k] + s[a][1][k] + s[a][2][k] : s[a][1][k] - s[a][2][k] - s[a][3][k];
         const long long off = ((static_cast<long long>(b) * H + y) * W + 2 * tx + e) * C;
-        epilogue_chunk<8, true>(p, acc, cg * 8, off, true, b);
+        epilogue_chunk<8, true>(p, acc, cg * 8, off, true, b, w_unscale_of(p));
       }
     }
   }
@@ -324,7 +324,7 @@ __global__ void __launch_bounds__(128) winograd4_out_kernel(const __grid_constan
 #pragma unroll
         for (int k = 0; k < 8; ++k) acc[k] = s[a][e][k] * y_scale;
         const long long off = ((static_cast<long long>(b) * H + y) * W + 4 * tx + e) * C;
-        epilogue_chunk<8, true>(p, acc, cg * 8, off, true, b);
+        epilogue_chunk<8, true>(p, acc, cg * 8, off, true, b);   // U carries its own exponent (u_exp), never w_unscale
       }
     }
   }
@@ -395,8 +395,9 @@ extern "C" int rn_winograd_gemm(const void* v, const void* u, float* m, int B, i
   return rn_conv_igemm(&d, stream);
 }
 
-extern "C" int rn_winograd_out(const float* m, const float* bias, const float* alpha, int act, const void* residual,
-                               int residual_is_f32, void* out16, float* out32, int B, int H, int W, int C, void* stream) {
+extern "C" int rn_winograd_out_scaled(const float* m, const float* w_unscale, const float* bias, const float* alpha, int act,
+                                      const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H,
+                                      int W, int C, void* stream) {
   if (m == nullptr || bias == nullptr || (out16 == nullptr && out32 == nullptr) || !wino_shape_ok(B, H, W, C)) return -1;
   if (act != ACT_NONE && act != ACT_PRELU && act != ACT_SIGMOID) return -1;
   if (act == ACT_PRELU && alpha == nullptr) return -5;
@@ -405,15 +406,22 @@ extern "C" int rn_winograd_out(const float* m, const float* bias, const float* a
   p.out16 = out16; p.out32 = out32; p.res = residual; p.res_is_f32 = residual_is_f32;
   p.bias = bias; p.alpha = alpha; p.act = act; p.n_valid = C; p.vec_ok = 1; p.ab_fmt = 0; p.split = 1;
   p.o_plane = static_cast<long long>(B) * H * W * C;
+  p.w_unscale = w_unscale;
   const long long n = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 8);
   winograd_out_kernel<<<wino_grid(n), 128, 0, static_cast<cudaStream_t>(stream)>>>(p, m, B, H, W, C);
   g_launch_count.fetch_add(1, std::memory_order_relaxed);
   return static_cast<int>(cudaGetLastError());
 }
 
-extern "C" int rn_conv2d_winograd(const void* x, const void* u, const float* bias, const float* alpha, int act,
-                                  const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W,
-                                  int C, void* workspace, long long workspace_bytes, const rn_tuning* tune, void* stream) {
+extern "C" int rn_winograd_out(const float* m, const float* bias, const float* alpha, int act, const void* residual,
+                               int residual_is_f32, void* out16, float* out32, int B, int H, int W, int C, void* stream) {
+  return rn_winograd_out_scaled(m, nullptr, bias, alpha, act, residual, residual_is_f32, out16, out32, B, H, W, C, stream);
+}
+
+extern "C" int rn_conv2d_winograd_scaled(const void* x, const void* u, const float* w_unscale, const float* bias,
+                                         const float* alpha, int act, const void* residual, int residual_is_f32, void* out16,
+                                         float* out32, int B, int H, int W, int C, void* workspace, long long workspace_bytes,
+                                         const rn_tuning* tune, void* stream) {
   const long long need = rn_winograd_workspace_bytes(B, H, W, C);
   if (need < 0 || workspace == nullptr || workspace_bytes < need) return -1;
   auto al16 = [](const void* q) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
@@ -422,8 +430,16 @@ extern "C" int rn_conv2d_winograd(const void* x, const void* u, const float* bia
   float* m = reinterpret_cast<float*>(v + 2 * 16LL * B * (H / 2) * (W / 2) * C);
   int rc = rn_winograd_in(x, v, B, H, W, C, stream);
   if (rc == 0) rc = rn_winograd_gemm(v, u, m, B, H, W, C, tune, stream);
-  if (rc == 0) rc = rn_winograd_out(m, bias, alpha, act, residual, residual_is_f32, out16, out32, B, H, W, C, stream);
+  if (rc == 0)
+    rc = rn_winograd_out_scaled(m, w_unscale, bias, alpha, act, residual, residual_is_f32, out16, out32, B, H, W, C, stream);
   return rc;
+}
+
+extern "C" int rn_conv2d_winograd(const void* x, const void* u, const float* bias, const float* alpha, int act,
+                                  const void* residual, int residual_is_f32, void* out16, float* out32, int B, int H, int W,
+                                  int C, void* workspace, long long workspace_bytes, const rn_tuning* tune, void* stream) {
+  return rn_conv2d_winograd_scaled(x, u, nullptr, bias, alpha, act, residual, residual_is_f32, out16, out32, B, H, W, C,
+                                   workspace, workspace_bytes, tune, stream);
 }
 
 extern "C" int rn_conv2d_winograd_tile(int fmt, int kh, int kw, int H, int W, int Cin, int Cout, int cout_pad,

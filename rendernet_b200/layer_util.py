@@ -38,7 +38,8 @@ def _packed(wvar: torch.Tensor, bvar: Optional[torch.Tensor], kind: str, stride:
     key = (getattr(wvar, "_rn_name", id(wvar)), kind, stride, tf.COMPUTE_DTYPE, st.fmt)
     L = st.packed.get(key)
     if L is None:
-        L = ops.pack_conv(kind, wvar, bvar, None, stride=stride, dtype=tf.COMPUTE_DTYPE, device=st.device, fmt=st.fmt)
+        L = ops.pack_conv(kind, wvar, bvar, None, stride=stride, dtype=tf.COMPUTE_DTYPE, device=st.device, fmt=st.fmt,
+                          exponent=True)
         st.packed[key] = L
     return L
 
@@ -419,14 +420,15 @@ def _deferred_conv(kind, x, w, b, stride):
             if sliced:
                 Ls = _store().packed.get(("sliced", w._rn_name, _store().fmt))
                 if Ls is None:
-                    Ls = ops.SlicedConv3d(w, b, dtype=tf.COMPUTE_DTYPE, device=_store().device, fmt=_store().fmt)
+                    Ls = ops.SlicedConv3d(w, b, dtype=tf.COMPUTE_DTYPE, device=_store().device, fmt=_store().fmt, exponent=True)
                     _store().packed[("sliced", w._rn_name, _store().fmt)] = Ls
                 return ops.conv3d_sliced(xt, Ls, act=act, residual=residual, alpha=a,
                                          alpha_tag=getattr(alpha, "_rn_name", None), want16=want16, want32=want32)
             if banded:
                 Lb = _store().packed.get(("banded", w._rn_name, stride, _store().fmt))
                 if Lb is None:
-                    Lb = ops.BandedConv3d(w, b, dtype=tf.COMPUTE_DTYPE, device=_store().device, sz=stride, fmt=_store().fmt)
+                    Lb = ops.BandedConv3d(w, b, dtype=tf.COMPUTE_DTYPE, device=_store().device, sz=stride, fmt=_store().fmt,
+                                          exponent=True)
                     _store().packed[("banded", w._rn_name, stride, _store().fmt)] = Lb
                 return ops.conv3d_banded(xt, Lb, act=act, residual=residual, alpha=a,
                                          alpha_tag=getattr(alpha, "_rn_name", None), want16=want16, want32=want32)
@@ -434,7 +436,7 @@ def _deferred_conv(kind, x, w, b, stride):
         if merged:
             Lm = _store().packed.get(("merged", w._rn_name, _store().fmt))
             if Lm is None:
-                Lm = ops.MergedConvT2(w, b, dtype=tf.COMPUTE_DTYPE, device=_store().device, fmt=_store().fmt)
+                Lm = ops.MergedConvT2(w, b, dtype=tf.COMPUTE_DTYPE, device=_store().device, fmt=_store().fmt, exponent=True)
                 _store().packed[("merged", w._rn_name, _store().fmt)] = Lm
             al = None
             if act == "prelu":
@@ -445,7 +447,7 @@ def _deferred_conv(kind, x, w, b, stride):
             F = xfold
             Lx = _store().packed.get(("xfold", w._rn_name, F, _store().fmt))
             if Lx is None:
-                Lx = ops.XFoldConvT(w, b, F, dtype=tf.COMPUTE_DTYPE, device=_store().device, fmt=_store().fmt)
+                Lx = ops.XFoldConvT(w, b, F, dtype=tf.COMPUTE_DTYPE, device=_store().device, fmt=_store().fmt, exponent=True)
                 _store().packed[("xfold", w._rn_name, F, _store().fmt)] = Lx
             al = None
             if act == "prelu":

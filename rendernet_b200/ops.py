@@ -231,6 +231,7 @@ class PackedConv:
     master: Optional[torch.Tensor] = None
     master_version: int = 0
     wino: Optional[dict] = None
+    w_unscale: Optional[torch.Tensor] = None   # exact mode: fp32 [1] 2^-s of w = 2^s w_tf (exact_filter), else None
 
 
 def _pad_vec(v: Optional[torch.Tensor], n: int, n_pad: int, device) -> Optional[torch.Tensor]:
@@ -241,11 +242,41 @@ def _pad_vec(v: Optional[torch.Tensor], n: int, n_pad: int, device) -> Optional[
     return out
 
 
+# The filter exponent of the exact mode (fmt 2, DESIGN.md §4): a pack made with exponent=True stores 2^s w, with s chosen from
+# max |w| so that max |2^s w| lies in (2^11, 2^12], and the epilogue multiplies the accumulator by 2^-s before the bias (exact in
+# fp32).  Without it, the LO half of any |w| < 2^-3 is an fp16 subnormal and keeps only an absolute step of 2^-25: a layer whose
+# filter is 2^8 smaller than xavier-sized misses the exact mode's bar.  The networks (layer_util, backward) pack with it; a
+# direct call packs the filter as given unless it asks, so the packed bits and results of every existing caller stay what they
+# were.  False turns it off everywhere (s = 0, the packing before it): for A/B runs and the tests that show the difference.
+FILTER_EXPONENT = True
+
+
+def filter_scales(w: torch.Tensor):
+    """(2^s, 2^-s) as fp32 [1] tensors on w's device, s by wino4_exponent's rule on m = max |w|: max |2^s w| in (2^11, 2^12],
+    clamped to |s| <= 100 (a zero filter gets 100, a non-finite one -100 or 100: its outputs are non-finite either way).
+    2^ceil(log2 m) is m's exponent field rounded up, so this is a handful of elementwise ops on one value, done where w lives:
+    a re-pack after an optimiser step never waits for the host, and adds few launches."""
+    m = torch.linalg.vector_norm(w.detach().reshape(-1), float("inf"), dtype=torch.float32).reshape(1)
+    p = ((m.view(torch.int32) + 0x7FFFFF) & 0x7F800000).view(torch.float32)   # 2^ceil(log2 m) for finite m > 0
+    p = p.clamp(2.0 ** -88, 2.0 ** 112)
+    return 2.0 ** 12 / p, p * 2.0 ** -12                                      # powers of two: exact
+
+
+def exact_filter(w_tf: torch.Tensor, fmt: int, exponent: bool = True):
+    """(the fp32 filter to pack, w_unscale): for fmt 2 with exponent, (2^s w_tf, fp32 [1] tensor 2^-s) (filter_scales) -- both
+    scalings exact, so a filter scaled by a power of two packs to the same bits; else (w_tf, None)."""
+    if fmt != 2 or not exponent or not FILTER_EXPONENT:
+        return w_tf, None
+    up, down = filter_scales(w_tf)
+    return (w_tf * up).contiguous(), down
+
+
 def pack_conv(kind: str, w_tf: torch.Tensor, bias: Optional[torch.Tensor], alpha: Optional[torch.Tensor],
               stride: int = 1, dtype: torch.dtype = torch.float16, device="cuda", fmt: Optional[int] = None,
-              winograd: bool = True) -> PackedConv:
+              winograd: bool = True, exponent: bool = False) -> PackedConv:
     """w_tf in TF filter layout: conv2d [kh,kw,Cin,Cout]; conv3d [k,k,k,Cin,Cout];
-    conv2d_transpose [kh,kw,Cout,Cin].  winograd=False keeps an exact-mode 3x3 C -> C conv on the direct kernel."""
+    conv2d_transpose [kh,kw,Cout,Cin].  winograd=False keeps an exact-mode 3x3 C -> C conv on the direct kernel.
+    exponent=True: an exact-mode filter is packed with its power-of-two exponent (exact_filter; F(2x2)'s U with it)."""
     w_tf = torch.as_tensor(w_tf, dtype=torch.float32).to(device).contiguous()
     fmt = fmt_of(dtype) if fmt is None else int(fmt)
     if kind == "conv2d_transpose":
@@ -264,17 +295,18 @@ def pack_conv(kind: str, w_tf: torch.Tensor, bias: Optional[torch.Tensor], alpha
     for k in ks:
         ntaps *= k
     packed = _alloc16((ntaps, cout_pad, cin), fmt, dtype, device)
+    w_pack, w_unscale = exact_filter(w_tf, fmt, exponent)
     if kind == "conv2d_transpose":
-        check(lib.rn_pack_conv2d_transpose_weights(w_tf.data_ptr(), packed.data_ptr(), ks[0], ks[1], cin, cout,
+        check(lib.rn_pack_conv2d_transpose_weights(w_pack.data_ptr(), packed.data_ptr(), ks[0], ks[1], cin, cout,
                                                    cout_pad, stride, fmt, _stream()), "pack transpose")
     else:
         if stride != 1:
             raise ValueError("tensor-core conv path is stride 1")
-        check(lib.rn_pack_conv_weights(w_tf.data_ptr(), packed.data_ptr(), ntaps, cin, cout, cout_pad, 0, None, 0,
+        check(lib.rn_pack_conv_weights(w_pack.data_ptr(), packed.data_ptr(), ntaps, cin, cout, cout_pad, 0, None, 0,
                                        fmt, _stream()), "pack")
     b = _pad_vec(bias if bias is not None else torch.zeros(cout), cout, cout_pad, device)
     a = _pad_vec(alpha, cout, cout_pad, device)
-    L = PackedConv(kind, ks, stride, cin, cout, cout_pad, packed, b, a, dtype, fmt)
+    L = PackedConv(kind, ks, stride, cin, cout, cout_pad, packed, b, a, dtype, fmt, w_unscale=w_unscale)
     if winograd and kind == "conv2d" and fmt == 2 and tuple(ks) == (3, 3) and cin == cout:
         L.master, L.master_version = w_tf, w_tf._version
     return L
@@ -335,13 +367,16 @@ def winograd4_filter_f32(w_tf: torch.Tensor):
 
 
 def winograd_filter_exp(L: PackedConv, tile: int = 2):
-    """(U as fp16 hi/lo planes [2][tile+2 squared][Cout][Cin], its power-of-two exponent: 0 for F(2x2)) of an exact-mode 3x3
-    layer, made on first use (an engine's warm-up, before graph capture) from the filter L was packed from."""
+    """(U as fp16 hi/lo planes [2][tile+2 squared][Cout][Cin], its power-of-two exponent) of an exact-mode 3x3 layer, made on
+    first use (an engine's warm-up, before graph capture) from the filter L was packed from.  F(2x2)'s U carries the layer's
+    filter exponent instead (U = G 2^s g G^T, undone by L.w_unscale in the epilogue), and the exponent returned is 0."""
     if L.wino is None:
         L.wino = {}
     if tile not in L.wino:
         if tile == 2:
             U, s = winograd_filter_f32(L.master), 0
+            if L.w_unscale is not None:
+                U = U / L.w_unscale                                    # a power of two: exact
         elif tile == 4:
             U, s = winograd4_filter_f32(L.master)
         else:
@@ -411,11 +446,11 @@ def conv2d(x: torch.Tensor, L: PackedConv, act: Optional[str] = None, residual: 
                                           _stream()), "rn_conv2d_winograd4")
         else:
             ws = torch.empty(lib.rn_winograd_workspace_bytes(B, H, W, Cin), device=x.device, dtype=torch.uint8)
-            check(lib.rn_conv2d_winograd(x.data_ptr(), U.data_ptr(), L.bias.data_ptr(), al, a, _ptr(residual), res_f32,
-                                         _ptr(out16), _ptr(out32), B, H, W, Cin, ws.data_ptr(), ws.numel(), _tune(tune),
-                                         _stream()), "rn_conv2d_winograd")
+            check(lib.rn_conv2d_winograd_scaled(x.data_ptr(), U.data_ptr(), _ptr(L.w_unscale), L.bias.data_ptr(), al, a,
+                                                _ptr(residual), res_f32, _ptr(out16), _ptr(out32), B, H, W, Cin, ws.data_ptr(),
+                                                ws.numel(), _tune(tune), _stream()), "rn_conv2d_winograd")
         return _ret(out16, out32, want16, want32, L.fmt)
-    check(lib.rn_conv2d_same(x.data_ptr(), L.w.data_ptr(), L.bias.data_ptr(),
+    check(lib.rn_conv2d_same_scaled(x.data_ptr(), L.w.data_ptr(), _ptr(L.w_unscale), L.bias.data_ptr(),
                              _ptr(alpha if alpha is not None else L.alpha) if a == ACT_PRELU else None, a, _ptr(residual), res_f32,
                              _ptr(out16), _ptr(out32), B, H, W, Cin, L.cout, L.cout_pad, L.ksize[0], L.ksize[1],
                              L.fmt, _tune(tune), _stream()), "rn_conv2d_same")
@@ -431,7 +466,7 @@ def conv3d(x: torch.Tensor, L: PackedConv, act: Optional[str] = None, residual: 
     out16, out32 = _out_buffers((B, H, W, D, L.cout), L.dtype, x.device, want16, want32, out16, out32, L.fmt)
     residual, res_f32 = _residual(residual, L.fmt)
     a = _ACT[act]
-    check(lib.rn_conv3d_same(x.data_ptr(), L.w.data_ptr(), L.bias.data_ptr(),
+    check(lib.rn_conv3d_same_scaled(x.data_ptr(), L.w.data_ptr(), _ptr(L.w_unscale), L.bias.data_ptr(),
                              _ptr(alpha if alpha is not None else L.alpha) if a == ACT_PRELU else None, a, _ptr(residual), res_f32,
                              _ptr(out16), _ptr(out32), B, H, W, D, Cin, L.cout, L.cout_pad, L.ksize[0],
                              L.fmt, _tune(tune), _stream()), "rn_conv3d_same")
@@ -443,7 +478,7 @@ class BandedConv3d:
     bias / alpha vectors (cached per D)."""
 
     def __init__(self, w_tf: torch.Tensor, bias: Optional[torch.Tensor], dtype=torch.float16, device="cuda", sz: int = 1,
-                 fmt: Optional[int] = None):
+                 fmt: Optional[int] = None, exponent: bool = False):
         w_tf = torch.as_tensor(w_tf, dtype=torch.float32).to(device).contiguous()
         assert tuple(w_tf.shape[:3]) == (3, 3, 3)
         self.cin, self.cout, self.sz = int(w_tf.shape[3]), int(w_tf.shape[4]), int(sz)
@@ -453,6 +488,7 @@ class BandedConv3d:
         self.dtype = dtype
         self.fmt = fmt_of(dtype) if fmt is None else int(fmt)
         self.w = _alloc16((nbytes // 2,), self.fmt, dtype, device)
+        w_tf, self.w_unscale = exact_filter(w_tf, self.fmt, exponent)
         check(lib.rn_pack_conv3d_banded(w_tf.data_ptr(), self.w.data_ptr(), self.cin, self.cout, self.sz, self.fmt,
                                         _stream()), "rn_pack_conv3d_banded")
         self.bias = (bias if bias is not None else torch.zeros(self.cout)).to(device=device, dtype=torch.float32)
@@ -500,7 +536,7 @@ def conv3d_banded(x: torch.Tensor, L: BandedConv3d, act: Optional[str] = None,
     residual, res_f32 = _residual(residual, L.fmt)
     a = _ACT[act]
     bias_full, alpha_full = _expanded_bias_alpha(L, a, alpha, alpha_tag, Do, x.device)
-    check(lib.rn_conv3d_banded_same(x.data_ptr(), L.w.data_ptr(), bias_full.data_ptr(), _ptr(alpha_full), a,
+    check(lib.rn_conv3d_banded_same_scaled(x.data_ptr(), L.w.data_ptr(), _ptr(L.w_unscale), bias_full.data_ptr(), _ptr(alpha_full), a,
                                     _ptr(residual), res_f32, _ptr(out16), _ptr(out32), B, H, W, D, Cin, L.cout, L.sz,
                                     L.fmt, _tune(tune), _stream()), "rn_conv3d_banded_same")
     return _ret(out16, out32, want16, want32, L.fmt)
@@ -514,7 +550,7 @@ class SlicedConv3d(BandedConv3d):
     TAP_ELEMS = 9 * 96 * 32            # 16-bit elements per plane of the packed filter
 
     def __init__(self, w_tf: torch.Tensor, bias: Optional[torch.Tensor], dtype=torch.float16, device="cuda",
-                 fmt: Optional[int] = None):
+                 fmt: Optional[int] = None, exponent: bool = False):
         w_tf = torch.as_tensor(w_tf, dtype=torch.float32).to(device).contiguous()
         if tuple(w_tf.shape) != (3, 3, 3, 32, 32):
             raise ValueError("the sliced conv3d is built for 3^3 filters with 32 input and 32 output channels")
@@ -522,6 +558,7 @@ class SlicedConv3d(BandedConv3d):
         self.dtype = dtype
         self.fmt = fmt_of(dtype) if fmt is None else int(fmt)
         self.w = _alloc16((self.TAP_ELEMS,), self.fmt, dtype, device)
+        w_tf, self.w_unscale = exact_filter(w_tf, self.fmt, exponent)
         check(lib.rn_pack_conv3d_sliced(w_tf.data_ptr(), self.w.data_ptr(), self.fmt, _stream()), "rn_pack_conv3d_sliced")
         self.bias = (bias if bias is not None else torch.zeros(self.cout)).to(device=device, dtype=torch.float32)
         self._full = {}
@@ -551,7 +588,7 @@ def conv3d_sliced(x: torch.Tensor, L: SlicedConv3d, act: Optional[str] = None,
     if a not in (ACT_NONE, ACT_PRELU):
         raise ValueError("the sliced conv3d fuses no activation or PReLU only")
     bias_full, alpha_full = _expanded_bias_alpha(L, a, alpha, alpha_tag, D, x.device)
-    check(lib.rn_conv3d_sliced_same(x.data_ptr(), L.w.data_ptr(), bias_full.data_ptr(), _ptr(alpha_full), a,
+    check(lib.rn_conv3d_sliced_same_scaled(x.data_ptr(), L.w.data_ptr(), _ptr(L.w_unscale), bias_full.data_ptr(), _ptr(alpha_full), a,
                                     _ptr(residual), res_f32, _ptr(out16), _ptr(out32), B, H, W, D, Cin, L.cout,
                                     L.fmt, _stream()), "rn_conv3d_sliced_same")
     return _ret(out16, out32, want16, want32, L.fmt)
@@ -566,7 +603,7 @@ def conv2d_transpose(x: torch.Tensor, L: PackedConv, act: Optional[str] = None, 
     s = L.stride
     out16, out32 = _out_buffers((B, H * s, W * s, L.cout), L.dtype, x.device, want16, want32, out16, out32, L.fmt)
     a = _ACT[act]
-    check(lib.rn_conv2d_transpose_same(x.data_ptr(), L.w.data_ptr(), L.bias.data_ptr(),
+    check(lib.rn_conv2d_transpose_same_scaled(x.data_ptr(), L.w.data_ptr(), _ptr(L.w_unscale), L.bias.data_ptr(),
                                        _ptr(alpha if alpha is not None else L.alpha) if a == ACT_PRELU else None, a, _ptr(out16), _ptr(out32),
                                        B, H, W, Cin, L.cout, L.cout_pad, L.ksize[0], L.ksize[1], s,
                                        L.fmt, _tune(tune), _stream()), "rn_conv2d_transpose_same")
@@ -577,12 +614,13 @@ class MergedConvT2:
     """k=4 stride-2 SAME transposed conv as one launch (rn_conv2d_transpose_s2_merged)."""
 
     def __init__(self, w_tf: torch.Tensor, bias: Optional[torch.Tensor], dtype=torch.float16, device="cuda",
-                 fmt: Optional[int] = None):
+                 fmt: Optional[int] = None, exponent: bool = False):
         w_tf = torch.as_tensor(w_tf, dtype=torch.float32).to(device).contiguous()
         assert tuple(w_tf.shape[:2]) == (4, 4)
         self.cout, self.cin, self.dtype = int(w_tf.shape[2]), int(w_tf.shape[3]), dtype
         self.fmt = fmt_of(dtype) if fmt is None else int(fmt)
         self.w = _alloc16((9, 4 * self.cout, self.cin), self.fmt, dtype, device)
+        w_tf, self.w_unscale = exact_filter(w_tf, self.fmt, exponent)
         check(lib.rn_pack_conv2d_transpose_s2_merged(w_tf.data_ptr(), self.w.data_ptr(), self.cin, self.cout, self.fmt,
                                                      _stream()), "pack merged tconv")
         b = bias if bias is not None else torch.zeros(self.cout)
@@ -609,7 +647,7 @@ def conv2d_transpose_s2_merged(x: torch.Tensor, L: MergedConvT2, act: Optional[s
             alpha4 = alpha.to(device=x.device, dtype=torch.float32).reshape(-1)[: L.cout].repeat(4).contiguous()
             if alpha_tag is not None:
                 L._alpha[alpha_tag] = alpha4
-    check(lib.rn_conv2d_transpose_s2_merged(x.data_ptr(), L.w.data_ptr(), L.bias.data_ptr(), _ptr(alpha4), a, _ptr(out16),
+    check(lib.rn_conv2d_transpose_s2_merged_scaled(x.data_ptr(), L.w.data_ptr(), _ptr(L.w_unscale), L.bias.data_ptr(), _ptr(alpha4), a, _ptr(out16),
                                             _ptr(out32), B, H, W, Cin, L.cout, L.fmt, _tune(tune), _stream()),
           "rn_conv2d_transpose_s2_merged")
     return _ret(out16, out32, want16, want32, L.fmt)
@@ -619,13 +657,14 @@ class XFoldConvT:
     """Stride-1 transposed conv with thin channels, x-folded (rn_conv2d_transpose_s1_xfold)."""
 
     def __init__(self, w_tf: torch.Tensor, bias: Optional[torch.Tensor], F: int, dtype=torch.float16, device="cuda",
-                 fmt: Optional[int] = None):
+                 fmt: Optional[int] = None, exponent: bool = False):
         w_tf = torch.as_tensor(w_tf, dtype=torch.float32).to(device).contiguous()
         self.kh, self.kw, self.cout, self.cin = (int(v) for v in w_tf.shape)
         self.F, self.dtype = F, dtype
         self.fmt = fmt_of(dtype) if fmt is None else int(fmt)
         self.cout_pad = round_up(F * self.cout, 16)
         self.w = _alloc16((self.kh * 3, self.cout_pad, F * self.cin), self.fmt, dtype, device)
+        w_tf, self.w_unscale = exact_filter(w_tf, self.fmt, exponent)
         check(lib.rn_pack_conv2d_transpose_xfold(w_tf.data_ptr(), self.w.data_ptr(), self.kh, self.kw, self.cin, self.cout,
                                                  F, self.cout_pad, self.fmt, _stream()), "pack xfold")
         b = bias if bias is not None else torch.zeros(self.cout)
@@ -676,7 +715,7 @@ def conv2d_transpose_xfold(x: torch.Tensor, L: XFoldConvT, act: Optional[str] = 
             alpha_x = L.tiled(alpha, x.device)
             if alpha_tag is not None:
                 L._alpha[alpha_tag] = alpha_x
-    check(lib.rn_conv2d_transpose_s1_xfold(x.data_ptr(), L.w.data_ptr(), L.bias.data_ptr(), _ptr(alpha_x), a, _ptr(out16),
+    check(lib.rn_conv2d_transpose_s1_xfold_scaled(x.data_ptr(), L.w.data_ptr(), _ptr(L.w_unscale), L.bias.data_ptr(), _ptr(alpha_x), a, _ptr(out16),
                                            _ptr(out32), B, H, W, Cin, L.cout, L.kh, L.kw, L.F, L.cout_pad, L.fmt,
                                            C.byref(ph) if ph is not None else None, _tune(tune), _stream()),
           "rn_conv2d_transpose_s1_xfold")
@@ -687,9 +726,10 @@ def conv2d_transpose_xfold(x: torch.Tensor, L: XFoldConvT, act: Optional[str] = 
 
 def conv_igemm_raw(x, w_packed, bias, taps, ndim, B, H, W, D, Cin, Cout, cout_pad, out16=None, out32=None,
                    alpha=None, act=ACT_NONE, residual=None, o=None, fmt=0, force_bn=0, force_kps=0, max_ctas=0,
-                   cluster=0, cta_group=0, ny=0, tile_w=0, msub=0, epi_groups=0, res_prefetch=0, tma_store=0):
+                   cluster=0, cta_group=0, ny=0, tile_w=0, msub=0, epi_groups=0, res_prefetch=0, tma_store=0, w_unscale=None):
     """Direct access to rn_conv_igemm for tests / tuning.  taps: list of (dx,dy,dz).  fmt 2: x, w_packed, out16 and a
-    16-bit residual are [2, ...] hi/lo plane tensors (or Split16).  bias None: the raw fp32 sums (out32 only)."""
+    16-bit residual are [2, ...] hi/lo plane tensors (or Split16), and w_unscale the layer's 2^-s (exact_filter).  bias None:
+    the raw fp32 sums (out32 only)."""
     n = len(taps)
     arr = (C.c_int8 * (3 * n))(*[v for t in taps for v in t])
     x, w_packed, out16, residual = _unwrap(x), _unwrap(w_packed), _unwrap(out16), _unwrap(residual)
@@ -713,6 +753,7 @@ def conv_igemm_raw(x, w_packed, bias, taps, ndim, B, H, W, D, Cin, Cout, cout_pa
     d.cta_group = cta_group
     d.ny, d.tile_w, d.msub = ny, tile_w, msub
     d.epi_groups, d.res_prefetch, d.tma_store = epi_groups, res_prefetch, tma_store
+    d.w_unscale = _ptr(w_unscale)
     if fmt == 2:
         d.x_plane = x.numel() // 2
         d.w_plane = w_packed.numel() // 2
@@ -1119,7 +1160,7 @@ def concat_channels(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
 
 # --------------------------------------------------------------------------------------- backward (input gradients)
 def conv2d_taps(x, w_packed, bias, taps, cout: int, cout_pad: int, fmt: int, residual=None, ny: int = 0, want32: bool = False,
-                dtype: torch.dtype = torch.float16):
+                dtype: torch.dtype = torch.float16, w_unscale=None):
     """Stride-1 2-D convolution with an explicit tap list (dx, dy) over the packed filter [ntaps][cout_pad][Cin]
     (rn_conv_igemm): what the data gradients of the k = 4 convolutions need (their mirrored taps are not a TF SAME set).
     x: 16-bit [B,H,W,Cin] (Split16 for fmt 2); returns 16-bit [B,H,W,cout] (or fp32 with want32)."""
@@ -1129,7 +1170,7 @@ def conv2d_taps(x, w_packed, bias, taps, cout: int, cout_pad: int, fmt: int, res
     out32 = torch.empty((B, H, W, cout), device=x.device, dtype=torch.float32) if want32 else None
     residual, _ = _residual(residual, fmt)
     conv_igemm_raw(x, w_packed, bias, [(int(t[0]), int(t[1]), 0) for t in taps], 2, B, H, W, 1, Cin, cout, cout_pad,
-                   out16=out16, out32=out32, residual=residual, fmt=fmt, ny=ny)
+                   out16=out16, out32=out32, residual=residual, fmt=fmt, ny=ny, w_unscale=w_unscale)
     return out32 if want32 else _wrap16(out16, fmt)
 
 
