@@ -406,6 +406,12 @@ int rn_phong_composite(const float* img, const float* light_dir, const float* li
 int rn_phong_shade(const float* normal, const float* albedo, const float* light_dir, const float* light_col, float ambient,
                    float k_diffuse, int composite, int background_white, int with_mask, float* shade_f32, float* compos_f32,
                    uint8_t* compos_u8, int B, int H, int W, void* stream);
+/* rn_phong_shade with the ambient term per item: ambient [B] fp32 on the device (the fitted shading of
+ * rn_phong_shade_backward_params and the fits).  The arithmetic is the scalar entry's, with the value loaded instead of passed:
+ * a uniform ambient array gives rn_phong_shade's bits. */
+int rn_phong_shade_ambient(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
+                           const float* ambient, float k_diffuse, int composite, int background_white, int with_mask,
+                           float* shade_f32, float* compos_f32, uint8_t* compos_u8, int B, int H, int W, void* stream);
 
 /* ---- backward pass: input gradients of the forward path (SURVEY 8 f-4) --------------------------------------------
  * What inverse rendering differentiates through the frozen network (Reconstruct_RenderNet_Face.py:383-412).  The data
@@ -487,6 +493,26 @@ int rn_phong_shade_backward(const float* normal, const float* albedo, const floa
                             float ambient, float k_diffuse, int composite, int background_white, int with_mask,
                             const float* g_compos, float* d_normal, float* d_albedo, float* d_light_dir, int B, int H, int W,
                             void* stream);
+/* Gradients of the shading parameters.  Each *_params entry is the entry above it with ambient read per item from a device array
+ * [B] (as rn_phong_shade_ambient) and two more outputs, each ACCUMULATED into (zero them first) and each may be NULL:
+ * d_light_col [B,3] and d_ambient [B].  Per pixel, with dx_c the upstream gradient passed through the outer clip(x, 0, 1) and
+ * dpre_c the one passed on through the diffuse clip (times the mask m, 1 without a mask):
+ *   d_ambient += sum_c m dx_c,   d_light_col_c += dpre_c fl(k_diffuse max(d, 0)),
+ * summed over the item's pixels, one atomic per block and component.  k_diffuse has no gradient: the composites see only the
+ * product k_diffuse col, which the fitted colour absorbs.  Every other output is the scalar entry's bit for bit when the ambient
+ * array holds the scalar. */
+int rn_phong_recon_loss_grad_params(const float* albedo, const float* normal, const float* target, const float* light_dir,
+                                    const float* light_col, const float* ambient, float k_diffuse, int black_background,
+                                    int with_mask, double* loss, float* d_albedo, float* d_normal, float* d_light_dir,
+                                    float* d_light_col, float* d_ambient, int B, int H, int W, void* stream);
+int rn_phong_composite_loss_grad_params(const float* img, const float* target, const float* light_dir, const float* light_col,
+                                        const float* ambient, float k_diffuse, int background_white, int with_mask, double* loss,
+                                        float* d_img, float* d_light_dir, float* d_light_col, float* d_ambient, int B, int H,
+                                        int W, void* stream);
+int rn_phong_shade_backward_params(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
+                                   const float* ambient, float k_diffuse, int composite, int background_white, int with_mask,
+                                   const float* g_compos, float* d_normal, float* d_albedo, float* d_light_dir,
+                                   float* d_light_col, float* d_ambient, int B, int H, int W, void* stream);
 long long rn_fully_connected_backward_workspace(int B, int K, int N);
 int rn_fully_connected_backward_data(const float* g, const float* w, float* work, float* dx, int B, int K, int N, void* stream);
 
@@ -640,6 +666,26 @@ int rn_phong_shade_backward_fixed(const float* normal, const float* albedo, cons
                                   float ambient, float k_diffuse, int composite, int background_white, int with_mask,
                                   const float* g_compos, float* d_normal, float* d_albedo, float* d_light_dir, int B, int H, int W,
                                   void* work, long long work_bytes, void* stream);
+/* twins of the *_params entries: d_light_col and d_ambient from per-block partials added in block order, like d_light_dir.
+ * rn_phong_shade_backward_params_fixed needs no work when d_light_dir, d_light_col and d_ambient are all NULL. */
+long long rn_phong_recon_loss_grad_params_fixed_workspace(int B, int H, int W);
+int rn_phong_recon_loss_grad_params_fixed(const float* albedo, const float* normal, const float* target, const float* light_dir,
+                                          const float* light_col, const float* ambient, float k_diffuse, int black_background,
+                                          int with_mask, double* loss, float* d_albedo, float* d_normal, float* d_light_dir,
+                                          float* d_light_col, float* d_ambient, int B, int H, int W, void* work,
+                                          long long work_bytes, void* stream);
+long long rn_phong_composite_loss_grad_params_fixed_workspace(int B, int H, int W);
+int rn_phong_composite_loss_grad_params_fixed(const float* img, const float* target, const float* light_dir,
+                                              const float* light_col, const float* ambient, float k_diffuse, int background_white,
+                                              int with_mask, double* loss, float* d_img, float* d_light_dir, float* d_light_col,
+                                              float* d_ambient, int B, int H, int W, void* work, long long work_bytes,
+                                              void* stream);
+long long rn_phong_shade_backward_params_fixed_workspace(int B, int H, int W);
+int rn_phong_shade_backward_params_fixed(const float* normal, const float* albedo, const float* light_dir,
+                                         const float* light_col, const float* ambient, float k_diffuse, int composite,
+                                         int background_white, int with_mask, const float* g_compos, float* d_normal,
+                                         float* d_albedo, float* d_light_dir, float* d_light_col, float* d_ambient, int B, int H,
+                                         int W, void* work, long long work_bytes, void* stream);
 long long rn_image_loss_grad_items_fixed_workspace(long long npix, int C, int batch);
 int rn_image_loss_grad_items_fixed(const float* img, const float* target, float* dimg, double* loss, long long npix, int C,
                                    int batch, int kind, void* work, long long work_bytes, void* stream);

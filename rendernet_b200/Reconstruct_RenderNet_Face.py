@@ -213,13 +213,15 @@ def light_pos(light_azimuth, light_elevation) -> np.ndarray:
 
 
 def reconstruction_gradients(tig, voxels, texture, view_params, light_azimuth, target, light_elevation, ambient=0.,
-                             k_diffuse=1., light_col=(1.0, 1.0, 1.0), dvox_on_device=False):
+                             k_diffuse=1., light_col=(1.0, 1.0, 1.0), dvox_on_device=False, want_shading_grad=False):
     """Loss and gradients of one reconstruction step (:358-412): compos = albedo * tf_phong_composite(normal, light(azimuth,
     elevation), light_col, ambient, k_diffuse, with_mask=True) (white background), loss[b] = mean (target - compos)^2.
     tig: a backward.TextureInputGradients of the batch size (model "pretrained" for the reference's network).  Returns
     (loss [B] float64, dL/dvoxels [B,64,64,64,1], dL/dtexture [B,199], dL/dview_params [B,3], dL/dlight_azimuth [B,1]); the
     objective and its image gradients run in rn_phong_recon_loss_grad, the azimuth map is differentiated on the host in float64.
-    dvox_on_device: dL/dvoxels is returned as a CUDA tensor (what ShapeDecoderGradients.backward takes)."""
+    dvox_on_device: dL/dvoxels is returned as a CUDA tensor (what ShapeDecoderGradients.backward takes).  light_col: 1 or B rows
+    of 3; ambient: a float or a [1|B] tensor.  want_shading_grad: two more results, dL/dlight_col [B,3] and dL/dambient [B]
+    (float64, rn_phong_recon_loss_grad_params)."""
     albedo, normal = tig.forward(voxels, texture, view_params)
     dev = albedo.device
     B = albedo.shape[0]
@@ -229,17 +231,22 @@ def reconstruction_gradients(tig, voxels, texture, view_params, light_azimuth, t
     tgt = torch.as_tensor(np.asarray(target, np.float32) if not isinstance(target, torch.Tensor) else target)
     tgt = tgt.to(device=dev, dtype=torch.float32).reshape(tuple(albedo.shape)).contiguous()
     with torch.cuda.device(dev):
-        loss, d_albedo, d_normal, d_light = ops.phong_recon_loss_grad(albedo, normal, tgt, ldir, lcol, ambient, k_diffuse,
-                                                                      black_background=False, with_mask=True)
+        out = ops.phong_recon_loss_grad(albedo, normal, tgt, ldir, lcol, ambient, k_diffuse, black_background=False,
+                                        with_mask=True, **(dict(want_shading_grad=True) if want_shading_grad else {}))
+        loss, d_albedo, d_normal, d_light = out[:4]
     dvox, dtex, dpose = tig.backward(d_albedo, d_normal, dvox_on_device=dvox_on_device)
     dl = d_light.double().cpu().numpy()
     el = float(np.float32(light_elevation))
     # d light / d azimuth = (-sin(el) sin(az), sin(el) cos(az), 0)
     dlaz = (dl[:, 0:1] * -np.sin(el) * np.sin(az) + dl[:, 1:2] * np.sin(el) * np.cos(az))
+    if want_shading_grad:
+        return loss.cpu().numpy(), dvox, dtex, dpose, dlaz, out[4].double().cpu().numpy(), out[5].double().cpu().numpy()
     return loss.cpu().numpy(), dvox, dtex, dpose, dlaz
 
 
 # ------------------------------------------------------------------------------------------ the reconstruction (:304-537)
+# step size of the light colour and the ambient term (FaceReconstruction(fit_shading=True)): not in the reference, not tuned
+SHADING_ETA = 0.5
 RECON_DEFAULTS = dict(shape_eta=0.8, pose_eta=0.01, tex_eta=0.8, light_eta=0.4, inner_step=200, max_epochs=10, z_dim=200,
                       target_azimuth_light=294.0, target_elevation_light=105.0)     # config_reconstruction_RenderNet.json
 
@@ -266,7 +273,8 @@ def create_param_center(phi_mid=90, phi_range=240, theta_mid=90, theta_range=120
 
 
 def reconstruction_loop(step_fn: Callable, loss_fn: Callable, target, batch_size: int = 5, z_dim: int = 200, max_epochs: int = 10,
-                        inner_step: int = 200, seed: int = 0, callback: Optional[Callable] = None) -> Dict[str, object]:
+                        inner_step: int = 200, seed: int = 0, callback: Optional[Callable] = None,
+                        shading: Optional[dict] = None) -> Dict[str, object]:
     """The outer / inner loop of :455-537 over any step function.
 
     step_fn(state, target) -> (new_state, loss [B], grads): one inner step from `state` {"latent" [B,z_dim], "pose" [B,3] (radians),
@@ -280,14 +288,16 @@ def reconstruction_loop(step_fn: Callable, loss_fn: Callable, target, batch_size
     selection_loss is the re-evaluated loss [B] after the last inner step of an epoch, else None.
 
     Returns {"latent", "texture", "light", "pose" (radians, the selected hypothesis), "best_param" (the reference's degree
-    form), "best_index", "best_loss" (per epoch), "state" (the last state)}."""
+    form), "best_index", "best_loss" (per epoch), "state" (the last state)}.
+    shading: the first epoch's {"light_col" [5,3], "ambient" [5]} or None; given, they join the state, later epochs restart from
+    the selected hypothesis' values, and the result holds the selected "light_col" [3] and "ambient"."""
     if batch_size != 5:
         raise ValueError(f"the reconstruction loop runs 5 pose hypotheses (create_param_center); batch_size is {batch_size}")
     rng = np.random.default_rng(seed)
     best_param = np.zeros(shape=(3))
     best_vector = np.zeros(shape=(z_dim))
     best_tex = np.zeros(shape=(199))
-    best_light = None
+    best_light = best_shading = None
     best_pose = best_index = None
     best_loss = []
     phi_range = 60
@@ -311,6 +321,10 @@ def reconstruction_loop(step_fn: Callable, loss_fn: Callable, target, batch_size
         # the assign ops of :481 store into float32 variables
         state = dict(latent=np.asarray(vector_batch, np.float32), pose=np.asarray(params_batch, np.float32),
                      texture=np.asarray(tex_batch, np.float32), light=np.asarray(light_batch, np.float32))
+        if shading is not None:
+            for k in ("light_col", "ambient"):
+                state[k] = (np.asarray(shading[k], np.float32).copy() if i == 0 else
+                            np.repeat(best_shading[k][np.newaxis], batch_size, 0))
         for idx in range(inner_step):
             state, loss, _ = step_fn(state, target)
             sel = None
@@ -320,6 +334,8 @@ def reconstruction_loop(step_fn: Callable, loss_fn: Callable, target, batch_size
                 best_vector = state["latent"][j]
                 best_tex = state["texture"][j]
                 best_light = state["light"][j]
+                if shading is not None:
+                    best_shading = {k: np.asarray(state[k][j], np.float32).copy() for k in ("light_col", "ambient")}
                 best_pose = state["pose"][j].copy()
                 best_param = state["pose"][j] * 180. / math.pi
                 best_param = np.array([best_param[0], 90 - best_param[1], 1])
@@ -327,8 +343,11 @@ def reconstruction_loop(step_fn: Callable, loss_fn: Callable, target, batch_size
                 best_loss.append(float(sel[j]))
             if callback is not None:
                 callback(i, idx, state, loss, sel)
-    return dict(latent=best_vector, texture=best_tex, light=best_light, pose=best_pose, best_param=best_param,
-                best_index=best_index, best_loss=best_loss, state=state)
+    out = dict(latent=best_vector, texture=best_tex, light=best_light, pose=best_pose, best_param=best_param,
+               best_index=best_index, best_loss=best_loss, state=state)
+    if shading is not None:
+        out.update(best_shading)
+    return out
 
 
 class FaceReconstruction:
@@ -339,15 +358,24 @@ class FaceReconstruction:
         out = rec.run(target)                                               # latent, texture, pose, light, voxels, ...
 
     The render network runs in `precision` ("exact" or "fast"); the shape and texture decoders run in fp32 in both modes.
-    Defaults are those of config_reconstruction_RenderNet.json (RECON_DEFAULTS)."""
+    Defaults are those of config_reconstruction_RenderNet.json (RECON_DEFAULTS).
+
+    fit_shading: the state also holds the light colour "light_col" [B,3] and the ambient term "ambient" [B], starting from the
+    reference's white light and ambient 0; step descends them with shading_eta (SHADING_ETA: untuned, not in the reference) and
+    projects them onto colour >= 0, 0 <= ambient <= 1; run returns the selected values and render shades with the state's.
+    k_diffuse stays 1: the composite sees only k_diffuse * colour, which the fitted colour absorbs."""
 
     def __init__(self, weight_dict, weight_dict_decoder, batch: int = 5, precision: str = "exact", shape_eta: float = 0.8,
                  pose_eta: float = 0.01, tex_eta: float = 0.8, light_eta: float = 0.4, inner_step: int = 200,
                  max_epochs: int = 10, z_dim: int = 200, target_azimuth_light: float = 294.0,
-                 target_elevation_light: float = 105.0, seed: int = 0, device: str = "cuda"):
+                 target_elevation_light: float = 105.0, seed: int = 0, device: str = "cuda", fit_shading: bool = False,
+                 shading_eta: float = SHADING_ETA):
         from .backward import ShapeDecoderGradients, TextureInputGradients
         self.B = int(batch)
         self.eta = dict(latent=float(shape_eta), pose=float(pose_eta), texture=float(tex_eta), light=float(light_eta))
+        self.fit_shading = bool(fit_shading)
+        if self.fit_shading:
+            self.eta["shading"] = float(shading_eta)
         self.inner_step, self.max_epochs, self.z_dim, self.seed = int(inner_step), int(max_epochs), int(z_dim), int(seed)
         self.elevation = (90 - target_elevation_light) * math.pi / 180.0        # :330-331
         self.azimuth = target_azimuth_light * math.pi / 180.0
@@ -375,9 +403,32 @@ class FaceReconstruction:
             self._target = (target, torch.as_tensor(np.asarray(target, np.float32)).to(self.device).contiguous())
         return self._target[1]
 
+    def initial_shading(self) -> Optional[dict]:
+        """The first epoch's {"light_col" [B,3], "ambient" [B]}: the reference's white light and ambient 0 (None without
+        fit_shading)."""
+        if not self.fit_shading:
+            return None
+        return dict(light_col=np.ones((self.B, 3), np.float32), ambient=np.zeros(self.B, np.float32))
+
+    def _shading(self, state):
+        """(light_col, ambient) at `state`: the reference's constants, or the state's with fit_shading."""
+        if not self.fit_shading:
+            return (1.0, 1.0, 1.0), 0.
+        return (np.asarray(state["light_col"], np.float32),
+                torch.as_tensor(np.asarray(state["ambient"], np.float32)).to(self.device))
+
     def gradients(self, state, target):
         """Loss [B] and the gradients of sum_b loss[b] (tf.gradients of the loss vector, :402) with respect to the latent [B,200],
-        the pose [B,3], the texture [B,199] and the light azimuth [B,1], at `state`."""
+        the pose [B,3], the texture [B,199] and the light azimuth [B,1], at `state`; with fit_shading also the light colour
+        [B,3] and the ambient term [B]."""
+        if self.fit_shading:
+            vox = self.sdg.forward(state["latent"])
+            lcol, amb = self._shading(state)
+            loss, dvox, dtex, dpose, dlight, dcol, damb = reconstruction_gradients(
+                self.tig, vox, state["texture"], state["pose"], state["light"], self._target_dev(target), self.elevation,
+                ambient=amb, light_col=lcol, dvox_on_device=True, want_shading_grad=True)
+            return loss, dict(latent=self.sdg.backward(dvox), pose=dpose, texture=dtex, light=dlight, light_col=dcol,
+                              ambient=damb)
         vox = self.sdg.forward(state["latent"])
         loss, dvox, dtex, dpose, dlight = reconstruction_gradients(self.tig, vox, state["texture"], state["pose"], state["light"],
                                                                    self._target_dev(target), self.elevation, dvox_on_device=True)
@@ -389,6 +440,12 @@ class FaceReconstruction:
         loss, grads = self.gradients(state, target)
         new = {k: (np.asarray(state[k], np.float32) - np.float32(self.eta[k]) * np.asarray(grads[k], np.float32)).astype(np.float32)
                for k in ("latent", "pose", "texture", "light")}
+        if self.fit_shading:
+            eta = np.float32(self.eta["shading"])
+            new["light_col"] = np.maximum(np.asarray(state["light_col"], np.float32) -
+                                          eta * np.asarray(grads["light_col"], np.float32), np.float32(0)).astype(np.float32)
+            new["ambient"] = np.clip(np.asarray(state["ambient"], np.float32) - eta * np.asarray(grads["ambient"], np.float32),
+                                     np.float32(0), np.float32(1)).astype(np.float32)
         return new, loss, grads
 
     def loss(self, state, target) -> np.ndarray:
@@ -399,8 +456,12 @@ class FaceReconstruction:
         az = np.asarray(state["light"], np.float64).reshape(B, 1)
         with torch.cuda.device(self.device):
             ldir = torch.from_numpy(light_pos(az, self.elevation)).to(self.device)
-            lcol = torch.ones((B, 3), device=self.device, dtype=torch.float32)
-            loss = ops.phong_recon_loss_grad(albedo, normal, self._target_dev(target), ldir, lcol, 0., 1.,
+            if self.fit_shading:
+                lc, amb = self._shading(state)
+                lcol = torch.from_numpy(lc).to(self.device)
+            else:
+                lcol, amb = torch.ones((B, 3), device=self.device, dtype=torch.float32), 0.
+            loss = ops.phong_recon_loss_grad(albedo, normal, self._target_dev(target), ldir, lcol, amb, 1.,
                                              black_background=False, with_mask=True)[0]
         return loss.cpu().numpy()
 
@@ -408,7 +469,8 @@ class FaceReconstruction:
         """The images of a state (what :497-508 fetches every 100 steps): the shape decoder, the Texture+Normal network and the
         shading of :372-378 (rn_phong_shade, TensorFlow's composite, white background, mask, ambient 0, k_d 1, light colour 1),
         i.e. the very image the loss measures.  view_params [B,3] / light_azimuth [B,1] (radians) render the state's face from
-        another pose or under another light; None keeps the state's own.  Returns NumPy albedo, normal, shading, compos
+        another pose or under another light; None keeps the state's own (with fit_shading the state's colour and ambient term
+        shade it).  Returns NumPy albedo, normal, shading, compos
         (float32 [B,512,512,3]), compos_u8 (clip(255 compos) as uint8) and voxels ([B,64,64,64] float32)."""
         B = self.B
         pose = state["pose"] if view_params is None else view_params
@@ -419,7 +481,8 @@ class FaceReconstruction:
         albedo, normal = self.tig.forward(vox, state["texture"], pose)
         with torch.cuda.device(self.device):
             ldir = torch.from_numpy(light_pos(az, self.elevation)).to(self.device)
-            shade, compos, u8 = ops.phong_shade(normal, ldir, (1.0, 1.0, 1.0), 0., 1., albedo=albedo, composite="tf",
+            lcol, amb = self._shading(state)
+            shade, compos, u8 = ops.phong_shade(normal, ldir, lcol, amb, 1., albedo=albedo, composite="tf",
                                                 background_white=True, with_mask=True)
         out = dict(albedo=albedo, normal=normal, shading=shade, compos=compos, compos_u8=u8, voxels=vox[..., 0])
         return {k: v.cpu().numpy() for k, v in out.items()}
@@ -427,8 +490,9 @@ class FaceReconstruction:
     def run(self, target, callback: Optional[Callable] = None) -> Dict[str, object]:
         """The whole reconstruction (:455-537) from a shaded target [B,512,512,3]: reconstruction_loop with this object's step and
         loss.  Returns its dictionary plus "voxels" [64,64,64] (the decoded best latent) as NumPy."""
+        more = dict(shading=self.initial_shading()) if self.fit_shading else {}
         out = reconstruction_loop(self.step, self.loss, target, batch_size=self.B, z_dim=self.z_dim, max_epochs=self.max_epochs,
-                                  inner_step=self.inner_step, seed=self.seed, callback=callback)
+                                  inner_step=self.inner_step, seed=self.seed, callback=callback, **more)
         vox = self.sdg.forward(np.tile(np.asarray(out["latent"], np.float32)[None], (self.B, 1)))
         out["voxels"] = vox[0, ..., 0].cpu().numpy()
         return out

@@ -144,6 +144,16 @@ SIGNATURES = {
     "rn_phong_shade_backward_fixed": (_i, [_vp, _vp, _vp, _vp, _f, _f, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _ll, _vp]),
     "rn_image_loss_grad_items_fixed_workspace": (_ll, [_ll, _i, _i]),
     "rn_image_loss_grad_items_fixed": (_i, [_vp, _vp, _vp, _vp, _ll, _i, _i, _i, _vp, _ll, _vp]),
+    "rn_phong_shade_ambient": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "rn_phong_recon_loss_grad_params": (_i, [_vp] * 6 + [_f, _i, _i] + [_vp] * 6 + [_i, _i, _i, _vp]),
+    "rn_phong_composite_loss_grad_params": (_i, [_vp] * 5 + [_f, _i, _i] + [_vp] * 5 + [_i, _i, _i, _vp]),
+    "rn_phong_shade_backward_params": (_i, [_vp] * 5 + [_f, _i, _i, _i] + [_vp] * 6 + [_i, _i, _i, _vp]),
+    "rn_phong_recon_loss_grad_params_fixed_workspace": (_ll, [_i] * 3),
+    "rn_phong_recon_loss_grad_params_fixed": (_i, [_vp] * 6 + [_f, _i, _i] + [_vp] * 6 + [_i, _i, _i, _vp, _ll, _vp]),
+    "rn_phong_composite_loss_grad_params_fixed_workspace": (_ll, [_i] * 3),
+    "rn_phong_composite_loss_grad_params_fixed": (_i, [_vp] * 5 + [_f, _i, _i] + [_vp] * 5 + [_i, _i, _i, _vp, _ll, _vp]),
+    "rn_phong_shade_backward_params_fixed_workspace": (_ll, [_i] * 3),
+    "rn_phong_shade_backward_params_fixed": (_i, [_vp] * 5 + [_f, _i, _i, _i] + [_vp] * 6 + [_i, _i, _i, _vp, _ll, _vp]),
 }
 # the exact-mode companions rn_*_scaled: the same arguments plus w_unscale (a device pointer) after the packed filter
 for _name, _at in (("rn_conv2d_same", 2), ("rn_conv3d_same", 2), ("rn_conv3d_banded_same", 2), ("rn_conv3d_sliced_same", 2),

@@ -533,6 +533,43 @@ __global__ void fc_bwd_data_reduce_kernel(const float* __restrict__ part, float*
   dx[i] = s;
 }
 
+// ------------------------------------------------------------------------------------------ shading-parameter gradients
+// The SP instantiations of the three Phong kernels below (rn_*_params) also sum, per item, dL/d light_col (3) and dL/d ambient
+// (phong_param_backward, rn_phong.cuh) and read the ambient term per item from ambient_b[b].  block_sum4 reduces the four terms
+// over the block (the result in thread 0) and store_param_grads writes them: one atomic per block and component (d_col [B,3],
+// d_amb [B], each may be NULL), or FX: to pslots[b][blockIdx.x][3] (colour) and pslots[3 B nblk + b nblk + blockIdx.x]
+// (ambient), summed in block order by slot_sum_kernel.  Every thread of the block calls block_sum4.
+__device__ __forceinline__ void block_sum4(float* v) {
+  __shared__ float red4[8][4];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float x = v[i];
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
+    if (lane == 0) red4[wib][i] = x;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < 4; ++i) v[i] = 0.f;
+    for (int w = 0; w < 8; ++w)
+      for (int i = 0; i < 4; ++i) v[i] += red4[w][i];
+  }
+}
+
+template <bool FX>
+__device__ __forceinline__ void store_param_grads(const float* v, int b, float* d_col, float* d_amb, double* pslots) {
+  if constexpr (FX) {
+    double* sl = pslots + (static_cast<size_t>(b) * gridDim.x + blockIdx.x) * 3;
+    for (int i = 0; i < 3; ++i) sl[i] = v[i];
+    pslots[3 * static_cast<size_t>(gridDim.y) * gridDim.x + static_cast<size_t>(b) * gridDim.x + blockIdx.x] = v[3];
+  } else {
+    if (d_col != nullptr)
+      for (int i = 0; i < 3; ++i) atomicAdd(d_col + 3 * b + i, v[i]);
+    if (d_amb != nullptr) atomicAdd(d_amb + b, v[3]);
+  }
+}
+
 // ------------------------------------------------------------------------------------------ face reconstruction objective
 // Reconstruct_RenderNet_Face.py:372-383 over TensorFlow's Phong composite (tools/Phong_shading.py:24-113 tf_mask /
 // tf_mask_white / tf_phong_shading / tf_phong_composite -- NOT the NumPy composite of phong_pixel):
@@ -547,16 +584,21 @@ __global__ void fc_bwd_data_reduce_kernel(const float* __restrict__ part, float*
 // the pixel adds nothing to d_light.  Where |n| = 0 the mask term is 0.  One thread per pixel; blockIdx.y = batch item.  loss is
 // accumulated in double (one atomic per block); dL/dL is reduced over the block and mapped through the normalisation
 // (I - L L^T) / |l| before one atomic per block and component.  FX (the fixed-order twin): the block's loss and d_light terms go
-// to slots[b][blockIdx.x][4] instead, summed in block order by slot_sum_kernel; the per-pixel code is the same.
-template <bool FX>
+// to slots[b][blockIdx.x][4] instead, summed in block order by slot_sum_kernel; the per-pixel code is the same.  SP: see
+// block_sum4 (pslots is used by FX only, d_col / d_amb by the atomic kernel only).
+template <bool FX, bool SP>
 __global__ void __launch_bounds__(256) phong_recon_loss_grad_kernel(const float* __restrict__ albedo, const float* __restrict__ normal,
                                                                     const float* __restrict__ target, const float* __restrict__ light_dir,
                                                                     const float* __restrict__ light_col, float ambient, float k_diffuse,
                                                                     int black, int with_mask, double* __restrict__ loss,
                                                                     float* __restrict__ d_albedo, float* __restrict__ d_normal,
-                                                                    float* __restrict__ d_light, int HW, double* __restrict__ slots) {
+                                                                    float* __restrict__ d_light, int HW, double* __restrict__ slots,
+                                                                    const float* __restrict__ ambient_b, float* __restrict__ d_col,
+                                                                    float* __restrict__ d_amb, double* __restrict__ pslots) {
   __shared__ float red[8][4];
   const int b = blockIdx.y;
+  if constexpr (SP) ambient = __ldg(ambient_b + b);
+  float pg[4] = {0.f, 0.f, 0.f, 0.f};                                  // SP: dL/d col (3), dL/d ambient
   const float l0 = __ldg(light_dir + 3 * b), l1 = __ldg(light_dir + 3 * b + 1), l2 = __ldg(light_dir + 3 * b + 2);
   const float lnorm = sqrtf(l0 * l0 + l1 * l1 + l2 * l2);
   const float L[3] = {l0 / lnorm, l1 / lnorm, l2 / lnorm};
@@ -581,8 +623,15 @@ __global__ void __launch_bounds__(256) phong_recon_loss_grad_kernel(const float*
       ds[c] = dpred * a;
     }
     tf_phong_pixel_backward(n, L, t, col, ambient, k_diffuse, black, with_mask, ds, dn, part + 1);
+    if constexpr (SP) phong_param_backward(t.d, t.m, t.pre, t.x, k_diffuse, with_mask, ds, pg, pg + 3);
 #pragma unroll
     for (int i = 0; i < 3; ++i) d_normal[o + i] = dn[i];
+  }
+  if constexpr (SP) {
+    if (FX ? pslots != nullptr : (d_col != nullptr || d_amb != nullptr)) {
+      block_sum4(pg);
+      if (threadIdx.x == 0) store_param_grads<FX>(pg, b, d_col, d_amb, pslots);
+    }
   }
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
 #pragma unroll
@@ -621,17 +670,21 @@ __global__ void __launch_bounds__(256) phong_recon_loss_grad_kernel(const float*
 // = dd u is reduced over the block and mapped through the light's normalisation (I - L L^T) / |l|.  At img = (0.5, 0.5, 0.5)
 // d is 0 * inf = NaN; phong_pixel's fmaxf turns it into 0 (the pixel is shaded as if unlit) and the gradient passes nothing
 // through the normal there (only the mask term reaches d_img; nothing reaches d_light).  Where |a| = 0 the mask term is 0.
-// FX: slots[b][blockIdx.x][4] as phong_recon_loss_grad_kernel's.
-template <bool FX>
+// FX: slots[b][blockIdx.x][4] as phong_recon_loss_grad_kernel's.  SP: as phong_recon_loss_grad_kernel's.
+template <bool FX, bool SP>
 __global__ void __launch_bounds__(256) phong_composite_loss_grad_kernel(const float* __restrict__ img, const float* __restrict__ target,
                                                                         const float* __restrict__ light_dir,
                                                                         const float* __restrict__ light_col, float ambient,
                                                                         float k_diffuse, int white, int with_mask,
                                                                         double* __restrict__ loss, float* __restrict__ d_img,
-                                                                        float* __restrict__ d_light, int HW, double* __restrict__ slots) {
+                                                                        float* __restrict__ d_light, int HW, double* __restrict__ slots,
+                                                                        const float* __restrict__ ambient_b, float* __restrict__ d_col,
+                                                                        float* __restrict__ d_amb, double* __restrict__ pslots) {
   __shared__ double red_loss[8];
   __shared__ float red[8][3];
   const int b = blockIdx.y;
+  if constexpr (SP) ambient = __ldg(ambient_b + b);
+  float pg[4] = {0.f, 0.f, 0.f, 0.f};                                 // SP: dL/d col (3), dL/d ambient
   const float l0 = __ldg(light_dir + 3 * b), l1 = __ldg(light_dir + 3 * b + 1), l2 = __ldg(light_dir + 3 * b + 2);
   const float col[3] = {__ldg(light_col + 3 * b), __ldg(light_col + 3 * b + 1), __ldg(light_col + 3 * b + 2)};
   const float inv_n = 2.f / (3.f * static_cast<float>(HW));          // d mean / d out, times the 2 of the square
@@ -644,10 +697,11 @@ __global__ void __launch_bounds__(256) phong_composite_loss_grad_kernel(const fl
     const float r = img[o], g = img[o + 1], bl = img[o + 2];
     float out[3];
     phong_pixel(r, g, bl, l0, l1, l2, col, ambient, k_diffuse, white, with_mask, out, &t);
-    float dndl = 0.f, dm = 0.f;
+    float dndl = 0.f, dm = 0.f, dout[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const float res = out[c] - target[o + c];
+      if constexpr (SP) dout[c] = inv_n * res;
       lsum += static_cast<double>(res) * res;
       const float dx = (t.x[c] >= 0.f && t.x[c] <= 1.f) ? inv_n * res : 0.f;      // clip(compos, 0, 1)
       if (with_mask) dm += dx * (ambient + t.diff[c] - 1.f);
@@ -678,6 +732,13 @@ __global__ void __launch_bounds__(256) phong_composite_loss_grad_kernel(const fl
     }
 #pragma unroll
     for (int i = 0; i < 3; ++i) d_img[o + i] = di[i];
+    if constexpr (SP) phong_param_backward(t.d, t.mask, t.pre, t.x, k_diffuse, with_mask, dout, pg, pg + 3);
+  }
+  if constexpr (SP) {
+    if (FX ? pslots != nullptr : (d_col != nullptr || d_amb != nullptr)) {
+      block_sum4(pg);
+      if (threadIdx.x == 0) store_param_grads<FX>(pg, b, d_col, d_amb, pslots);
+    }
   }
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
 #pragma unroll
@@ -721,16 +782,21 @@ __global__ void __launch_bounds__(256) phong_composite_loss_grad_kernel(const fl
 // reduced over the block and mapped through the forward's normalisation of the light: (I - L L^T) / |l| with the TF composite's
 // division by |l|, or times the NumPy composite's reciprocal 1 / |l|; one atomic per block and component.  One thread per pixel,
 // blockIdx.y = batch item.  FX: the block's three d_light terms go to slots[b][blockIdx.x][3] (summed by slot_sum_kernel).
-template <bool TF, bool FX>
+// SP: as phong_recon_loss_grad_kernel's.
+template <bool TF, bool FX, bool SP>
 __global__ void __launch_bounds__(256) phong_shade_backward_kernel(const float* __restrict__ normal, const float* __restrict__ albedo,
                                                                    const float* __restrict__ light_dir,
                                                                    const float* __restrict__ light_col, float ambient,
                                                                    float k_diffuse, int white, int with_mask,
                                                                    const float* __restrict__ g_compos, float* __restrict__ d_normal,
                                                                    float* __restrict__ d_albedo, float* __restrict__ d_light, int HW,
-                                                                   double* __restrict__ slots) {
+                                                                   double* __restrict__ slots, const float* __restrict__ ambient_b,
+                                                                   float* __restrict__ d_col, float* __restrict__ d_amb,
+                                                                   double* __restrict__ pslots) {
   __shared__ float red[8][3];
   const int b = blockIdx.y;
+  if constexpr (SP) ambient = __ldg(ambient_b + b);
+  float pg[4] = {0.f, 0.f, 0.f, 0.f};                                 // SP: dL/d col (3), dL/d ambient
   const float l0 = __ldg(light_dir + 3 * b), l1 = __ldg(light_dir + 3 * b + 1), l2 = __ldg(light_dir + 3 * b + 2);
   const float col[3] = {__ldg(light_col + 3 * b), __ldg(light_col + 3 * b + 1), __ldg(light_col + 3 * b + 2)};
   float L[3], lscale;                                                 // the normalised light; 1/|l| (NumPy) or |l| (TF)
@@ -759,6 +825,7 @@ __global__ void __launch_bounds__(256) phong_shade_backward_kernel(const float* 
         for (int c = 0; c < 3; ++c) ds[c] = g[c];
       }
       tf_phong_pixel_backward(n, L, t, col, ambient, k_diffuse, !white, with_mask, ds, dn, dl);
+      if constexpr (SP) phong_param_backward(t.d, t.m, t.pre, t.x, k_diffuse, with_mask, ds, pg, pg + 3);
     } else {
       PhongTerms t;
       phong_pixel(n[0], n[1], n[2], l0, l1, l2, col, ambient, k_diffuse, white, with_mask, s, &t);
@@ -770,12 +837,19 @@ __global__ void __launch_bounds__(256) phong_shade_backward_kernel(const float* 
         for (int c = 0; c < 3; ++c) ds[c] = g[c];
       }
       phong_pixel_backward(n[0], n[1], n[2], t, col, ambient, k_diffuse, white, with_mask, ds, dn, dl);
+      if constexpr (SP) phong_param_backward(t.d, t.mask, t.pre, t.x, k_diffuse, with_mask, ds, pg, pg + 3);
     }
 #pragma unroll
     for (int i = 0; i < 3; ++i) d_normal[o + i] = dn[i];
     if (albedo != nullptr && d_albedo != nullptr) {
 #pragma unroll
       for (int c = 0; c < 3; ++c) d_albedo[o + c] = g[c] * s[c];
+    }
+  }
+  if constexpr (SP) {
+    if (FX ? pslots != nullptr : (d_col != nullptr || d_amb != nullptr)) {
+      block_sum4(pg);
+      if (threadIdx.x == 0) store_param_grads<FX>(pg, b, d_col, d_amb, pslots);
     }
   }
   if (FX ? slots == nullptr : d_light == nullptr) return;             // the same in every thread: the barrier below stays whole
@@ -943,9 +1017,9 @@ extern "C" int rn_phong_recon_loss_grad(const float* albedo, const float* normal
     return -1;
   const int HW = H * W;
   const dim3 grid((HW + 255) / 256, B);
-  phong_recon_loss_grad_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  phong_recon_loss_grad_kernel<false, false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       albedo, normal, target, light_dir, light_col, ambient, k_diffuse, black_background, with_mask, loss, d_albedo, d_normal,
-      d_light_dir, HW, nullptr);
+      d_light_dir, HW, nullptr, nullptr, nullptr, nullptr, nullptr);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }
@@ -957,8 +1031,9 @@ extern "C" int rn_phong_composite_loss_grad(const float* img, const float* targe
   if (static_cast<long long>(H) * W > 0x7fffffffLL - 256 || B > 65535) return -2;
   const int HW = H * W;
   const dim3 grid((HW + 255) / 256, B);
-  phong_composite_loss_grad_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      img, target, light_dir, light_col, ambient, k_diffuse, background_white, with_mask, loss, d_img, d_light_dir, HW, nullptr);
+  phong_composite_loss_grad_kernel<false, false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      img, target, light_dir, light_col, ambient, k_diffuse, background_white, with_mask, loss, d_img, d_light_dir, HW, nullptr,
+      nullptr, nullptr, nullptr, nullptr);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }
@@ -974,13 +1049,13 @@ extern "C" int rn_phong_shade_backward(const float* normal, const float* albedo,
   const dim3 grid((HW + 255) / 256, B);
   const int white = background_white != 0, mask = with_mask != 0;
   if (composite == RN_PHONG_TF)
-    phong_shade_backward_kernel<true, false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    phong_shade_backward_kernel<true, false, false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, g_compos, d_normal, d_albedo, d_light_dir, HW,
-        nullptr);
+        nullptr, nullptr, nullptr, nullptr, nullptr);
   else
-    phong_shade_backward_kernel<false, false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    phong_shade_backward_kernel<false, false, false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, g_compos, d_normal, d_albedo, d_light_dir, HW,
-        nullptr);
+        nullptr, nullptr, nullptr, nullptr, nullptr);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
 }
@@ -1134,9 +1209,9 @@ extern "C" int rn_phong_recon_loss_grad_fixed(const float* albedo, const float* 
   if (!work || work_bytes < rn_phong_recon_loss_grad_fixed_workspace(B, H, W)) return -4;
   const int HW = H * W, nblk = (HW + 255) / 256;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  phong_recon_loss_grad_kernel<true><<<dim3(nblk, B), 256, 0, st>>>(albedo, normal, target, light_dir, light_col, ambient, k_diffuse,
-                                                                      black_background, with_mask, nullptr, d_albedo, d_normal,
-                                                                      nullptr, HW, static_cast<double*>(work));
+  phong_recon_loss_grad_kernel<true, false><<<dim3(nblk, B), 256, 0, st>>>(
+      albedo, normal, target, light_dir, light_col, ambient, k_diffuse, black_background, with_mask, nullptr, d_albedo, d_normal,
+      nullptr, HW, static_cast<double*>(work), nullptr, nullptr, nullptr, nullptr);
   RN_COUNT_LAUNCH();
   return launch_slot_sum(static_cast<double*>(work), B, nblk, 4, 1, loss, d_light_dir, nullptr, 0, st);
 }
@@ -1150,9 +1225,9 @@ extern "C" int rn_phong_composite_loss_grad_fixed(const float* img, const float*
   if (!work || work_bytes < rn_phong_composite_loss_grad_fixed_workspace(B, H, W)) return -4;
   const int HW = H * W, nblk = (HW + 255) / 256;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  phong_composite_loss_grad_kernel<true><<<dim3(nblk, B), 256, 0, st>>>(img, target, light_dir, light_col, ambient, k_diffuse,
-                                                                          background_white, with_mask, nullptr, d_img, nullptr, HW,
-                                                                          static_cast<double*>(work));
+  phong_composite_loss_grad_kernel<true, false><<<dim3(nblk, B), 256, 0, st>>>(
+      img, target, light_dir, light_col, ambient, k_diffuse, background_white, with_mask, nullptr, d_img, nullptr, HW,
+      static_cast<double*>(work), nullptr, nullptr, nullptr, nullptr);
   RN_COUNT_LAUNCH();
   return launch_slot_sum(static_cast<double*>(work), B, nblk, 4, 1, loss, d_light_dir, nullptr, 0, st);
 }
@@ -1171,12 +1246,174 @@ extern "C" int rn_phong_shade_backward_fixed(const float* normal, const float* a
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   double* slots = d_light_dir ? static_cast<double*>(work) : nullptr;
   if (composite == RN_PHONG_TF)
-    phong_shade_backward_kernel<true, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, ambient, k_diffuse, white,
-                                                                  mask, g_compos, d_normal, d_albedo, nullptr, HW, slots);
+    phong_shade_backward_kernel<true, true, false><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, ambient, k_diffuse,
+                                                                         white, mask, g_compos, d_normal, d_albedo, nullptr, HW, slots,
+                                                                         nullptr, nullptr, nullptr, nullptr);
   else
-    phong_shade_backward_kernel<false, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, ambient, k_diffuse, white,
-                                                                   mask, g_compos, d_normal, d_albedo, nullptr, HW, slots);
+    phong_shade_backward_kernel<false, true, false><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, ambient, k_diffuse,
+                                                                          white, mask, g_compos, d_normal, d_albedo, nullptr, HW,
+                                                                          slots, nullptr, nullptr, nullptr, nullptr);
   RN_COUNT_LAUNCH();
   if (d_light_dir) return launch_slot_sum(slots, B, nblk, 3, 0, nullptr, d_light_dir, nullptr, 0, st);
   return static_cast<int>(cudaGetLastError());
+}
+
+// ------------------------------------------------------------------------------------------ shading-parameter entries
+// The SP instantiations: each is its scalar-ambient entry with ambient read per item from a device array [B] and the
+// gradients of light_col [B,3] and ambient [B] (either may be NULL).  The atomic entries accumulate into them (zero them
+// first); the twins overwrite them.  Twin workspace: slots of 4 doubles per (item, 256-pixel block) for the loss and d_light_dir
+// terms, then 3 for the colour and 1 for the ambient term.
+namespace {
+long long phong_params_fixed_bytes(int B, int H, int W) {
+  if (B < 1 || H < 1 || W < 1) return -1;
+  return 8LL * B * ((static_cast<long long>(H) * W + 255) / 256) * 8;
+}
+// the colour and ambient sums of a twin (pslots = work + 4 B nblk doubles)
+int param_slot_sums(const double* pslots, int B, int nblk, float* d_col, float* d_amb, cudaStream_t st) {
+  int rc = 0;
+  if (d_col) rc = launch_slot_sum(pslots, B, nblk, 3, 0, nullptr, d_col, nullptr, 0, st);
+  if (rc == 0 && d_amb) rc = launch_slot_sum(pslots + 3LL * B * nblk, B, nblk, 1, 0, nullptr, d_amb, nullptr, 0, st);
+  return rc;
+}
+}  // namespace
+
+extern "C" int rn_phong_recon_loss_grad_params(const float* albedo, const float* normal, const float* target,
+                                               const float* light_dir, const float* light_col, const float* ambient,
+                                               float k_diffuse, int black_background, int with_mask, double* loss,
+                                               float* d_albedo, float* d_normal, float* d_light_dir, float* d_light_col,
+                                               float* d_ambient, int B, int H, int W, void* stream) {
+  if (!albedo || !normal || !target || !light_dir || !light_col || !ambient || !loss || !d_albedo || !d_normal || B < 1 || H < 1 ||
+      W < 1)
+    return -1;
+  if (static_cast<long long>(H) * W > 0x7fffffffLL - 255 || B > 65535) return -2;
+  const int HW = H * W;
+  const dim3 grid((HW + 255) / 256, B);
+  phong_recon_loss_grad_kernel<false, true><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      albedo, normal, target, light_dir, light_col, 0.f, k_diffuse, black_background, with_mask, loss, d_albedo, d_normal,
+      d_light_dir, HW, nullptr, ambient, d_light_col, d_ambient, nullptr);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int rn_phong_composite_loss_grad_params(const float* img, const float* target, const float* light_dir,
+                                                   const float* light_col, const float* ambient, float k_diffuse,
+                                                   int background_white, int with_mask, double* loss, float* d_img,
+                                                   float* d_light_dir, float* d_light_col, float* d_ambient, int B, int H, int W,
+                                                   void* stream) {
+  if (!img || !target || !light_dir || !light_col || !ambient || !loss || !d_img || B < 1 || H < 1 || W < 1) return -1;
+  if (static_cast<long long>(H) * W > 0x7fffffffLL - 256 || B > 65535) return -2;
+  const int HW = H * W;
+  const dim3 grid((HW + 255) / 256, B);
+  phong_composite_loss_grad_kernel<false, true><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      img, target, light_dir, light_col, 0.f, k_diffuse, background_white, with_mask, loss, d_img, d_light_dir, HW, nullptr,
+      ambient, d_light_col, d_ambient, nullptr);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int rn_phong_shade_backward_params(const float* normal, const float* albedo, const float* light_dir,
+                                              const float* light_col, const float* ambient, float k_diffuse, int composite,
+                                              int background_white, int with_mask, const float* g_compos, float* d_normal,
+                                              float* d_albedo, float* d_light_dir, float* d_light_col, float* d_ambient, int B,
+                                              int H, int W, void* stream) {
+  if (!normal || !light_dir || !light_col || !ambient || !g_compos || !d_normal || B < 1 || H < 1 || W < 1) return -1;
+  if (composite != RN_PHONG_NUMPY && composite != RN_PHONG_TF) return -1;
+  if (B > 65535 || static_cast<long long>(H) * W > 0x7fffffffLL - 255) return -2;
+  const int HW = H * W;
+  const dim3 grid((HW + 255) / 256, B);
+  const int white = background_white != 0, mask = with_mask != 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (composite == RN_PHONG_TF)
+    phong_shade_backward_kernel<true, false, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, 0.f, k_diffuse,
+                                                                         white, mask, g_compos, d_normal, d_albedo, d_light_dir,
+                                                                         HW, nullptr, ambient, d_light_col, d_ambient, nullptr);
+  else
+    phong_shade_backward_kernel<false, false, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, 0.f, k_diffuse,
+                                                                          white, mask, g_compos, d_normal, d_albedo, d_light_dir,
+                                                                          HW, nullptr, ambient, d_light_col, d_ambient, nullptr);
+  RN_COUNT_LAUNCH();
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" long long rn_phong_recon_loss_grad_params_fixed_workspace(int B, int H, int W) {
+  return phong_params_fixed_bytes(B, H, W);
+}
+extern "C" long long rn_phong_composite_loss_grad_params_fixed_workspace(int B, int H, int W) {
+  return phong_params_fixed_bytes(B, H, W);
+}
+extern "C" long long rn_phong_shade_backward_params_fixed_workspace(int B, int H, int W) {
+  return phong_params_fixed_bytes(B, H, W);
+}
+
+extern "C" int rn_phong_recon_loss_grad_params_fixed(const float* albedo, const float* normal, const float* target,
+                                                     const float* light_dir, const float* light_col, const float* ambient,
+                                                     float k_diffuse, int black_background, int with_mask, double* loss,
+                                                     float* d_albedo, float* d_normal, float* d_light_dir, float* d_light_col,
+                                                     float* d_ambient, int B, int H, int W, void* work, long long work_bytes,
+                                                     void* stream) {
+  if (!albedo || !normal || !target || !light_dir || !light_col || !ambient || !loss || !d_albedo || !d_normal || B < 1 || H < 1 ||
+      W < 1)
+    return -1;
+  if (static_cast<long long>(H) * W > 0x7fffffffLL - 255 || B > 65535) return -2;
+  if (!work || work_bytes < phong_params_fixed_bytes(B, H, W)) return -4;
+  const int HW = H * W, nblk = (HW + 255) / 256;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* slots = static_cast<double*>(work);
+  double* pslots = (d_light_col || d_ambient) ? slots + 4LL * B * nblk : nullptr;
+  phong_recon_loss_grad_kernel<true, true><<<dim3(nblk, B), 256, 0, st>>>(
+      albedo, normal, target, light_dir, light_col, 0.f, k_diffuse, black_background, with_mask, nullptr, d_albedo, d_normal,
+      nullptr, HW, slots, ambient, nullptr, nullptr, pslots);
+  RN_COUNT_LAUNCH();
+  int rc = launch_slot_sum(slots, B, nblk, 4, 1, loss, d_light_dir, nullptr, 0, st);
+  return rc ? rc : param_slot_sums(pslots, B, nblk, d_light_col, d_ambient, st);
+}
+
+extern "C" int rn_phong_composite_loss_grad_params_fixed(const float* img, const float* target, const float* light_dir,
+                                                         const float* light_col, const float* ambient, float k_diffuse,
+                                                         int background_white, int with_mask, double* loss, float* d_img,
+                                                         float* d_light_dir, float* d_light_col, float* d_ambient, int B, int H,
+                                                         int W, void* work, long long work_bytes, void* stream) {
+  if (!img || !target || !light_dir || !light_col || !ambient || !loss || !d_img || B < 1 || H < 1 || W < 1) return -1;
+  if (static_cast<long long>(H) * W > 0x7fffffffLL - 256 || B > 65535) return -2;
+  if (!work || work_bytes < phong_params_fixed_bytes(B, H, W)) return -4;
+  const int HW = H * W, nblk = (HW + 255) / 256;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* slots = static_cast<double*>(work);
+  double* pslots = (d_light_col || d_ambient) ? slots + 4LL * B * nblk : nullptr;
+  phong_composite_loss_grad_kernel<true, true><<<dim3(nblk, B), 256, 0, st>>>(
+      img, target, light_dir, light_col, 0.f, k_diffuse, background_white, with_mask, nullptr, d_img, nullptr, HW, slots, ambient,
+      nullptr, nullptr, pslots);
+  RN_COUNT_LAUNCH();
+  int rc = launch_slot_sum(slots, B, nblk, 4, 1, loss, d_light_dir, nullptr, 0, st);
+  return rc ? rc : param_slot_sums(pslots, B, nblk, d_light_col, d_ambient, st);
+}
+
+extern "C" int rn_phong_shade_backward_params_fixed(const float* normal, const float* albedo, const float* light_dir,
+                                                    const float* light_col, const float* ambient, float k_diffuse, int composite,
+                                                    int background_white, int with_mask, const float* g_compos, float* d_normal,
+                                                    float* d_albedo, float* d_light_dir, float* d_light_col, float* d_ambient,
+                                                    int B, int H, int W, void* work, long long work_bytes, void* stream) {
+  if (!normal || !light_dir || !light_col || !ambient || !g_compos || !d_normal || B < 1 || H < 1 || W < 1) return -1;
+  if (composite != RN_PHONG_NUMPY && composite != RN_PHONG_TF) return -1;
+  if (B > 65535 || static_cast<long long>(H) * W > 0x7fffffffLL - 255) return -2;
+  const bool any = d_light_dir || d_light_col || d_ambient;
+  if (any && (!work || work_bytes < phong_params_fixed_bytes(B, H, W))) return -4;
+  const int HW = H * W, nblk = (HW + 255) / 256;
+  const dim3 grid(nblk, B);
+  const int white = background_white != 0, mask = with_mask != 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* slots = d_light_dir ? static_cast<double*>(work) : nullptr;
+  double* pslots = (d_light_col || d_ambient) ? static_cast<double*>(work) + 4LL * B * nblk : nullptr;
+  if (composite == RN_PHONG_TF)
+    phong_shade_backward_kernel<true, true, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, 0.f, k_diffuse, white,
+                                                                        mask, g_compos, d_normal, d_albedo, nullptr, HW, slots,
+                                                                        ambient, nullptr, nullptr, pslots);
+  else
+    phong_shade_backward_kernel<false, true, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, 0.f, k_diffuse,
+                                                                         white, mask, g_compos, d_normal, d_albedo, nullptr, HW,
+                                                                         slots, ambient, nullptr, nullptr, pslots);
+  RN_COUNT_LAUNCH();
+  int rc = d_light_dir ? launch_slot_sum(slots, B, nblk, 3, 0, nullptr, d_light_dir, nullptr, 0, st) : 0;
+  rc = rc ? rc : param_slot_sums(pslots, B, nblk, d_light_col, d_ambient, st);
+  return rc ? rc : static_cast<int>(cudaGetLastError());
 }

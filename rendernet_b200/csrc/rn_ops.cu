@@ -997,15 +997,17 @@ __global__ void binvox_decode_kernel(const uint8_t* __restrict__ pairs, const in
 // The one Phong pass (rn_phong_shade; rn_phong_composite is its NumPy-composite, no-albedo case).  One thread per pixel,
 // blockIdx.y = batch item.  shade = phong_pixel (TF = false) or tf_phong_pixel (TF = true); compos = albedo * shade, or shade
 // itself without an albedo; each of shade_f32, compos_f32 and compos_u8 (= clip(255 compos) truncated) may be NULL.
-template <bool TF>
+// PA (rn_phong_shade_ambient): the item's ambient term is loaded from ambient_b[b] instead of passed; the arithmetic is the same.
+template <bool TF, bool PA>
 __global__ void __launch_bounds__(256) phong_shade_kernel(const float* __restrict__ normal, const float* __restrict__ albedo,
                                                           const float* __restrict__ light_dir, const float* __restrict__ light_col,
                                                           float ambient, float k_diffuse, int white, int with_mask,
                                                           float* __restrict__ shade_f32, float* __restrict__ compos_f32,
-                                                          uint8_t* __restrict__ compos_u8, int HW) {
+                                                          uint8_t* __restrict__ compos_u8, int HW, const float* __restrict__ ambient_b) {
   const int b = blockIdx.y;
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= HW) return;
+  if constexpr (PA) ambient = __ldg(ambient_b + b);
   const size_t o = (static_cast<size_t>(b) * HW + p) * 3;
   const float l0 = __ldg(light_dir + 3 * b), l1 = __ldg(light_dir + 3 * b + 1), l2 = __ldg(light_dir + 3 * b + 2);
   const float col[3] = {__ldg(light_col + 3 * b), __ldg(light_col + 3 * b + 1), __ldg(light_col + 3 * b + 2)};
@@ -1706,21 +1708,45 @@ extern "C" int rn_phong_composite(const float* img, const float* light_dir, cons
                         nullptr, out_f32, out_u8, B, H, W, stream);
 }
 
-extern "C" int rn_phong_shade(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
-                              float ambient, float k_diffuse, int composite, int background_white, int with_mask, float* shade_f32,
-                              float* compos_f32, uint8_t* compos_u8, int B, int H, int W, void* stream) {
+namespace {
+int phong_shade_launch(const float* normal, const float* albedo, const float* light_dir, const float* light_col, float ambient,
+                       const float* ambient_b, float k_diffuse, int composite, int background_white, int with_mask,
+                       float* shade_f32, float* compos_f32, uint8_t* compos_u8, int B, int H, int W, void* stream) {
   if (!normal || !light_dir || !light_col || (!shade_f32 && !compos_f32 && !compos_u8) || B < 1 || H < 1 || W < 1) return -1;
   if (composite != RN_PHONG_NUMPY && composite != RN_PHONG_TF) return -1;
   if (B > 65535 || static_cast<long long>(H) * W > 0x7fffffffLL - 255) return -2;
   const int HW = H * W;
   const dim3 grid((HW + 255) / 256, B);
   const int white = background_white != 0, mask = with_mask != 0;
-  if (composite == RN_PHONG_TF)
-    phong_shade_kernel<true><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, shade_f32, compos_f32, compos_u8, HW);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (composite == RN_PHONG_TF && ambient_b)
+    phong_shade_kernel<true, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, 0.f, k_diffuse, white, mask,
+                                                         shade_f32, compos_f32, compos_u8, HW, ambient_b);
+  else if (composite == RN_PHONG_TF)
+    phong_shade_kernel<true, false><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask,
+                                                          shade_f32, compos_f32, compos_u8, HW, nullptr);
+  else if (ambient_b)
+    phong_shade_kernel<false, true><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, 0.f, k_diffuse, white, mask,
+                                                          shade_f32, compos_f32, compos_u8, HW, ambient_b);
   else
-    phong_shade_kernel<false><<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask, shade_f32, compos_f32, compos_u8, HW);
+    phong_shade_kernel<false, false><<<grid, 256, 0, st>>>(normal, albedo, light_dir, light_col, ambient, k_diffuse, white, mask,
+                                                           shade_f32, compos_f32, compos_u8, HW, nullptr);
   RN_COUNT_LAUNCH();
   return static_cast<int>(cudaGetLastError());
+}
+}  // namespace
+
+extern "C" int rn_phong_shade(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
+                              float ambient, float k_diffuse, int composite, int background_white, int with_mask, float* shade_f32,
+                              float* compos_f32, uint8_t* compos_u8, int B, int H, int W, void* stream) {
+  return phong_shade_launch(normal, albedo, light_dir, light_col, ambient, nullptr, k_diffuse, composite, background_white,
+                            with_mask, shade_f32, compos_f32, compos_u8, B, H, W, stream);
+}
+
+extern "C" int rn_phong_shade_ambient(const float* normal, const float* albedo, const float* light_dir, const float* light_col,
+                                      const float* ambient, float k_diffuse, int composite, int background_white, int with_mask,
+                                      float* shade_f32, float* compos_f32, uint8_t* compos_u8, int B, int H, int W, void* stream) {
+  if (!ambient) return -1;
+  return phong_shade_launch(normal, albedo, light_dir, light_col, 0.f, ambient, k_diffuse, composite, background_white,
+                            with_mask, shade_f32, compos_f32, compos_u8, B, H, W, stream);
 }

@@ -187,4 +187,23 @@ __device__ __forceinline__ void tf_phong_pixel_backward(const float* n, const fl
   }
 }
 
+// Gradients of the shading parameters for one pixel of either composite, from the terms its forward recorded (PhongTerms:
+// d, mask; TfPhongTerms: d, m; both: pre, x).  Both composites form x_c = m (ambient + clip(pre_c)) + (1 - m) (x_c = ambient +
+// clip(pre_c) without a mask) with pre_c = fl(k_d max(d, 0)) col_c, so with dx_c = ds_c where 0 <= x_c <= 1 and dpre_c = m dx_c
+// where 0 <= pre_c <= 1:  dL/d ambient += sum_c m dx_c,  dL/d col_c += dpre_c fl(k_d max(d, 0)).  At a NaN d (n = (0.5, 0.5, 0.5))
+// max(d, 0) is 0 and the colour gets nothing.  A helper of its own, so phong_pixel_backward / tf_phong_pixel_backward and the
+// kernels that inline them are untouched; dcol[3] and *damb are accumulated into.
+__device__ __forceinline__ void phong_param_backward(float d, float m, const float* pre, const float* x, float k_diffuse,
+                                                     int with_mask, const float* ds, float* dcol, float* damb) {
+  const float kd = k_diffuse * fmaxf(d, 0.f);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float dx = (x[c] >= 0.f && x[c] <= 1.f) ? ds[c] : 0.f;                   // clip(compos, 0, 1)
+    const float ddiff = with_mask ? dx * m : dx;
+    *damb += ddiff;
+    const float dpre = (pre[c] >= 0.f && pre[c] <= 1.f) ? ddiff : 0.f;             // clip(diffuse, 0, 1)
+    dcol[c] += dpre * kd;
+  }
+}
+
 }  // namespace rn

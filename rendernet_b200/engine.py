@@ -66,6 +66,15 @@ class _EngineBase:
         """User arguments -> CPU tensors shaped like `self.inputs` (poses become 3x4 matrices here)."""
         raise NotImplementedError
 
+    @staticmethod
+    def _light_rows(t, B, what) -> torch.Tensor:
+        t = torch.as_tensor(np.asarray(t.cpu() if isinstance(t, torch.Tensor) else t, np.float32))
+        if t.dim() == 1 and t.numel() == 3:
+            t = t.reshape(1, 3)
+        if t.dim() != 2 or t.shape[1] != 3 or t.shape[0] not in (1, B):
+            raise ValueError(f"{what} must have shape [1,3] or [{B},3], not {tuple(t.shape)}")
+        return t.expand(B, 3).contiguous()
+
     # ---- construction ------------------------------------------------------------------------------
     def _run_forward(self):
         with torch.cuda.device(self.device), tf.use_store(self.store):
@@ -200,9 +209,11 @@ class RenderEngine(_EngineBase):
                  seed: int = 0, device: str = "cuda", precision: str = "fast", strict: bool = True,
                  fuse_phong: bool = True):
         """weights: {tf variable name: array} (None -> the reference's initialisers, seeded).
-        phong: None, or dict(light_dir[1|B,3], light_col, ambient, k_diffuse) to apply the demo's
+        phong: None, or dict(light_dir[1|B,3], light_col[1|B,3], ambient, k_diffuse) to apply the demo's
         Phong composite + uint8 quantisation; fuse_phong: inside the output layer's epilogue (default) or as a separate pass.
-        precision: "fast" | "exact" (module docstring)."""
+        The light direction and colour are device inputs like the voxels: `upload`, `submit` and `render` take light_dir= and
+        light_col= ([1|B,3]; None keeps the last one given, initially phong's), so relighting needs no re-capture.  ambient and
+        k_diffuse are fixed here.  precision: "fast" | "exact" (module docstring)."""
         super().__init__(weights, precision, seed, device, use_graph, strict)
         self.B, self.size, self.new_size = batch, size, new_size
         self.is_greyscale = is_greyscale
@@ -213,12 +224,15 @@ class RenderEngine(_EngineBase):
         self.phong = phong
         self.fuse_phong = fuse_phong
         if phong is not None:
-            self.light_dir = torch.as_tensor(np.asarray(phong["light_dir"], np.float32)).reshape(-1, 3).to(dev)
-            self.light_col = torch.as_tensor(np.asarray(phong["light_col"], np.float32)).reshape(-1, 3).to(dev)
+            # the graph reads these buffers (the fused epilogue through their pointers): a step's light is uploaded into them
+            self._light_host = [self._light_rows(np.asarray(phong["light_dir"], np.float32).reshape(-1, 3), batch, "light_dir"),
+                                self._light_rows(np.asarray(phong["light_col"], np.float32).reshape(-1, 3), batch, "light_col")]
+            self.light_dir, self.light_col = (t.to(dev) for t in self._light_host)
+            self.inputs += [self.light_dir, self.light_col]
         self.out = None
         self.out_u8 = None
         self._finish_init()
-        self.vox_host, self.minv_host = self.inputs_host
+        self.vox_host, self.minv_host = self.inputs_host[:2]
         self.out_host = self.outputs_host[0]
         self.out_u8_host = self.outputs_host[1] if phong is not None else None
 
@@ -251,9 +265,17 @@ class RenderEngine(_EngineBase):
 
     pose_to_matrix = staticmethod(pose_to_matrix)
 
-    def _host_inputs(self, voxels, view_params):
+    def _host_inputs(self, voxels, view_params, light_dir=None, light_col=None):
         v = voxels if isinstance(voxels, torch.Tensor) else torch.as_tensor(np.asarray(voxels, np.float32))
-        return [v, torch.from_numpy(pose_to_matrix(view_params, self.size, self.new_size))]
+        got = [v, torch.from_numpy(pose_to_matrix(view_params, self.size, self.new_size))]
+        if self.phong is None:
+            if light_dir is not None or light_col is not None:
+                raise ValueError("light_dir / light_col need an engine built with phong=")
+            return got
+        for i, (t, what) in enumerate(((light_dir, "light_dir"), (light_col, "light_col"))):
+            if t is not None:
+                self._light_host[i] = self._light_rows(t, self.B, what)
+        return got + list(self._light_host)
 
     def _pipe_outputs(self):
         return [0] if self.phong is None else [1]            # the float image, or the uint8 Phong image
@@ -262,23 +284,24 @@ class RenderEngine(_EngineBase):
         super().step_device()
         return self.out
 
-    def upload(self, voxels, view_params, non_blocking=True):
-        self._upload(self._host_inputs(voxels, view_params))
+    def upload(self, voxels, view_params, non_blocking=True, light_dir=None, light_col=None):
+        self._upload(self._host_inputs(voxels, view_params, light_dir, light_col))
 
-    def submit(self, voxels, view_params) -> int:
+    def submit(self, voxels, view_params, light_dir=None, light_col=None) -> int:
         """Asynchronously enqueue one step: pinned-host staging -> H2D (copy stream) -> graph replay (compute
         stream) -> D2H (copy stream).  Uploads of step i+1 and downloads of step i-1 overlap the compute of step i.
+        light_dir / light_col (phong engines): this step's light, [1|B,3] (None: the last one given).
         Returns a ticket for `result()`."""
-        return self._submit(self._host_inputs(voxels, view_params))
+        return self._submit(self._host_inputs(voxels, view_params, light_dir, light_col))
 
     def result(self, ticket: int) -> torch.Tensor:
         """Block until the step `ticket` (one of the last two submitted) has landed in pinned host memory."""
         return self._result(ticket)[0]
 
-    def render(self, voxels, view_params, to_host: bool = True):
+    def render(self, voxels, view_params, to_host: bool = True, light_dir=None, light_col=None):
         """voxels [B,64,64,64,1] float32 (host), view_params [B,3] -> image [B,512,512,3|1] float32
-        (and uint8 Phong image when configured).  Includes H2D and D2H."""
-        self.upload(voxels, view_params)
+        (and uint8 Phong image when configured; light_dir / light_col as in `submit`).  Includes H2D and D2H."""
+        self.upload(voxels, view_params, light_dir=light_dir, light_col=light_col)
         self.step_device()
         if not to_host:
             return self.out if self.phong is None else (self.out, self.out_u8)
@@ -340,15 +363,6 @@ class TextureRenderEngine(_EngineBase):
         self._finish_init()
         self.vox_host, self.tex_host, self.minv_host = self.inputs_host[:3]
         self.out_host = tuple(self.outputs_host)
-
-    @staticmethod
-    def _light_rows(t, B, what) -> torch.Tensor:
-        t = torch.as_tensor(np.asarray(t.cpu() if isinstance(t, torch.Tensor) else t, np.float32))
-        if t.dim() == 1 and t.numel() == 3:
-            t = t.reshape(1, 3)
-        if t.dim() != 2 or t.shape[1] != 3 or t.shape[0] not in (1, B):
-            raise ValueError(f"{what} must have shape [1,3] or [{B},3], not {tuple(t.shape)}")
-        return t.expand(B, 3).contiguous()
 
     def _forward(self):
         from .RenderNet_Texture_Face_Normal import RenderNet as RenderNetTexture, decoder_texture

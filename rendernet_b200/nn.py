@@ -458,31 +458,49 @@ class ShapeDecoder(_Renderer):
 # ----------------------------------------------------------------------------------------------- Phong composite
 class _PhongFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, normal, light_dir, albedo, opts):
-        _, compos, _ = ops.phong_shade(normal, light_dir, albedo=albedo, want_shade=False, want_compos=True, want_u8=False, **opts)
+    def forward(ctx, normal, light_dir, albedo, light_col, ambient, opts):
+        _, compos, _ = ops.phong_shade(normal, light_dir, albedo=albedo, light_col=light_col, ambient=ambient, want_shade=False,
+                                       want_compos=True, want_u8=False, **opts)
         ctx.opts = opts
-        ctx.save_for_backward(normal, light_dir, albedo)
+        ctx.consts = (None if isinstance(light_col, torch.Tensor) else light_col,
+                      None if isinstance(ambient, torch.Tensor) else ambient)
+        ctx.save_for_backward(normal, light_dir, albedo, *(t for t in (light_col, ambient) if isinstance(t, torch.Tensor)))
         return compos
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        normal, light_dir, albedo = ctx.saved_tensors
+        normal, light_dir, albedo, *rest = ctx.saved_tensors
+        light_col, ambient = ctx.consts
+        if light_col is None:
+            light_col = rest.pop(0)
+        if ambient is None:
+            ambient = rest.pop(0)
         need = ctx.needs_input_grad
-        d_normal, d_albedo, d_light = ops.phong_shade_backward(normal, g, light_dir, albedo=albedo, want_light_grad=need[1],
-                                                               **ctx.opts)
+        shading = need[3] or need[4]
+        out = ops.phong_shade_backward(normal, g, light_dir, albedo=albedo, light_col=light_col, ambient=ambient,
+                                       want_light_grad=need[1], want_shading_grad=shading, **ctx.opts)
+        d_normal, d_albedo, d_light = out[:3]
+
+        def per_input(d, t):          # a [1,...] row (or a 0-d ambient) gets the gradient summed over the batch
+            d = d.sum(0, keepdim=True) if t.shape[:1] != d.shape[:1] else d
+            return d.reshape(t.shape).to(device=t.device, dtype=t.dtype)
+        d_col = per_input(out[3], light_col) if need[3] else None
+        d_amb = per_input(out[4], ambient) if need[4] else None
         if need[1]:
-            d_light = d_light.sum(0, keepdim=True) if light_dir.shape[0] == 1 else d_light
-            d_light = d_light.to(device=light_dir.device, dtype=light_dir.dtype)
-        return (d_normal if need[0] else None), (d_light if need[1] else None), (d_albedo if need[2] else None), None
+            d_light = per_input(d_light, light_dir)
+        return (d_normal if need[0] else None), (d_light if need[1] else None), (d_albedo if need[2] else None), d_col, d_amb, None
 
 
 def phong_shade(normal, light_dir, albedo=None, composite: str = "tf", light_col=(1.0, 1.0, 1.0), ambient: float = 0.0,
                 k_diffuse: float = 1.0, background_white: bool = True, with_mask: bool = True):
     """Differentiable Phong composite: compos = albedo * shade (albedo None: shade) of a normal map [B,H,W,3] fp32 CUDA tensor;
-    the forward is ops.phong_shade's image bit for bit, the backward rn_phong_shade_backward.  composite "tf" (face
-    reconstruction) or "numpy" (the demo's).  light_dir: a [1,3] (its gradient summed over the batch) or [B,3] tensor; light_col,
-    ambient and k_diffuse are constants.  Gradients reach normal, albedo and light_dir."""
+    the forward is ops.phong_shade's image bit for bit, the backward rn_phong_shade_backward (rn_phong_shade_backward_params when
+    the light colour or the ambient term needs a gradient).  composite "tf" (face reconstruction) or "numpy" (the demo's).
+    light_dir: a [1,3] (its gradient summed over the batch) or [B,3] tensor.  light_col: a [1|B,3] floating-point tensor (or a
+    constant triple), ambient: a float or a [1|B] (or 0-d) floating-point tensor; either tensor may require grad, and a single
+    row gets its gradient summed over the batch.  k_diffuse is a constant: the composites see only k_diffuse * light_col, so its
+    gradient would duplicate the colour's.  Gradients reach normal, albedo, light_dir, light_col and ambient."""
     if len(getattr(normal, "shape", ())) != 4 or normal.shape[3] != 3:
         raise ValueError(f"phong_shade: normal map must be [B,H,W,3], not {tuple(getattr(normal, 'shape', ()))}")
     B = int(normal.shape[0])
@@ -490,6 +508,20 @@ def phong_shade(normal, light_dir, albedo=None, composite: str = "tf", light_col
         light_dir = torch.as_tensor(np.asarray(light_dir, np.float32))
     if light_dir.dim() != 2 or light_dir.shape[1] != 3 or light_dir.shape[0] not in (1, B):
         raise ValueError(f"phong_shade: light_dir must be [1,3] or [{B},3], not {tuple(light_dir.shape)}")
+    if isinstance(light_col, torch.Tensor):
+        if light_col.dim() != 2 or light_col.shape[1] != 3 or light_col.shape[0] not in (1, B):
+            raise ValueError(f"phong_shade: light_col must be [1,3] or [{B},3], not {tuple(light_col.shape)}")
+    if isinstance(ambient, torch.Tensor):
+        if ambient.dim() > 1 or ambient.numel() not in (1, B):
+            raise ValueError(f"phong_shade: ambient must be a float or [1] or [{B}], not {tuple(ambient.shape)}")
+    else:
+        ambient = float(ambient)
+    for name, t in (("light_col", light_col), ("ambient", ambient)):
+        if isinstance(t, torch.Tensor):
+            if not t.dtype.is_floating_point:
+                raise TypeError(f"phong_shade: {name} must be a floating-point tensor, not {t.dtype}")
+            if t.is_cuda and t.device != normal.device:
+                raise ValueError(f"phong_shade: {name} is on {t.device}, the normal map on {normal.device}")
     if composite not in ops.PHONG_COMPOSITES:
         raise ValueError(f"composite must be one of {sorted(ops.PHONG_COMPOSITES)}, not {composite!r}")
     for name, t in (("normal", normal), ("albedo", albedo)):
@@ -497,6 +529,6 @@ def phong_shade(normal, light_dir, albedo=None, composite: str = "tf", light_col
             raise TypeError(f"phong_shade: {name} must be a float32 CUDA tensor")
     if albedo is not None and tuple(albedo.shape) != tuple(normal.shape):
         raise ValueError(f"phong_shade: albedo {tuple(albedo.shape)} and normal map {tuple(normal.shape)} differ in shape")
-    opts = dict(light_col=light_col, ambient=float(ambient), k_diffuse=float(k_diffuse), composite=composite,
-                background_white=bool(background_white), with_mask=bool(with_mask))
-    return _PhongFn.apply(normal, light_dir, albedo, opts)
+    opts = dict(k_diffuse=float(k_diffuse), composite=composite, background_white=bool(background_white),
+                with_mask=bool(with_mask))
+    return _PhongFn.apply(normal, light_dir, albedo, light_col, ambient, opts)

@@ -916,14 +916,34 @@ def _light_rows(t, B: int, device, what: str) -> torch.Tensor:
     return (t.expand(B, 3) if t.shape[0] != B else t).contiguous()
 
 
+def _ambient_rows(ambient, B: int, device) -> Optional[torch.Tensor]:
+    """Ambient term: a float (None: the scalar entries) or a [1|B] tensor -> contiguous fp32 [B] on `device` (the per-item
+    entries).  A [B] fp32 CUDA tensor on `device` is used as it is."""
+    if not isinstance(ambient, torch.Tensor):
+        return None
+    if ambient.dim() > 1 or ambient.numel() not in (1, B):
+        raise ValueError(f"ambient must be a float or have shape [1] or [{B}], not {tuple(ambient.shape)}")
+    if not ambient.dtype.is_floating_point:
+        raise TypeError(f"ambient must be a floating-point tensor, not {ambient.dtype}")
+    a = ambient.reshape(-1).to(device=device, dtype=torch.float32)
+    return (a.expand(B) if a.numel() != B else a).contiguous()
+
+
+def _ambient_array(ambient, B: int, device) -> torch.Tensor:
+    """The [B] fp32 ambient array of the *_params entries, also for a float."""
+    a = _ambient_rows(ambient, B, device)
+    return a if a is not None else torch.full((B,), float(ambient), device=device, dtype=torch.float32)
+
+
 def phong_shade(normal: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambient: float = 0.0, k_diffuse: float = 1.0,
                 albedo: Optional[torch.Tensor] = None, composite: str = "tf", background_white: bool = True,
                 with_mask: bool = True, want_shade: bool = True, want_compos: bool = True, want_u8: bool = True):
     """Shaded image (rn_phong_shade): shade = Phong composite of the normal map, compos = albedo * shade.
     normal, albedo: fp32 [B,H,W,3] CUDA tensors (albedo None: compos is shade).  light_dir, light_col: 1 or B rows of 3.
     composite "tf": TensorFlow's tf_phong_composite, the image the reconstruction loss measures (rn_phong_recon_loss_grad);
-    "numpy": the demo's np_phong_composite (rn_phong_composite).  Returns (shade fp32, compos fp32, compos uint8 = clip(255 x)),
-    each None unless asked for; without an albedo, compos is the shade tensor itself."""
+    "numpy": the demo's np_phong_composite (rn_phong_composite).  ambient: a float, or a [1|B] tensor of per-item terms
+    (rn_phong_shade_ambient: the same bits as the float for a uniform array).  Returns (shade fp32, compos fp32, compos uint8 =
+    clip(255 x)), each None unless asked for; without an albedo, compos is the shade tensor itself."""
     if composite not in PHONG_COMPOSITES:
         raise ValueError(f"composite must be one of {sorted(PHONG_COMPOSITES)}, not {composite!r}")
     if len(normal.shape) != 4 or normal.shape[3] != 3:
@@ -933,6 +953,7 @@ def phong_shade(normal: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambi
         raise ValueError(f"phong_shade: albedo {tuple(albedo.shape)} and normal map {tuple(normal.shape)} differ in shape")
     ld = _light_rows(light_dir, B, normal.device, "light_dir")
     lc = _light_rows(light_col, B, normal.device, "light_col")
+    amb = _ambient_rows(ambient, B, normal.device)
     normal = _cuda(normal, torch.float32)
     albedo = None if albedo is None else _cuda(albedo, torch.float32)
     alias = albedo is None and want_compos
@@ -943,6 +964,12 @@ def phong_shade(normal: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambi
     shade = torch.empty_like(normal) if want_shade else None
     compos = torch.empty_like(normal) if want_compos else None
     u8 = torch.empty(normal.shape, device=normal.device, dtype=torch.uint8) if want_u8 else None
+    if amb is not None:
+        check(lib.rn_phong_shade_ambient(normal.data_ptr(), _ptr(albedo), ld.data_ptr(), lc.data_ptr(), amb.data_ptr(),
+                                         float(k_diffuse), PHONG_COMPOSITES[composite], 1 if background_white else 0,
+                                         1 if with_mask else 0, _ptr(shade), _ptr(compos), _ptr(u8), B, H, W, _stream()),
+              "rn_phong_shade_ambient")
+        return shade, (shade if alias else compos), u8
     check(lib.rn_phong_shade(normal.data_ptr(), _ptr(albedo), ld.data_ptr(), lc.data_ptr(), float(ambient), float(k_diffuse),
                              PHONG_COMPOSITES[composite], 1 if background_white else 0, 1 if with_mask else 0, _ptr(shade),
                              _ptr(compos), _ptr(u8), B, H, W, _stream()), "rn_phong_shade")
@@ -951,10 +978,12 @@ def phong_shade(normal: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambi
 
 def phong_shade_backward(normal: torch.Tensor, g_compos: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambient: float = 0.0,
                          k_diffuse: float = 1.0, albedo: Optional[torch.Tensor] = None, composite: str = "tf",
-                         background_white: bool = True, with_mask: bool = True, want_light_grad: bool = True):
+                         background_white: bool = True, with_mask: bool = True, want_light_grad: bool = True,
+                         want_shading_grad: bool = False):
     """Vector-Jacobian product of phong_shade's compos (rn_phong_shade_backward) for g_compos = dL/d(compos): the arguments
     are phong_shade's.  normal, albedo (or None), g_compos: fp32 [B,H,W,3] CUDA tensors; light_dir, light_col: 1 or B rows of
-    3.  Returns (d_normal, d_albedo or None without an albedo, d_light_dir [B,3] per item or None)."""
+    3; ambient a float or a [1|B] tensor.  Returns (d_normal, d_albedo or None without an albedo, d_light_dir [B,3] per item or
+    None), and with want_shading_grad also (d_light_col [B,3], d_ambient [B]) per item (rn_phong_shade_backward_params)."""
     if composite not in PHONG_COMPOSITES:
         raise ValueError(f"composite must be one of {sorted(PHONG_COMPOSITES)}, not {composite!r}")
     if len(normal.shape) != 4 or normal.shape[3] != 3:
@@ -965,10 +994,28 @@ def phong_shade_backward(normal: torch.Tensor, g_compos: torch.Tensor, light_dir
             raise ValueError(f"phong_shade_backward: {name} {tuple(t.shape)} and normal map {tuple(normal.shape)} differ in shape")
     ld = _light_rows(light_dir, B, normal.device, "light_dir")
     lc = _light_rows(light_col, B, normal.device, "light_col")
+    amb = _ambient_rows(ambient, B, normal.device)
     normal, g_compos = _cuda(normal, torch.float32), _cuda(g_compos, torch.float32)
     albedo = None if albedo is None else _cuda(albedo, torch.float32)
     d_normal = torch.empty_like(normal)
     d_albedo = None if albedo is None else torch.empty_like(normal)
+    if want_shading_grad or amb is not None:
+        amb = amb if amb is not None else _ambient_array(ambient, B, normal.device)
+        fixed = _fixed_order()
+        new = torch.empty if fixed else torch.zeros
+        d_light = new((B, 3), device=normal.device, dtype=torch.float32) if want_light_grad else None
+        d_col = new((B, 3), device=normal.device, dtype=torch.float32) if want_shading_grad else None
+        d_amb = new((B,), device=normal.device, dtype=torch.float32) if want_shading_grad else None
+        args = (normal.data_ptr(), _ptr(albedo), ld.data_ptr(), lc.data_ptr(), amb.data_ptr(), float(k_diffuse),
+                PHONG_COMPOSITES[composite], 1 if background_white else 0, 1 if with_mask else 0, g_compos.data_ptr(),
+                d_normal.data_ptr(), _ptr(d_albedo), _ptr(d_light), _ptr(d_col), _ptr(d_amb), B, H, W)
+        if fixed:
+            work = _workspace(lib.rn_phong_shade_backward_params_fixed_workspace(B, H, W), normal.device)
+            check(lib.rn_phong_shade_backward_params_fixed(*args, work.data_ptr(), work.numel(), _stream()),
+                  "rn_phong_shade_backward_params_fixed")
+        else:
+            check(lib.rn_phong_shade_backward_params(*args, _stream()), "rn_phong_shade_backward_params")
+        return (d_normal, d_albedo, d_light) + ((d_col, d_amb) if want_shading_grad else ())
     if _fixed_order():
         d_light = torch.empty((B, 3), device=normal.device, dtype=torch.float32) if want_light_grad else None
         work = _workspace(lib.rn_phong_shade_backward_fixed_workspace(B, H, W), normal.device) if want_light_grad else None
@@ -1313,10 +1360,11 @@ def fully_connected_backward_data(g: torch.Tensor, w: torch.Tensor) -> torch.Ten
 
 def phong_recon_loss_grad(albedo: torch.Tensor, normal: torch.Tensor, target: torch.Tensor, light_dir: torch.Tensor,
                           light_col: torch.Tensor, ambient: float = 0.0, k_diffuse: float = 1.0, black_background: bool = False,
-                          with_mask: bool = True):
+                          with_mask: bool = True, want_shading_grad: bool = False):
     """Face reconstruction objective (rn_phong_recon_loss_grad): loss[b] = mean (target - albedo * tf_phong_composite(normal,
-    light_dir, light_col, ...))^2 and its gradients.  albedo, normal, target fp32 [B,H,W,3]; light_dir, light_col [B,3] (or [1,3]).
-    Returns (loss fp64 [B], d_albedo, d_normal fp32 [B,H,W,3], d_light_dir fp32 [B,3])."""
+    light_dir, light_col, ...))^2 and its gradients.  albedo, normal, target fp32 [B,H,W,3]; light_dir, light_col [B,3] (or [1,3]);
+    ambient a float or a [1|B] tensor.  Returns (loss fp64 [B], d_albedo, d_normal fp32 [B,H,W,3], d_light_dir fp32 [B,3]), and
+    with want_shading_grad also (d_light_col [B,3], d_ambient [B]) (rn_phong_recon_loss_grad_params)."""
     albedo, normal, target = (_cuda(t, torch.float32) for t in (albedo, normal, target))
     B, H, W, C3 = albedo.shape
     if C3 != 3 or tuple(normal.shape) != tuple(albedo.shape) or tuple(target.shape) != tuple(albedo.shape):
@@ -1324,6 +1372,25 @@ def phong_recon_loss_grad(albedo: torch.Tensor, normal: torch.Tensor, target: to
     ld, lc = (_cuda(t.to(device=albedo.device, dtype=torch.float32).reshape(-1, 3).expand(B, 3).contiguous(), torch.float32)
               for t in (light_dir, light_col))
     d_albedo, d_normal = torch.empty_like(albedo), torch.empty_like(albedo)
+    amb = _ambient_rows(ambient, B, albedo.device)
+    if want_shading_grad or amb is not None:
+        amb = amb if amb is not None else _ambient_array(ambient, B, albedo.device)
+        fixed = _fixed_order()
+        new = torch.empty if fixed else torch.zeros
+        loss = new(B, device=albedo.device, dtype=torch.float64)
+        d_light = new((B, 3), device=albedo.device, dtype=torch.float32)
+        d_col = new((B, 3), device=albedo.device, dtype=torch.float32) if want_shading_grad else None
+        d_amb = new((B,), device=albedo.device, dtype=torch.float32) if want_shading_grad else None
+        args = (albedo.data_ptr(), normal.data_ptr(), target.data_ptr(), ld.data_ptr(), lc.data_ptr(), amb.data_ptr(),
+                float(k_diffuse), 1 if black_background else 0, 1 if with_mask else 0, loss.data_ptr(), d_albedo.data_ptr(),
+                d_normal.data_ptr(), d_light.data_ptr(), _ptr(d_col), _ptr(d_amb), B, H, W)
+        if fixed:
+            work = _workspace(lib.rn_phong_recon_loss_grad_params_fixed_workspace(B, H, W), albedo.device)
+            check(lib.rn_phong_recon_loss_grad_params_fixed(*args, work.data_ptr(), work.numel(), _stream()),
+                  "rn_phong_recon_loss_grad_params_fixed")
+        else:
+            check(lib.rn_phong_recon_loss_grad_params(*args, _stream()), "rn_phong_recon_loss_grad_params")
+        return (loss, d_albedo, d_normal, d_light) + ((d_col, d_amb) if want_shading_grad else ())
     if _fixed_order():
         loss = torch.empty(B, device=albedo.device, dtype=torch.float64)
         d_light = torch.empty((B, 3), device=albedo.device, dtype=torch.float32)
@@ -1345,12 +1412,13 @@ def phong_recon_loss_grad(albedo: torch.Tensor, normal: torch.Tensor, target: to
 
 def phong_composite_loss_grad(img: torch.Tensor, target: torch.Tensor, light_dir, light_col=(1.0, 1.0, 1.0), ambient: float = 0.1,
                               k_diffuse: float = 0.9, background_white: bool = False, with_mask: bool = True,
-                              want_light_grad: bool = True):
+                              want_light_grad: bool = True, want_shading_grad: bool = False):
     """The Shader fit's objective over the demo's composite (rn_phong_composite_loss_grad): loss[b] = mean (target -
     np_phong_composite(img, light_dir, light_col, ambient, k_diffuse, background, with_mask))^2, the shading being
     rn_phong_composite's bit for bit.  img, target fp32 [B,H,W,3] CUDA tensors; light_dir, light_col: 1 or B rows of 3 (the
-    direction need not be unit).  Defaults are the demo's (RenderNet_demo.py:18-20, black background, mask).  Returns
-    (loss fp64 [B], d_img fp32 [B,H,W,3], d_light_dir fp32 [B,3] or None)."""
+    direction need not be unit); ambient a float or a [1|B] tensor.  Defaults are the demo's (RenderNet_demo.py:18-20, black
+    background, mask).  Returns (loss fp64 [B], d_img fp32 [B,H,W,3], d_light_dir fp32 [B,3] or None), and with
+    want_shading_grad also (d_light_col [B,3], d_ambient [B]) (rn_phong_composite_loss_grad_params)."""
     if len(img.shape) != 4 or img.shape[3] != 3:
         raise ValueError(f"phong_composite_loss_grad: img must be [B,H,W,3], not {tuple(img.shape)}")
     if tuple(target.shape) != tuple(img.shape):
@@ -1358,8 +1426,27 @@ def phong_composite_loss_grad(img: torch.Tensor, target: torch.Tensor, light_dir
     B, H, W, _ = img.shape
     ld = _light_rows(light_dir, B, img.device, "light_dir")
     lc = _light_rows(light_col, B, img.device, "light_col")
+    amb = _ambient_rows(ambient, B, img.device)
     img, target = _cuda(img, torch.float32), _cuda(target, torch.float32)
     d_img = torch.empty_like(img)
+    if want_shading_grad or amb is not None:
+        amb = amb if amb is not None else _ambient_array(ambient, B, img.device)
+        fixed = _fixed_order()
+        new = torch.empty if fixed else torch.zeros
+        loss = new(B, device=img.device, dtype=torch.float64)
+        d_light = new((B, 3), device=img.device, dtype=torch.float32) if want_light_grad else None
+        d_col = new((B, 3), device=img.device, dtype=torch.float32) if want_shading_grad else None
+        d_amb = new((B,), device=img.device, dtype=torch.float32) if want_shading_grad else None
+        args = (img.data_ptr(), target.data_ptr(), ld.data_ptr(), lc.data_ptr(), amb.data_ptr(), float(k_diffuse),
+                1 if background_white else 0, 1 if with_mask else 0, loss.data_ptr(), d_img.data_ptr(), _ptr(d_light),
+                _ptr(d_col), _ptr(d_amb), B, H, W)
+        if fixed:
+            work = _workspace(lib.rn_phong_composite_loss_grad_params_fixed_workspace(B, H, W), img.device)
+            check(lib.rn_phong_composite_loss_grad_params_fixed(*args, work.data_ptr(), work.numel(), _stream()),
+                  "rn_phong_composite_loss_grad_params_fixed")
+        else:
+            check(lib.rn_phong_composite_loss_grad_params(*args, _stream()), "rn_phong_composite_loss_grad_params")
+        return (loss, d_img, d_light) + ((d_col, d_amb) if want_shading_grad else ())
     if _fixed_order():
         loss = torch.empty(B, device=img.device, dtype=torch.float64)
         d_light = torch.empty((B, 3), device=img.device, dtype=torch.float32) if want_light_grad else None

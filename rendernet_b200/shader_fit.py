@@ -23,6 +23,10 @@ Search (`pose_search`, the reference's loop with `create_param_center`): five po
 `inner_step` descent steps; the loss is re-evaluated after the last one, the argmin kept and the window halved around it for the
 next epoch.  Unlike the reference, the scale is the initial guess's (create_param_center writes 1.0) and is held fixed unless
 `fit_scale`.
+
+Shading (`fit_shading=True`, "phong" only): the light's colour [B,3] and the ambient term [B] join the state, starting from the
+constructor's constants (PHONG_DEFAULTS), descend with their own eta and are projected onto colour >= 0 and 0 <= ambient <= 1
+after every step.  k_diffuse stays a constant: the composite sees only k_diffuse * colour, and the fitted colour absorbs it.
 """
 from __future__ import annotations
 
@@ -42,6 +46,9 @@ OBJECTIVES = ("phong", "mse", "bce")
 # the demo's shading (RenderNet_demo.py:18-20): ambient 0.1, k_diffuse 0.9, white light, black background with the soft mask
 PHONG_DEFAULTS = dict(light_col=(1.0, 1.0, 1.0), ambient=0.1, k_diffuse=0.9, background_white=False, with_mask=True)
 FIT_DEFAULTS = dict(pose_eta=0.01, light_eta=0.4, inner_step=200, max_epochs=10)       # config_reconstruction_RenderNet.json
+# step size of the light colour and the ambient term (fit_shading): not in the reference and not tuned.  The loss is a pixel
+# mean, so its curvature in the ambient term is about twice the masked fraction of the image (up to 2): 0.5 keeps the steps stable
+SHADING_ETA = 0.5
 LIGHT_AZIMUTHS_DEG = np.linspace(230, 320, num=5)                                       # Reconstruct_RenderNet_Face.py:465
 
 
@@ -80,14 +87,15 @@ def shader_fit_gradients(ig, voxels, view_params, target, objective: str, light=
                          ambient: float = PHONG_DEFAULTS["ambient"], k_diffuse: float = PHONG_DEFAULTS["k_diffuse"],
                          background_white: bool = PHONG_DEFAULTS["background_white"],
                          with_mask: bool = PHONG_DEFAULTS["with_mask"], want_dvox: bool = False, want_dpose: bool = True,
-                         dvox_on_device: bool = False):
+                         dvox_on_device: bool = False, want_shading_grad: bool = False):
     """Loss [B] (float64) and the gradients of sum_b loss[b] at (voxels, view_params[, light]).
 
     ig: a backward.ShaderInputGradients of the batch size.  objective "phong" (RGB network only; light [B,2] = (azimuth,
     elevation) radians, required), "mse" or "bce" (raw output; light must be None).  target: [B,512,512,C] image (NumPy or
     tensor).  Returns (loss, {"pose": dL/dview_params [B,3] if want_dpose else None, "light": dL/d(azimuth, elevation) [B,2] or
     None, "voxels": dL/dvoxels [B,64,64,64,1] if want_dvox else None}), NumPy float64 except dL/dvoxels (float32; a CUDA tensor
-    if dvox_on_device)."""
+    if dvox_on_device).  light_col: 1 or B rows of 3; ambient: a float or a [1|B] tensor.  want_shading_grad ("phong"): the
+    dictionary also holds "light_col" [B,3] and "ambient" [B] (rn_phong_composite_loss_grad_params)."""
     check_objective(objective, ig.is_greyscale)
     B = ig.B
     if objective == "phong":
@@ -99,19 +107,26 @@ def shader_fit_gradients(ig, voxels, view_params, target, objective: str, light=
         light = np.broadcast_to(light.reshape(-1, 2), (B, 2))
     elif light is not None:
         raise ValueError(f"objective {objective!r} has no light")
+    if want_shading_grad and objective != "phong":
+        raise ValueError(f"objective {objective!r} has no shading")
     img = ig.forward(voxels, view_params)
     tgt = _target_on(target, img.shape, img.device)
     dlight = None
+    shading = {}
     with torch.cuda.device(img.device):
         if objective == "phong":
             ld = torch.from_numpy(light_dir(light)).to(img.device)
-            loss, dimg, dl = ops.phong_composite_loss_grad(img, tgt, ld, light_col, ambient, k_diffuse, background_white,
-                                                           with_mask)
+            out = ops.phong_composite_loss_grad(img, tgt, ld, light_col, ambient, k_diffuse, background_white, with_mask,
+                                                **(dict(want_shading_grad=True) if want_shading_grad else {}))
+            loss, dimg, dl = out[:3]
             dlight = np.einsum("bi,bij->bj", dl.double().cpu().numpy(), light_dir_jacobian(light))
+            if want_shading_grad:
+                shading = dict(light_col=out[3].double().cpu().numpy(), ambient=out[4].double().cpu().numpy())
         else:
             loss, dimg = ops.image_loss_grad_items(img, tgt, objective)
     dvox, dpose = ig.backward(dimg, want_dvox=want_dvox, want_dpose=want_dpose, dvox_on_device=dvox_on_device)
-    return loss.cpu().numpy(), dict(pose=np.asarray(dpose, np.float64) if want_dpose else None, light=dlight, voxels=dvox)
+    return loss.cpu().numpy(), dict(pose=np.asarray(dpose, np.float64) if want_dpose else None, light=dlight, voxels=dvox,
+                                    **shading)
 
 
 def _deg(x):
@@ -134,7 +149,7 @@ def in_window(pose, window, slack_deg: float = 0.0) -> bool:
 
 
 def pose_search(step_fn: Callable, loss_fn: Callable, target, init_pose, light=None, batch_size: int = 5, max_epochs: int = 10,
-                inner_step: int = 200, callback: Optional[Callable] = None) -> Dict[str, object]:
+                inner_step: int = 200, callback: Optional[Callable] = None, shading: Optional[dict] = None) -> Dict[str, object]:
     """The reference's outer / inner loop (Reconstruct_RenderNet_Face.py:455-537) over the pose and, optionally, the light.
 
     step_fn(state, target) -> (new_state, loss [B], grads): one descent step from `state` {"pose" [B,3] radians, "light" [B,2]
@@ -147,7 +162,8 @@ def pose_search(step_fn: Callable, loss_fn: Callable, target, init_pose, light=N
 
     Returns {"pose" [3], "light" [2] or None (the selected hypothesis), "best_param" (degrees, the reference's form),
     "best_index", "best_loss" (per epoch), "windows" (per epoch: phi_mid, phi_range, theta_mid, theta_range, degrees),
-    "state" (the last state)}."""
+    "state" (the last state)}.  shading: the first epoch's {"light_col" [5,3], "ambient" [5]}, or None; given, they join the state,
+    later epochs restart from the selected hypothesis' values, and the result holds the selected "light_col" [3] and "ambient"."""
     if batch_size != 5:
         raise ValueError(f"the pose search runs 5 hypotheses (create_param_center); batch_size is {batch_size}")
     if int(max_epochs) < 1 or int(inner_step) < 1:
@@ -160,7 +176,7 @@ def pose_search(step_fn: Callable, loss_fn: Callable, target, init_pose, light=N
         light = np.asarray(light, np.float32)
         if light.shape != (batch_size, 2):
             raise ValueError(f"light must be [{batch_size},2] (azimuth, elevation), not {light.shape}")
-    best_light = best_pose = best_index = None
+    best_light = best_pose = best_index = best_shading = None
     best_loss, windows = [], []
     phi_range, theta_range = 60.0, 30.0
     state = None
@@ -176,6 +192,10 @@ def pose_search(step_fn: Callable, loss_fn: Callable, target, init_pose, light=N
         state = dict(pose=params)
         if light is not None:
             state["light"] = light.copy() if i == 0 else np.tile(best_light[np.newaxis, :], (batch_size, 1))
+        if shading is not None:
+            for k in ("light_col", "ambient"):
+                v = np.asarray(shading[k], np.float32) if i == 0 else best_shading[k]
+                state[k] = v.copy() if i == 0 else np.repeat(v[np.newaxis], batch_size, 0)
         for idx in range(int(inner_step)):
             state, loss, _ = step_fn(state, target)
             sel = None
@@ -184,6 +204,8 @@ def pose_search(step_fn: Callable, loss_fn: Callable, target, init_pose, light=N
                 j = int(np.argmin(sel))
                 best_pose = np.asarray(state["pose"][j], np.float32).copy()
                 best_light = None if light is None else np.asarray(state["light"][j], np.float32).copy()
+                if shading is not None:
+                    best_shading = {k: np.asarray(state[k][j], np.float32).copy() for k in ("light_col", "ambient")}
                 w = pose_window(best_pose)
                 best_param = np.array([w["phi"], w["theta"], 1.0])
                 scale = best_pose[2]
@@ -191,8 +213,11 @@ def pose_search(step_fn: Callable, loss_fn: Callable, target, init_pose, light=N
                 best_loss.append(float(sel[j]))
             if callback is not None:
                 callback(i, idx, state, loss, sel)
-    return dict(pose=best_pose, light=best_light, best_param=best_param, best_index=best_index, best_loss=best_loss,
-                windows=windows, state=state)
+    out = dict(pose=best_pose, light=best_light, best_param=best_param, best_index=best_index, best_loss=best_loss,
+               windows=windows, state=state)
+    if shading is not None:
+        out.update(best_shading)
+    return out
 
 
 def weights_are_greyscale(weights) -> Optional[bool]:
@@ -211,7 +236,11 @@ class ShaderPoseFit:
 
     `gradients`, `step` (plain descent, var -= eta * grad in float32 like FaceReconstruction.step), `loss` and `render` work on a
     state {"pose" [5,3], "light" [5,2] ("phong" only)}; `run` is `pose_search` over them.  The voxels ([64,64,64], [1|5,...,1])
-    are held fixed.  is_greyscale: None takes it from the weights' e_conv11 filter (False for seeded weights)."""
+    are held fixed.  is_greyscale: None takes it from the weights' e_conv11 filter (False for seeded weights).
+
+    fit_shading ("phong" only): the state also holds "light_col" [5,3] and "ambient" [5], starting from light_col / ambient;
+    step descends them with shading_eta (SHADING_ETA: untuned) and projects them onto colour >= 0, 0 <= ambient <= 1; run
+    returns the selected hypothesis' values and render shades with the state's."""
 
     def __init__(self, weights, voxels, objective: str = "phong", batch: int = 5, precision: str = "exact",
                  pose_eta: float = FIT_DEFAULTS["pose_eta"], light_eta: float = FIT_DEFAULTS["light_eta"],
@@ -219,7 +248,8 @@ class ShaderPoseFit:
                  fit_scale: bool = False, is_greyscale: Optional[bool] = None, light_col=PHONG_DEFAULTS["light_col"],
                  ambient: float = PHONG_DEFAULTS["ambient"], k_diffuse: float = PHONG_DEFAULTS["k_diffuse"],
                  background_white: bool = PHONG_DEFAULTS["background_white"], with_mask: bool = PHONG_DEFAULTS["with_mask"],
-                 loss_scale=None, seed: int = 0, device: str = "cuda"):
+                 loss_scale=None, seed: int = 0, device: str = "cuda", fit_shading: bool = False,
+                 shading_eta: float = SHADING_ETA):
         if int(batch) != 5:
             raise ValueError(f"the pose search runs 5 hypotheses (create_param_center); batch is {batch}")
         found = weights_are_greyscale(weights)
@@ -228,12 +258,17 @@ class ShaderPoseFit:
         elif found is not None and found != bool(is_greyscale):
             raise ValueError(f"is_greyscale={is_greyscale}, but the weights' e_conv11 filter says {found}")
         check_objective(objective, is_greyscale)
+        if fit_shading and objective != "phong":
+            raise ValueError(f"fit_shading fits the Phong composite's light; objective {objective!r} has none")
         v = np.asarray(voxels, np.float32)
         if v.size not in (64 ** 3, 5 * 64 ** 3):
             raise ValueError(f"voxels must hold one or 5 grids of 64^3, not shape {v.shape}")
         self.voxels = np.ascontiguousarray(np.broadcast_to(v.reshape(-1, 64, 64, 64, 1), (5, 64, 64, 64, 1)))
         self.B, self.objective, self.is_greyscale = 5, objective, bool(is_greyscale)
         self.eta = dict(pose=float(pose_eta), light=float(light_eta))
+        self.fit_shading = bool(fit_shading)
+        if self.fit_shading:
+            self.eta["shading"] = float(shading_eta)
         self.inner_step, self.max_epochs, self.fit_scale = int(inner_step), int(max_epochs), bool(fit_scale)
         self.phong = dict(light_col=light_col, ambient=float(ambient), k_diffuse=float(k_diffuse),
                           background_white=bool(background_white), with_mask=bool(with_mask))
@@ -253,8 +288,27 @@ class ShaderPoseFit:
     def _light(self, state):
         return state["light"] if self.objective == "phong" else None
 
+    def _phong(self, state) -> dict:
+        """The shading arguments at `state`: the constants, or with fit_shading the state's colour and ambient terms."""
+        if not self.fit_shading:
+            return self.phong
+        return dict(self.phong, light_col=np.asarray(state["light_col"], np.float32),
+                    ambient=torch.as_tensor(np.asarray(state["ambient"], np.float32)).to(self.device))
+
+    def initial_shading(self) -> Optional[dict]:
+        """The first epoch's {"light_col" [5,3], "ambient" [5]} (the constructor's constants), or None without fit_shading."""
+        if not self.fit_shading:
+            return None
+        lc = np.asarray(self.phong["light_col"], np.float32).reshape(-1, 3)
+        return dict(light_col=np.ascontiguousarray(np.broadcast_to(lc, (self.B, 3))),
+                    ambient=np.full(self.B, self.phong["ambient"], np.float32))
+
     def gradients(self, state, target):
-        """Loss [B] and dL/d(pose) [B,3], dL/d(light) [B,2] ("phong"; else None) of sum_b loss[b] at `state`."""
+        """Loss [B] and dL/d(pose) [B,3], dL/d(light) [B,2] ("phong"; else None) of sum_b loss[b] at `state`; with fit_shading
+        also dL/d(light_col) [B,3] and dL/d(ambient) [B]."""
+        if self.fit_shading:
+            return shader_fit_gradients(self.ig, self.voxels, state["pose"], self._target_dev(target), self.objective,
+                                        light=self._light(state), want_shading_grad=True, **self._phong(state))
         return shader_fit_gradients(self.ig, self.voxels, state["pose"], self._target_dev(target), self.objective,
                                     light=self._light(state), **(self.phong if self.objective == "phong" else {}))
 
@@ -269,6 +323,12 @@ class ShaderPoseFit:
         if self.objective == "phong":
             new["light"] = (np.asarray(state["light"], np.float32) -
                             np.float32(self.eta["light"]) * np.asarray(grads["light"], np.float32)).astype(np.float32)
+        if self.fit_shading:
+            eta = np.float32(self.eta["shading"])
+            new["light_col"] = np.maximum(np.asarray(state["light_col"], np.float32) -
+                                          eta * np.asarray(grads["light_col"], np.float32), np.float32(0)).astype(np.float32)
+            new["ambient"] = np.clip(np.asarray(state["ambient"], np.float32) - eta * np.asarray(grads["ambient"], np.float32),
+                                     np.float32(0), np.float32(1)).astype(np.float32)
         return new, loss, grads
 
     def loss(self, state, target) -> np.ndarray:
@@ -278,7 +338,7 @@ class ShaderPoseFit:
         with torch.cuda.device(self.device):
             if self.objective == "phong":
                 ld = torch.from_numpy(light_dir(state["light"])).to(self.device)
-                p = self.phong
+                p = self._phong(state)
                 loss = ops.phong_composite_loss_grad(img, tgt, ld, p["light_col"], p["ambient"], p["k_diffuse"],
                                                      p["background_white"], p["with_mask"], want_light_grad=False)[0]
             else:
@@ -292,7 +352,13 @@ class ShaderPoseFit:
         img = self.ig.forward(self.voxels, state["pose"])
         out = dict(image=img)
         with torch.cuda.device(self.device):
-            if self.objective == "phong":
+            if self.objective == "phong" and self.fit_shading:
+                p = self._phong(state)
+                ld = torch.from_numpy(light_dir(state["light"])).to(self.device)
+                out["shaded"], _, out["shaded_u8"] = ops.phong_shade(img, ld, p["light_col"], p["ambient"], p["k_diffuse"],
+                                                                     composite="numpy", background_white=p["background_white"],
+                                                                     with_mask=p["with_mask"])
+            elif self.objective == "phong":
                 p = self.phong
                 ld = torch.from_numpy(light_dir(state["light"])).to(self.device)
                 lc = ops._light_rows(p["light_col"], self.B, img.device, "light_col")
@@ -320,6 +386,10 @@ class ShaderPoseFit:
         reference's first window), "light" or "light_elevation" (see initial_light)}.  Returns pose_search's dictionary."""
         init = dict(init or {})
         pose = np.asarray(init.get("pose", [math.radians(270.0), 0.0, 1.0]), np.float64).reshape(3)
+        if self.fit_shading:
+            return pose_search(self.step, self.loss, target, pose, light=self.initial_light(init), batch_size=self.B,
+                               max_epochs=self.max_epochs, inner_step=self.inner_step, callback=callback,
+                               shading=self.initial_shading())
         return pose_search(self.step, self.loss, target, pose, light=self.initial_light(init), batch_size=self.B,
                            max_epochs=self.max_epochs, inner_step=self.inner_step, callback=callback)
 
@@ -348,6 +418,9 @@ def main(argv=None):
     parser.add_argument('--pose_eta', type=float, default=FIT_DEFAULTS["pose_eta"])
     parser.add_argument('--light_eta', type=float, default=FIT_DEFAULTS["light_eta"])
     parser.add_argument('--fit_scale', action='store_true')
+    parser.add_argument('--fit_shading', action='store_true',
+                        help="Also fit the light colour and the ambient term (objective phong; k_diffuse stays 0.9).")
+    parser.add_argument('--shading_eta', type=float, default=SHADING_ETA, help="Step size of the colour and ambient terms.")
     parser.add_argument('--out_dir', type=str, default="./fit", help="Where the JSON and the PNG of the fit go.")
     args = parser.parse_args(argv)
     from PIL import Image
@@ -360,7 +433,8 @@ def main(argv=None):
     target = np.tile(target.reshape((1, 512, 512, -1)), (5, 1, 1, 1))
     fit = ShaderPoseFit(graph.weights, voxel, objective=args.objective, precision=args.precision, pose_eta=args.pose_eta,
                         light_eta=args.light_eta, inner_step=args.inner_step, max_epochs=args.max_epochs,
-                        fit_scale=args.fit_scale, is_greyscale=graph.is_greyscale)
+                        fit_scale=args.fit_scale, is_greyscale=graph.is_greyscale,
+                        **(dict(fit_shading=True, shading_eta=args.shading_eta) if args.fit_shading else {}))
     init = dict(pose=compute_pose_param(args.azimuth, args.elevation, args.radius)[0],
                 light_elevation=math.radians(args.light_elevation))
     if args.light_azimuth is not None:
@@ -373,6 +447,8 @@ def main(argv=None):
                first_step_loss=[float(v) for v in first[0]], windows=out["windows"])
     if light is not None:
         res.update(light_azimuth=_deg(light[0]) % 360.0, light_elevation=_deg(light[1]), light=[float(v) for v in light])
+    if args.fit_shading:
+        res.update(light_col=[float(v) for v in out["light_col"]], ambient=float(out["ambient"]))
     imgs = fit.render(out["state"])                  # the selected hypothesis is out["best_index"] of the last state
     u8 = (imgs["shaded_u8"] if args.objective == "phong" else imgs["image_u8"])[out["best_index"]][None]
     os.makedirs(args.out_dir, exist_ok=True)
